@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""cbir_eval.py — stand-alone CBIR evaluation on B200 (entry point kept from the reference; new code).
+"""cbir_eval.py — stand-alone CBIR evaluation on H100 (entry point kept from the reference; new code).
 
     python cbir_eval.py [--cfgs configs/faceX/cbir_convnext_b200.yaml] [--weight Epoch_N.pt] [--ema]
                         [--gallery 100000] [--queries 1000] [--k 10]
 
 The reference script (cbir_eval.py) hard-codes its paths, builds a random-init model, extracts gallery and query
 embeddings, builds a faiss Flat/IP index and searches k=10.  This one does the same through visiondk_b200:
-ConvNeXt embeddings on the sm_100a kernels, FlatIPIndex for index/search, everything resident in HBM.  Without a
+ConvNeXt embeddings on the sm_90a kernels, FlatIPIndex for index/search, everything resident in HBM.  Without a
 dataset on disk it evaluates on synthetic images (random tensors: timing / plumbing) — real datasets plug in through
 any iterable of [B,3,S,S] float tensors (the reference's CBIRDatasets + DataLoader yield exactly that).
 """

@@ -1,4 +1,4 @@
-"""CBIR evaluation of the reference (engine/cbir/evaluation.py:106-291) on the B200 kernels — same function names and
+"""CBIR evaluation of the reference (engine/cbir/evaluation.py:106-291) on the H100 kernels — same function names and
 argument meaning: `index`, `search`, `compute_metrics`, `valuate`.
 
 `valuate` (:226-291) = build query / gallery loaders (shuffle=False) -> FeatureExtractor -> index(gallery) -> search(queries,

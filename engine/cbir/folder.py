@@ -3,7 +3,7 @@
     <root>/query/<identity>/*.jpg|png        <root>/gallery/<identity>/*.jpg|png        (query identities must be a subset)
 
 read the way the reference reads it (`Image.open(path).convert('RGB')`, cv2 fallback: basedataset.py:234-241) and fed to the
-B200 path: decoded RGB bytes -> visiondk_b200.preprocess (the val transform list on the device, bit-exact with the reference's
+H100 path: decoded RGB bytes -> visiondk_b200.preprocess (the val transform list on the device, bit-exact with the reference's
 PIL / torchvision pipeline) -> embed -> index -> search.  Decoding stays on host threads (`nw`), one batch ahead of the device.
 
 Only the deterministic eval list of the reference's configs is built — `resize_and_padding(size, training=False)` ->

@@ -1,8 +1,8 @@
-"""Face pair verification of the reference (engine/faceX/evaluation.py:8-140) on the B200 kernels — same names and argument
+"""Face pair verification of the reference (engine/faceX/evaluation.py:8-140) on the H100 kernels — same names and argument
 meaning: `process_pairtxt`, `Evaluator.test / test_one_model`, `valuate(model, data_cfg, device) -> (mean, std)`.
 
 `valuate` = parse `data.val.pair_txt` (rows "<img a> <img b> <0|1>", images under <root>/val/) -> embed every distinct image once
-(FeatureExtractor.extract_face: host decode, device val transforms, B200 backbone, L2-normalised) -> cosine score per pair ->
+(FeatureExtractor.extract_face: host decode, device val transforms, H100 backbone, L2-normalised) -> cosine score per pair ->
 10-fold LFW protocol (threshold chosen on nine folds, accuracy on the tenth): visiondk_b200.metrics.face_verification_accuracy,
 pinned to the reference's Evaluator by tests/golden/face_verification.npz.  Pair scores are one gather + row-wise dot on the
 device instead of the reference's per-pair Python loop over a dict.  With a synthetic:// root the pairs are drawn from the

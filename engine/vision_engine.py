@@ -1,4 +1,4 @@
-"""Orchestrator of the faceX / CBIR embedding path on B200 — the surface of the reference's
+"""Orchestrator of the faceX / CBIR embedding path on H100 — the surface of the reference's
 engine/vision_engine.py (yaml_load :35-38, increment_path :41-57, CenterProcessor.__init__ :67-167,
 run_embedding :438-560) over the visiondk_b200 kernels.  Written from scratch: model / step / eval come from
 visiondk_b200.{train,cbir} and engine.cbir.evaluation; the dataset layer is out of the hot-path scope, so `data.root`
@@ -84,7 +84,7 @@ def check(task: str, cfgs: dict) -> None:
         num_classes = len([x for x in os.listdir(train_dir) if not (x.startswith(".") or x.startswith("_"))])
     else:
         raise ValueError(f"Dataset loading error: {root} is neither a synthetic:// URL nor a local directory "
-                         "(HuggingFace hub datasets need a network, which the B200 box does not have)")
+                         "(HuggingFace hub datasets need a network, which the GPU hosts may not have)")
     model_classes = head["num_class"]
     assert model_classes == num_classes, \
         f"Model configuration error: Number of classes mismatch. Expected {num_classes} from dataset, but got {model_classes} in model configuration"
@@ -96,21 +96,21 @@ class CenterProcessor:
         self.model_cfg, self.data_cfg, self.hyp_cfg = cfgs["model"], cfgs["data"], cfgs["hyp"]
         self.task = self.model_cfg["task"]
         if self.task not in ("face", "cbir"):
-            raise ValueError("only the faceX / cbir embedding tasks are built for B200")
+            raise ValueError("only the faceX / cbir embedding tasks are built for H100")
         if not torch.cuda.is_available():
-            raise RuntimeError("visiondk_b200 needs a CUDA (sm_100a) device; there is no CPU path")
+            raise RuntimeError("visiondk_b200 needs a CUDA (sm_90a) device; there is no CPU path")
         self.device = torch.device("cuda", max(rank, 0))
         torch.cuda.set_device(self.device)
         self.world = int(os.environ.get("WORLD_SIZE", "1")) if rank != -1 else 1
         if getattr(opt, "sync_bn", False) and self.world > 1:
-            # main.py:57-60 -> vision_engine.py:224-225 converts the neck's two BatchNorms to SyncBatchNorm.  The B200 neck
+            # main.py:57-60 -> vision_engine.py:224-225 converts the neck's two BatchNorms to SyncBatchNorm.  The H100 neck
             # kernels normalise with the LOCAL batch statistics; silently ignoring the flag would train a different model.
             raise NotImplementedError("--sync_bn with WORLD_SIZE > 1: cross-rank BatchNorm statistics are not built for the "
-                                      "B200 neck kernels (they use per-rank batch statistics); drop the flag")
+                                      "H100 neck kernels (they use per-rank batch statistics); drop the flag")
         self.model = FaceTrainingModel(self.model_cfg).to(self.device)
         root = str(self.data_cfg["root"])
         if not is_synthetic(root):
-            raise NotImplementedError("dataset loading is outside the B200 hot-path scope: use a synthetic:// root or drive "
+            raise NotImplementedError("dataset loading is outside the H100 hot-path scope: use a synthetic:// root or drive "
                                       "FaceTrainer / engine.cbir.evaluation with your own (images, labels) iterables")
         self.data = SyntheticFaceData(root, self.model_cfg["image_size"], self.data_cfg["train"]["bs"], self.device,
                                       max(rank, 0), self.world)
@@ -153,7 +153,7 @@ class CenterProcessor:
         steps_per_epoch = len(self.data)
         name, layer_wise = hyp["optimizer"][0], bool(hyp["optimizer"][1])
         if name != "sgd" or hyp["scheduler"] != "cosine_with_warm":
-            raise NotImplementedError("the B200 step implements sgd + cosine_with_warm (the faceX / cbir configs)")
+            raise NotImplementedError("the H100 step implements sgd + cosine_with_warm (the faceX / cbir configs)")
         if self.model_cfg.get("load_from"):
             self._load_from(self.model_cfg["load_from"])
         trainer = FaceTrainer(self.model, lr0=hyp["lr0"], momentum=hyp["warmup_momentum"], weight_decay=hyp["weight_decay"],

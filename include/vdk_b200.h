@@ -1,4 +1,4 @@
-/* vdk_b200.h — C ABI of libvdk_b200.so, the sm_100a implementation of DORAEMON's (wuji3/visiondk)
+/* vdk_b200.h — C ABI of libvdk_b200.so, the sm_90a implementation of DORAEMON's (wuji3/visiondk)
  * embedding hot path.  The reference is pure Python and has no FFI of its own (SURVEY.md §8b); each
  * entry point below names the reference call site (file:line under /root/reference) whose arithmetic
  * it replaces.  A maintainer binds these with ctypes (INTEGRATION.md shows the stubs).
@@ -36,7 +36,7 @@ int vdk_device_check(void);
 /* Replaces the cuBLAS/cuDNN GEMMs inside timm's ConvNeXt/ViT blocks that models/faceX/backbone/
  * timm_wrapper.py:52 runs (pointwise Linear layers, patchify convs as GEMMs) and the neck Linear
  * (timm_wrapper.py:36).  A is [M,K] row-major (pitch lda), B is [N,K] row-major (pitch ldb) — the
- * layout of nn.Linear.weight — both 16-bit (bf16 or fp16); accumulation is fp32 on tcgen05/TMEM. */
+ * layout of nn.Linear.weight — both 16-bit (bf16 or fp16); accumulation is fp32 on wgmma (register accumulators). */
 #define VDK_DTYPE_BF16 0
 #define VDK_DTYPE_FP16 1
 #define VDK_DTYPE_FP32 2
@@ -318,7 +318,7 @@ int vdk_attention_bwd(const void* qkv, const void* out, const void* d_out, const
 /* Replaces ArcFace.forward (models/faceX/head/arcface.py:20-36), CircleLoss.forward (models/faceX/head/
  * circleloss.py:21-43), nn.CrossEntropyLoss(label_smoothing) (models/losses/loss.py:71-73) and their autograd
  * backward, as called at engine/procedure/train.py:196.  fp32 in / fp32 out like the reference (no autocast on the
- * face path); the three contractions run on tcgen05 with a 3-way bf16 operand split (fp32-grade accuracy). */
+ * face path); the three contractions run on wgmma with a 3-way bf16 operand split (fp32-grade accuracy). */
 #define VDK_HEAD_ARCFACE 0
 #define VDK_HEAD_CIRCLELOSS 1
 #define VDK_HEAD_MV_SOFTMAX 2 /* MV_Softmax.forward, models/faceX/head/mv_softmax.py:25-44 */
@@ -508,7 +508,7 @@ int vdk_preprocess_resize_pad_normalize(const uint8_t* packed, const vdk_image_d
 /* Live kernel timing inside a real step (bench.py's roofline legs; not part of the reference's surface).  Between
  * vdk_prof_begin() and vdk_prof_end() every launch of the categories below is bracketed by two CUDA events on the stream it
  * is launched on; vdk_prof_end synchronises on them and returns, per category, the launch count, the summed event time and
- * the summed ALGORITHMIC flops / bytes of those launches.  Categories: 0 tcgen05 GEMM (vdk_gemm and every internal GEMM),
+ * the summed ALGORITHMIC flops / bytes of those launches.  Categories: 0 wgmma GEMM (vdk_gemm and every internal GEMM),
  * 1 depthwise 7x7 (forward+LN, data gradient, weight gradient), 2 attention (forward, backward), 3 retrieval score/filter,
  * 4 other.  Profiling perturbs the step (two event records per launch): never time a step with a profile open. */
 typedef struct vdk_prof_total {

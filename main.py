@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """main.py — train entry point (reference flags: --cfgs --resume --sync_bn --project --name --local_rank --print_freq
 --save_freq; env LOCAL_RANK / WORLD_SIZE from torchrun).  New code: dispatches the faceX / cbir embedding task to
-engine.vision_engine.CenterProcessor.run_embedding on the B200 kernels.
+engine.vision_engine.CenterProcessor.run_embedding on the H100 kernels.
 
     python main.py --cfgs configs/faceX/cbir_convnext_b200.yaml
     torchrun --nproc_per_node 8 --master-addr 127.0.0.1 main.py --cfgs configs/faceX/cbir_convnext_b200.yaml

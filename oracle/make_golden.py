@@ -1,6 +1,6 @@
 """Generates tests/golden/*.npz by executing the REFERENCE's own modules (authoring container only).
 
-    python oracle/make_golden.py            # needs /root/reference; never runs on the GPU box
+    python oracle/make_golden.py            # needs the reference tree; never runs on the GPU
 
 The reference package cannot be imported as a whole (timm / faiss / torchmetrics are not installed), so the
 torch-only files are loaded by path: models/faceX/head/{arcface,circleloss}.py, models/losses/loss.py,

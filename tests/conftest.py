@@ -8,15 +8,15 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
-# GPU tests written after the round's GPU budget was spent have never executed on a B200.  They are recorded as non-strict
+# GPU tests written after the round's GPU budget was spent have never executed on an H100.  They are recorded as non-strict
 # xfail so that an unvalidated TEST cannot turn a validated suite red: "xpassed" in a GPU run means the test ran and held,
 # "xfailed" means the new test (or what it checks) needs attention.  The mark is removed once a GPU run has shown XPASS.
-not_yet_run_on_gpu = pytest.mark.xfail(reason="added after the round's GPU budget was spent: never executed on a B200 "
+not_yet_run_on_gpu = pytest.mark.xfail(reason="added after the round's GPU budget was spent: never executed on an H100 "
                                               "(XPASS = validated)", strict=False)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100a) GPU; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU; run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):

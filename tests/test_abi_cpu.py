@@ -1,4 +1,4 @@
-"""CPU-side checks of the C-ABI boundary: the library builds for sm_100a, loads without a GPU, exports every
+"""CPU-side checks of the C-ABI boundary: the library builds for sm_90a, loads without a GPU, exports every
 symbol include/vdk_b200.h declares, and its host-only entry points (plans, argument validation) behave."""
 import ctypes as C
 import re
@@ -27,11 +27,11 @@ def test_library_builds_and_exports_every_declared_symbol(lib):
     assert sorted(_lib.SIGNATURES) == names
 
 
-def test_library_is_sm100a_only(lib):
+def test_library_is_sm90a_only(lib):
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", str(_lib.lib_path())], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_version_and_error_string(lib):

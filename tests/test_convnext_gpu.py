@@ -1,4 +1,4 @@
-"""GPU parity of the ConvNeXt embedding forward (csrc/convnext.cu + tcgen05 GEMM epilogues) against the fp32
+"""GPU parity of the ConvNeXt embedding forward (csrc/convnext.cu + wgmma GEMM epilogues) against the fp32
 oracle (oracle/convnext.py, timm 0.9.16 restatement).
 
 Tolerance (stated, floating point): the CUDA path keeps activations in bf16 between kernels (fp32 accumulation

@@ -186,9 +186,9 @@ def test_train_forward_backward_matches_oracle_autograd(lib):
 
 def test_convnext_base_224_training_gradients_match_oracle(lib):
     """Full-size ConvNeXt-B 224^2 (BASELINE configs[1] backbone), batch 3: the shapes that select the clustered depthwise
-    kernel with 1/2/4/8 chunks, the CTA-pair and auxiliary-epilogue GEMMs, the 14x14 / 7x7 weight-gradient tiles.  Every
+    kernel with 1/2/4/8 chunks, the wide and narrow GEMM tiles with every epilogue, the 14x14 / 7x7 weight-gradient tiles.  Every
     parameter gradient is compared with fp32 autograd of the oracle.  Tolerance: bf16 activations through 36 blocks of
-    forward and backward against fp32 (measured: rel L2 0.03-0.11, cosine >= 0.994 at batch 3) -> rel <= 0.15, cos >= 0.99."""
+    forward and backward against fp32 -> rel <= 0.15, cos >= 0.99."""
     torch.set_num_threads(min(16, torch.get_num_threads()))
     oracle = randomize_(TimmWrapperOracle("convnext_base", 512, 224), seed=3).train()
     ours = TimmWrapper("convnext_base", 512, 224, pretrained=False)
@@ -249,7 +249,7 @@ def test_backward_in_unit_ranges_equals_single_call(lib):
 
 
 def test_train_step_with_head_and_fused_optimizer(lib):
-    """One full faceX train step on the B200 kernels: backbone fwd -> ArcFace+CE -> backward -> clip+SGD+EMA."""
+    """One full faceX train step on the H100 kernels: backbone fwd -> ArcFace+CE -> backward -> clip+SGD+EMA."""
     import copy
     from visiondk_b200.heads import ArcFace, margin_ce_loss
     from visiondk_b200.optim import FusedSGDClipEMA

@@ -156,8 +156,8 @@ def test_resume_restores_optimizer_scheduler_ema_and_head(lib, tmp_path):
 
     def close(a, b, what):
         err = (a.float() - b.float()).norm().item() / (b.float().norm().item() + 1e-12)
-        # same kernels, same batches: run-to-run differences come from the summation order of atomics (measured up to 2e-3 on
-        # the small bias vectors after 8 steps).  Parameters whose exact gradient is 0 (head.norm.* in front of a
+        # same kernels, same batches: run-to-run differences come from the summation order of atomics (largest on the
+        # small bias vectors after 8 steps).  Parameters whose exact gradient is 0 (head.norm.* in front of a
         # batch-statistics BatchNorm) only ever move by rounding noise: for them the absolute difference is what is bounded.
         assert err <= 1e-2 or (a.float() - b.float()).abs().max().item() <= 5e-4, (what, err)
 

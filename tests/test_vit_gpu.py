@@ -173,9 +173,8 @@ def test_vit_toy_training_gradients_match_oracle_autograd(lib):
 
 def test_vit_base_patch16_224_training_gradients_match_oracle(lib):
     """BASELINE config 3 backbone at full size (ViT-B/16 224^2, 12 blocks, 197 tokens), batch 8 (BatchNorm1d on batch statistics
-    is ill-conditioned for 3 samples: the same kernels measured rel 0.2 there): every parameter gradient vs fp32 autograd of the
-    oracle (bf16 activations: weight matrices rel <= 0.15, cos >= 0.99; 1-D parameters rel <= 0.25, cos >= 0.97: measured worst
-    0.186 / 0.983 on model.norm.bias)."""
+    is ill-conditioned for 3 samples): every parameter gradient vs fp32 autograd of the oracle (bf16 activations: weight
+    matrices rel <= 0.15, cos >= 0.99; 1-D parameters, model.norm.bias the worst of them, rel <= 0.25, cos >= 0.97)."""
     torch.set_num_threads(min(16, torch.get_num_threads()))
     oracle = randomize_(ViTWrapperOracle("vit_base_patch16_224", 512, 224), seed=5).train()
     ours = ViTWrapper("vit_base_patch16_224", 512, 224, pretrained=False)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""A W-way sharded search of the bench's gallery emulated on ONE B200 (W shards, one host thread each, the collectives replaced by
+"""A W-way sharded search of the bench's gallery emulated on ONE H100 (W shards, one host thread each, the collectives replaced by
 barriers — visiondk_b200.sharding.LocalShardGroup): checks the protocol against the unsharded search and prints the device time
 of ONE shard's share of the work (total / W) for the exchange variants and range schedules.  What it cannot see: the NCCL
 latency of the 2-3 small all-gathers and the 8 MB-per-rank list gather (measured by bench.py --gpus N).

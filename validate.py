@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """validate.py — eval entry point (reference flags --cfgs --weight --ema --eval_topk): loads a checkpoint written by the
-trainer (keys 'state_dict' / 'ema', models/faceX/face_model.py:73-86) into the B200 backbone and runs the CBIR evaluation
+trainer (keys 'state_dict' / 'ema', models/faceX/face_model.py:73-86) into the H100 backbone and runs the CBIR evaluation
 (engine/cbir/evaluation.py::valuate: extract -> index -> search -> MRR / Recall / Precision / AUC / nDCG at the config's
 cutoffs), printing the metrics dict like the reference's validate.py:69-75; the face task runs the 10-fold pair verification
 (engine/faceX/evaluation.py::valuate -> mean accuracy, standard error: validate.py:61-66).  New code over visiondk_b200."""
@@ -30,7 +30,7 @@ def main(opt):
     cfgs = yaml_load(opt.cfgs)
     task = cfgs["model"]["task"]
     if task not in ("face", "cbir"):
-        raise ValueError(f"Unknown task {task}")  # validate.py:77 (the classification task is not a B200 path)
+        raise ValueError(f"Unknown task {task}")  # validate.py:77 (the classification task is not an H100 path)
     check(task, cfgs)
     device = torch.device("cuda", int(os.getenv("LOCAL_RANK", 0)))
     model = BackboneFactory(cfgs["model"]["backbone"]).get_backbone()

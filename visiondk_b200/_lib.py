@@ -2,7 +2,7 @@
 
 There is no CPU fallback anywhere in this package: if the library is missing it must be built
 (`python -m visiondk_b200.build`), and every compute entry point raises RuntimeError when the C ABI
-returns a non-zero status (e.g. no sm_100 device).
+returns a non-zero status (e.g. no sm_90 device).
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Backbone seam of the faceX / CBIR path on B200 (SURVEY.md §8b, Seam 1).
+"""Backbone seam of the faceX / CBIR path on H100 (SURVEY.md §8b, Seam 1).
 
 The reference builds `TimmWrapper(model_name, feat_dim, image_size, pretrained)` in
 models/faceX/backbone/backbone_def.py:16-26 (config key `timm-<name>`), i.e. a timm backbone created with
@@ -8,7 +8,7 @@ state_dict prefixes `model.` / `output_layer.`.
 
 This module keeps exactly that surface (constructor arguments, parameter names and shapes — timm 0.9.16
 ConvNeXt checkpoints and the reference's Epoch_N.pt `state_dict` / `ema` entries load with strict=True) but the
-arithmetic is the hand-written sm_100a path: vdk_convnext_forward in csrc/convnext.cu (tcgen05 GEMMs with fused
+arithmetic is the hand-written sm_90a path: vdk_convnext_forward in csrc/convnext.cu (wgmma GEMMs with fused
 LayerNorm / GELU / layer-scale+residual epilogues, NHWC bf16 activations).  The nn.Module children below are
 parameter containers only; their own forward() is never used on the hot path, and there is no CPU fallback.
 """
@@ -138,7 +138,7 @@ class TimmWrapper(nn.Module):
         super().__init__()
         if depths is None:
             if model_name not in CONVNEXT_ARCHS:
-                raise ValueError(f"backbone '{model_name}' is not built for B200 yet; available: {sorted(CONVNEXT_ARCHS)}")
+                raise ValueError(f"backbone '{model_name}' is not built for H100 yet; available: {sorted(CONVNEXT_ARCHS)}")
             depths, dims = CONVNEXT_ARCHS[model_name]
         if image_size % 32 != 0:
             raise ValueError("image_size must be a multiple of 32")
@@ -160,13 +160,13 @@ class TimmWrapper(nn.Module):
             return _ConvNeXtTrainFn.apply(self, x, *self._ordered_params())
         return self.embed(x, l2_normalize=False)
 
-    # ---- B200 path -------------------------------------------------------------------------------
+    # ---- H100 path -------------------------------------------------------------------------------
     @torch.no_grad()
     def embed(self, x: torch.Tensor, l2_normalize: bool = False) -> torch.Tensor:
         """[B,3,S,S] fp32 (NCHW, already normalised like the reference's transforms) -> fp32 [B, feat_dim]."""
         lib = _lib.load()
         if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.TimmWrapper runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200.TimmWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
         if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
             raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
         x = x.contiguous().float()
@@ -265,7 +265,7 @@ class TimmWrapper(nn.Module):
     def _train_forward(self, x: torch.Tensor) -> torch.Tensor:
         lib = _lib.load()
         if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.TimmWrapper runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200.TimmWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
         x = x.contiguous().float()
         B = x.shape[0]
         st, net, params = self._train_structs(x.device)

@@ -1,8 +1,8 @@
-"""Builds libvdk_b200.so (the sm_100a C-ABI library) in-tree with nvcc.
+"""Builds libvdk_b200.so (the sm_90a C-ABI library) in-tree with nvcc.
 
     python -m visiondk_b200.build [--force]
 
-The library is compiled for sm_100a only (-gencode arch=compute_100a,code=sm_100a); nvcc cross-compiles
+The library is compiled for sm_90a only (-gencode arch=compute_90a,code=sm_90a); nvcc cross-compiles
 without a GPU.  Objects are rebuilt when a source or header is newer than the object.
 """
 from __future__ import annotations
@@ -21,7 +21,7 @@ LIB = LIBDIR / "libvdk_b200.so"
 INCLUDE = PKG.parent / "include"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -72,7 +72,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
                 if verbose and out:
                     print(out, file=sys.stderr)
     if jobs or not LIB.exists():
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB), *map(str, objs)]
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB), *map(str, objs)]
         run(cmd)
     return LIB
 

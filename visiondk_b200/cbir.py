@@ -1,10 +1,10 @@
-"""CBIR eval path on B200: extract -> index -> search (SURVEY.md §8b, Seams 5 and 6).
+"""CBIR eval path on H100: extract -> index -> search (SURVEY.md §8b, Seams 5 and 6).
 
 Mirrors, by name and argument meaning:
   FeatureExtractor.extract_cbir   models/faceX/face_model.py:120-144   (.extract_face :93-118)
   index(...)                      engine/cbir/evaluation.py:106-169   (cbir_eval.py:35-96)
   search(...)                     engine/cbir/evaluation.py:171-200   (cbir_eval.py:98-122)
-with the arithmetic on the sm_100a kernels: the backbone's `embed()` fuses F.normalize into the neck epilogue,
+with the arithmetic on the sm_90a kernels: the backbone's `embed()` fuses F.normalize into the neck epilogue,
 embeddings stay in HBM between extraction and search (the reference copies every batch to the host,
 face_model.py:140), and the faiss objects are replaced by visiondk_b200.retrieval.FlatIPIndex.
 """
@@ -65,7 +65,7 @@ class FeatureExtractor:
         """Device-resident fp32 [N, feat_dim], rows L2-normalised, dataloader order preserved."""
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("visiondk_b200 extraction runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200 extraction runs on CUDA (sm_90a) only; there is no CPU fallback")
         model = self.model
         model.eval()
         model.to(device)
@@ -83,7 +83,7 @@ class FeatureExtractor:
         `image_name2feature` dict the face evaluator (engine/faceX/evaluation.py:34-113) looks pairs up in."""
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("visiondk_b200 extraction runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200 extraction runs on CUDA (sm_90a) only; there is no CPU fallback")
         model = self.model
         model.eval()
         model.to(device)
@@ -102,7 +102,7 @@ class FeatureExtractor:
         memory asynchronously (the reference blocks on `.cpu().numpy()` per batch, face_model.py:140)."""
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("visiondk_b200 extraction runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200 extraction runs on CUDA (sm_90a) only; there is no CPU fallback")
         model = self.model
         model.eval()
         model.to(device)

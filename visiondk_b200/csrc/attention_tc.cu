@@ -1,4 +1,4 @@
-// attention_tc.cu — softmax(Q K^T / sqrt(d)) V on the 5th-generation tensor cores (tcgen05), head_dim 64, bf16.
+// attention_tc.cu — softmax(Q K^T / sqrt(d)) V on the sm_90a warpgroup tensor cores (wgmma), head_dim 64, bf16.
 //
 // Replaces timm's Attention.forward inside every ViT block of the reference's backbone
 // (models/faceX/backbone/timm_wrapper.py:52 -> timm VisionTransformer blocks; SURVEY.md §2.4 K4): scores are never
@@ -6,22 +6,16 @@
 // (+ optionally the log2-domain log-sum-exp per row, which the training backward consumes).
 //
 // CTAs are PERSISTENT (one per SM); an item = one (image, head) x TWO 128-query tiles (ViT-B/16's 197 tokens are exactly two),
-// items strided over the grid.  320 threads:
-//   warps 0-3   softmax group of query tile 0 (TMEM lane = query row: one thread owns one row, no shuffles)
-//   warps 4-7   softmax group of query tile 1
-//   warp  8     TMA producer: Q tile pair once per item (double-buffered: the next item's Q lands during this item), K/V tiles (64 keys) through a
-//               four-deep mbarrier ring
-//   warp  9     tcgen05.mma issuer: S_t = Q_t K_j^T (128x64x64, both operands K-major) into TMEM, O_t += P_t V_j (128x64x64:
-//               P from shared memory, written by the softmax group in the swizzle-128B K-major layout; V as stored =
-//               MN-major operand)
-// TMEM: S_0, S_1, O_0, O_1, 64 fp32 columns each.  A group pulls its 64 scores per row into registers with two
-// `tcgen05.ld.32x32b.x32`, hands S_t back at once (s_free) — so the tensor core computes S_t of the NEXT key tile while the
-// group exponentiates this one — and double-buffers P_t, so P V of tile j runs under the softmax of tile j+1.  History
-// (`profiles/r02_attention.md`): one CTA per item 152 TFLOP/s; persistent 198; 128-key tiles with S read twice 210; this 64-key
-// pipeline removes the S -> softmax -> P V -> S round trip from every tile's critical path.
+// items strided over the grid.  288 threads:
+//   warpgroup 0 (warps 0-3)   query tile 0: S = Q K^T (two wgmma m64 x 64 x 64, Q and K K-major) into registers, the
+//                             softmax on the accumulator fragments (a row lives in one quad of threads), then
+//                             O += P V with P taken straight from registers (bf16) and V as stored (MN-major operand)
+//   warpgroup 1 (warps 4-7)   query tile 1
+//   warp 8                    TMA producer: Q tile pair once per item (double-buffered: the next item's Q lands during this
+//                             item), K/V tiles (64 keys) through a four-deep mbarrier ring shared by both warpgroups
 // Softmax is the online recurrence in the log2 domain with a LAZY rescale: the running reference maximum only moves (and
-// O / l are only rescaled, TMEM -> registers -> TMEM) when a row's maximum grows by more than 2^8; P = exp2(s - m_ref) then
-// stays below 256, exact in bf16's range, and the final O / l cancels the stale reference.
+// O / l are only rescaled) when a row's maximum grows by more than 2^8; P = exp2(s - m_ref) then stays below 256, exact in
+// bf16's range, and the final O / l cancels the stale reference.
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
 
@@ -31,15 +25,14 @@
 namespace vdk {
 
 constexpr int kAtD = 64;          // head dim
-constexpr int kAtQM = 128;        // query rows per tile (TMEM lanes)
+constexpr int kAtQM = 128;        // query rows per tile (two m64 halves)
 constexpr int kAtKV = 64;         // keys per tile
 constexpr int kAtStages = 4;      // K/V ring (16 KB per stage)
-constexpr int kAtThreads = 320;
-constexpr int kAtQTile = kAtQM * kAtD * 2;   // 16 KB: a 128 x 64 bf16 tile (Q, P)
+constexpr int kAtThreads = 288;
+constexpr int kAtQTile = kAtQM * kAtD * 2;   // 16 KB: a 128 x 64 bf16 Q tile
 constexpr int kAtKTile = kAtKV * kAtD * 2;   // 8 KB: a 64 x 64 bf16 tile (K, V)
-constexpr int kAtSmem = 2 * 2 * kAtQTile + kAtStages * 2 * kAtKTile + 2 * 2 * kAtQTile + 32 * 8 + 16 + 1024;  // Q double-buffered
+constexpr int kAtSmem = 2 * 2 * kAtQTile + kAtStages * 2 * kAtKTile + 16 * 8 + 1024;  // Q double-buffered
 static_assert(kAtSmem <= 227 * 1024, "attention shared memory budget");
-constexpr uint32_t kAtTmemCols = 256;  // S_0, S_1 (64 fp32 columns each), O_0, O_1 (64 each)
 
 struct AttParams {
   int B, N, H;
@@ -54,16 +47,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {  // 3-input FMNMX3 (sm_100)
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {  // add.rn.f32x2: two row-sum accumulations per instruction
-  unsigned long long ra = *reinterpret_cast<unsigned long long*>(&a), rb = *reinterpret_cast<unsigned long long*>(&b), rd;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  return *reinterpret_cast<float2*>(&rd);
-}
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
@@ -76,16 +59,10 @@ attention_fwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_
   uint8_t* smem = att_smem_raw + ((1024u - (smem_u32(att_smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_q = smem;                                     // [2 items in flight][2 tiles][16 KB]
   uint8_t* smem_kv = smem + 2 * 2 * kAtQTile;                 // [stages][K 8 KB | V 8 KB]
-  uint8_t* smem_p = smem_kv + kAtStages * 2 * kAtKTile;       // [2 groups][2 buffers][16 KB]
-  uint64_t* q_full = reinterpret_cast<uint64_t*>(smem_p + 2 * 2 * kAtQTile);  // [2]
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(smem_kv + kAtStages * 2 * kAtKTile);  // [2]
   uint64_t* q_empty = q_full + 2;            // [2]
   uint64_t* kv_full = q_empty + 2;           // [stages]
   uint64_t* kv_empty = kv_full + kAtStages;  // [stages]
-  uint64_t* s_full = kv_empty + kAtStages;   // [2]      S_t is in TMEM
-  uint64_t* s_free = s_full + 2;             // [2]      the group holds S_t in registers: TMEM may be overwritten
-  uint64_t* p_full = s_free + 2;             // [2][2]   P_t[buffer] is in shared memory
-  uint64_t* p_empty = p_full + 4;            // [2][2]   the P V that read P_t[buffer] has retired
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(p_empty + 4);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int J = p.n_kvtiles, N = p.N;
@@ -97,27 +74,15 @@ attention_fwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_
     prefetch_tensormap(&map_kv);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&q_full[i], 1);
-      mbar_init(&q_empty[i], 1);
+      mbar_init(&q_empty[i], 8);  // one arrival per warp of both warpgroups
     }
     for (int i = 0; i < kAtStages; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 4);  // one arrival per warp of the group
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&p_full[i], 4);
-      mbar_init(&p_empty[i], 1);
+      mbar_init(&kv_empty[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 9) tmem_alloc<kAtTmemCols>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   auto decode = [&](int item, int& pair, int& h, int& b) {
     pair = item % n_pairs;
@@ -135,225 +100,169 @@ attention_fwd_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_
         decode(item, pair, h, b);
         const int qt0 = pair * 2, n_t = min(2, p.n_qtiles - qt0);
         const int qb = qc & 1;  // Q is double-buffered: the next item's tiles land while this item is still in its softmax
-        if (qc >= 2) mbar_wait_relaxed(&q_empty[qb], ((qc >> 1) - 1) & 1);  // every S = Q K^T of the item two back has retired
+        if (qc >= 2) mbar_wait_relaxed<true>(&q_empty[qb], ((qc >> 1) - 1) & 1);  // every S = Q K^T of the item two back has retired
         mbar_arrive_expect_tx(&q_full[qb], n_t * kAtQTile);
         for (int t = 0; t < n_t; ++t)
           tma_load_3d(smem_q + (qb * 2 + t) * kAtQTile, &map_q, &q_full[qb], h * kAtD, (qt0 + t) * kAtQM, b);
         for (int j = 0; j < J; ++j, ++kvc) {
           const int st = kvc % kAtStages;
-          if (kvc >= kAtStages) mbar_wait_relaxed(&kv_empty[st], ((kvc / kAtStages) - 1) & 1);
+          if (kvc >= kAtStages) mbar_wait_relaxed<true>(&kv_empty[st], ((kvc / kAtStages) - 1) & 1);
           mbar_arrive_expect_tx(&kv_full[st], 2 * kAtKTile);
           tma_load_3d(smem_kv + st * 2 * kAtKTile, &map_kv, &kv_full[st], (p.H + h) * kAtD, j * kAtKV, b);
           tma_load_3d(smem_kv + st * 2 * kAtKTile + kAtKTile, &map_kv, &kv_full[st], (2 * p.H + h) * kAtD, j * kAtKV, b);
         }
       }
     }
-  } else if (warp == 9) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_f16<true>(kAtQM, kAtKV);        // Q, K both K-major
-      constexpr uint32_t idesc_o = umma_idesc_f16<true>(kAtQM, kAtD, 0u, 1u);  // P K-major, V MN-major (d contiguous)
-      int qc = 0, kvc = 0;
-      int sg[2] = {0, 0};  // S tiles issued per group (phases of s_full / s_free)
-      int pg[2] = {0, 0};  // P V issued per group (buffer = pg & 1, phase = pg >> 1)
-      auto issue_s = [&](int t, int stage) {
-        const uint64_t da = umma_desc_k_sw128(smem_u32(smem_q + ((qc & 1) * 2 + t) * kAtQTile));
-        const uint64_t db = umma_desc_k_sw128(smem_u32(smem_kv + stage * 2 * kAtKTile));
-        const uint32_t d = tmem_base + t * kAtKV;
-#pragma unroll
-        for (int k = 0; k < kAtD / 16; ++k) umma_f16_ss(d, da + 2 * k, db + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(&s_full[t]);
-        ++sg[t];
-      };
-      auto issue_pv = [&](int t, int stage, bool first) {
-        const int buf = pg[t] & 1;
-        const uint64_t da = umma_desc_k_sw128(smem_u32(smem_p + (t * 2 + buf) * kAtQTile));
-        const uint64_t db = umma_desc_mn_sw128(smem_u32(smem_kv + stage * 2 * kAtKTile + kAtKTile), 8192);
-        const uint32_t d = tmem_base + 2 * kAtKV + t * kAtD;
-#pragma unroll
-        for (int k = 0; k < kAtKV / 16; ++k) umma_f16_ss(d, da + 2 * k, db + 128u * k, idesc_o, (!first || k > 0) ? 1u : 0u);
-        umma_commit(&p_empty[t * 2 + buf]);
-        ++pg[t];
-      };
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++qc) {
-        int pair, h, b;
-        decode(item, pair, h, b);
-        const int n_t = min(2, p.n_qtiles - pair * 2);
-        mbar_wait(&q_full[qc & 1], (qc >> 1) & 1);
-        mbar_wait(&kv_full[kvc % kAtStages], (kvc / kAtStages) & 1);
-        tc_fence_after();
-        for (int t = 0; t < n_t; ++t) {
-          if (sg[t] > 0) {  // the group has pulled its previous S tile into registers
-            mbar_wait(&s_free[t], (sg[t] - 1) & 1);
-            tc_fence_after();
-          }
-          issue_s(t, kvc % kAtStages);
-        }
-        if (J == 1) umma_commit(&q_empty[qc & 1]);
-        for (int j = 0; j < J; ++j, ++kvc) {
-          const int st = kvc % kAtStages;
-          if (j + 1 < J) {  // next S of both groups as soon as their registers hold the current one: runs under the softmax
-            mbar_wait(&kv_full[(kvc + 1) % kAtStages], ((kvc + 1) / kAtStages) & 1);
-            for (int t = 0; t < n_t; ++t) {
-              mbar_wait(&s_free[t], (sg[t] - 1) & 1);
-              tc_fence_after();
-              issue_s(t, (kvc + 1) % kAtStages);
-            }
-            if (j + 2 == J) umma_commit(&q_empty[qc & 1]);  // the item's last S MMAs are in flight: its Q buffer is free once they retire
-          }
-          for (int t = 0; t < n_t; ++t) {
-            mbar_wait(&p_full[t * 2 + (pg[t] & 1)], (pg[t] >> 1) & 1);
-            tc_fence_after();
-            issue_pv(t, st, j == 0);
-          }
-          umma_commit(&kv_empty[st]);  // K_j / V_j free once every MMA issued so far has retired
-        }
-      }
-    }
   } else {
-    // ===================== softmax group t: one query row per thread =====================
+    // ===================== warpgroup t: query tile t of the item =====================
     const int t = warp >> 2;
-    const int lane_base = (warp & 3) * 32;
-    const int r = lane_base + lane;                // row inside the tile
-    const uint32_t s_addr = tmem_base + (static_cast<uint32_t>(lane_base) << 16) + t * kAtKV;
-    const uint32_t o_addr = tmem_base + (static_cast<uint32_t>(lane_base) << 16) + 2 * kAtKV + t * kAtD;
-    const int rsw = r & 7;
-    int gt = 0;  // tiles this group has processed (phases)
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const int wl = warp & 3;
+    const int fcol = (lane & 3) * 2;  // first of this thread's two columns in every 8-column block
+    int qc = 0, kvc = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++qc) {
       int pair, h, b;
       decode(item, pair, h, b);
       const int qt0 = pair * 2;
-      if (t >= min(2, p.n_qtiles - qt0)) continue;   // odd tile count: the pair's second group idles for this item
-      const int row = (qt0 + t) * kAtQM + r;         // token index of this query
-      const bool warp_rows_valid = (qt0 + t) * kAtQM + lane_base < N;  // warp-uniform
-      float m_ref = -INFINITY, l = 0.f;
-      for (int j = 0; j < J; ++j, ++gt) {
-        const int buf = gt & 1;
-        uint8_t* prow = smem_p + (t * 2 + buf) * kAtQTile + r * 128;
-        mbar_wait(&s_full[t], gt & 1);
-        tc_fence_after();
+      const int qb = qc & 1;
+      if (t >= min(2, p.n_qtiles - qt0)) {
+        // odd tile count: this warpgroup idles for the item but still releases what the producer counts on.  Waiting for
+        // each fill first keeps its arrivals in the phase they belong to.
+        mbar_wait<true>(&q_full[qb], (qc >> 1) & 1);
+        if (lane == 0) mbar_arrive(&q_empty[qb]);
+        for (int j = 0; j < J; ++j, ++kvc) {
+          const int st = kvc % kAtStages;
+          mbar_wait<true>(&kv_full[st], (kvc / kAtStages) & 1);
+          if (lane == 0) mbar_arrive(&kv_empty[st]);
+        }
+        continue;
+      }
+      mbar_wait<true>(&q_full[qb], (qc >> 1) & 1);
+      // rows of this thread: (hm, i) -> tile row hm * 64 + wl * 16 + lane / 4 + 8 i
+      float o[2][32];
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[hm][i] = 0.f;
+      float m_ref[2][2], l[2][2];
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          m_ref[hm][i] = -INFINITY;
+          l[hm][i] = 0.f;
+        }
+      for (int j = 0; j < J; ++j, ++kvc) {
+        const int st = kvc % kAtStages;
+        mbar_wait<true>(&kv_full[st], (kvc / kAtStages) & 1);
+        // ---- S = Q K^T ----
+        float s[2][32];
+        wgmma_fence();
+#pragma unroll
+        for (int hm = 0; hm < 2; ++hm) {
+          const uint64_t da = wgmma_desc_k_sw128(smem_u32(smem_q + (qb * 2 + t) * kAtQTile + hm * 8192));
+          const uint64_t db = wgmma_desc_k_sw128(smem_u32(smem_kv + st * 2 * kAtKTile));
+#pragma unroll
+          for (int k = 0; k < kAtD / 16; ++k) wgmma_m64n64k16_ss<true, 0, 0>(s[hm], da + 2 * k, db + 2 * k, k > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s[0]);
+        wgmma_fence_regs(s[1]);
+        if (j + 1 == J && lane == 0) mbar_arrive(&q_empty[qb]);  // the item's last S MMAs have retired: its Q buffer is free
         const int valid = min(kAtKV, N - j * kAtKV);  // keys of this tile that exist
-        // ---- the tile row of S: TMEM -> registers, then TMEM is handed back at once (the next S = Q K^T runs under this softmax) ----
-        uint32_t v[2][32];
-        if (warp_rows_valid) {
-          tmem_ld_32x32b_x32(s_addr, v[0]);
-          tmem_ld_32x32b_x32(s_addr + 32, v[1]);
-          tmem_ld_wait();
+        // ---- row maxima (a row's 64 scores are spread over the 4 threads of a quad) ----
+        float mx[2][2];
+        bool grow = false;
+#pragma unroll
+        for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            float m = -INFINITY;
+#pragma unroll
+            for (int jb = 0; jb < 8; ++jb)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                if (valid == kAtKV || jb * 8 + fcol + e < valid) m = fmaxf(m, s[hm][4 * jb + 2 * i + e]);
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            mx[hm][i] = m * p.scale_log2e;
+            if (j > 0 && fmaxf(m_ref[hm][i], mx[hm][i]) - m_ref[hm][i] > 8.0f) grow = true;
+          }
+        if (j == 0) {
+#pragma unroll
+          for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) m_ref[hm][i] = mx[hm][i];
+        } else if (__any_sync(0xffffffffu, grow)) {
+          // rescale O and l of the rows of this warp (alpha = 1 for rows whose maximum did not move)
+#pragma unroll
+          for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const float m_new = fmaxf(m_ref[hm][i], mx[hm][i]);
+              const float alpha = ex2_approx(m_ref[hm][i] - m_new);
+              m_ref[hm][i] = m_new;
+              l[hm][i] *= alpha;
+#pragma unroll
+              for (int jb = 0; jb < 8; ++jb) {
+                o[hm][4 * jb + 2 * i] *= alpha;
+                o[hm][4 * jb + 2 * i + 1] *= alpha;
+              }
+            }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_free[t]);
-        if (warp_rows_valid) {  // warps whose 32 query rows all lie beyond N skip the arithmetic (their O rows are never stored)
-          float mx = -INFINITY;
-          if (valid == kAtKV) {
+        // ---- P = exp2(s * c - m_ref) -> bf16 A fragments (the accumulator layout of a 64 x 16 block), row sums in fp32 ----
+        uint32_t pa[2][4][4];
 #pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              mx = fmax3(mx, __uint_as_float(v[0][i]), __uint_as_float(v[0][i + 1]));
-              mx = fmax3(mx, __uint_as_float(v[1][i]), __uint_as_float(v[1][i + 1]));
-            }
-          } else {
+        for (int hm = 0; hm < 2; ++hm) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              if (i < valid) mx = fmaxf(mx, __uint_as_float(v[0][i]));
-              if (32 + i < valid) mx = fmaxf(mx, __uint_as_float(v[1][i]));
-            }
-          }
-          mx *= p.scale_log2e;
-          if (j == 0) {
-            m_ref = mx;
-          } else {
-            const float m_new = fmaxf(m_ref, mx);
-            if (__any_sync(0xffffffffu, m_new - m_ref > 8.0f)) {
-              // rescale O and l of the rows of this warp (alpha = 1 for rows whose maximum did not move)
-              const float alpha = ex2_approx(m_ref - m_new);
-              m_ref = m_new;
-              l *= alpha;
-              mbar_wait(&p_empty[t * 2 + ((gt - 1) & 1)], ((gt - 1) >> 1) & 1);  // every earlier P V has retired: O is stable
-              tc_fence_after();
+          for (int jb = 0; jb < 8; ++jb)
 #pragma unroll
-              for (int hc = 0; hc < kAtD / 32; ++hc) {
-                uint32_t o[32];
-                tmem_ld_32x32b_x32(o_addr + hc * 32, o);
-                tmem_ld_wait();
+            for (int i = 0; i < 2; ++i) {
+              float e2[2];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                tmem_st_32x32b_x32(o_addr + hc * 32, o);
+              for (int e = 0; e < 2; ++e) {
+                const float x = fmaf(s[hm][4 * jb + 2 * i + e], p.scale_log2e, -m_ref[hm][i]);
+                // the sequence's ragged last tile: keys beyond N get P = 0 exactly (never NaN garbage)
+                e2[e] = (valid == kAtKV || jb * 8 + fcol + e < valid) ? ex2_approx(x) : 0.f;
+                l[hm][i] += e2[e];
               }
-              tmem_st_wait();
+              pa[hm][jb >> 1][(jb & 1) * 2 + i] = pack_bf16x2(e2[0], e2[1]);
             }
-          }
-          if (gt >= 2) mbar_wait(&p_empty[t * 2 + buf], ((gt >> 1) - 1) & 1);  // the P V that read this P buffer two tiles ago has retired
-          // ---- P = exp2(s * c - m_ref) -> bf16 -> shared memory (K-major, 128-byte swizzle), row sum in fp32 ----
-          const float2 sc2 = make_float2(p.scale_log2e, p.scale_log2e), nm2 = make_float2(-m_ref, -m_ref);
-          float2 lsum = make_float2(0.f, 0.f);
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t pk[16];
-            if (valid == kAtKV) {  // full tile: no per-element predicates
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                const float2 x = ffma2(make_float2(__uint_as_float(v[c][i]), __uint_as_float(v[c][i + 1])), sc2, nm2);
-                const float2 e = make_float2(ex2_approx(x.x), ex2_approx(x.y));
-                lsum = fadd2(lsum, e);
-                pk[i >> 1] = pack_bf16x2(e.x, e.y);
-              }
-            } else {  // the sequence's ragged last tile: keys beyond N get P = 0 exactly (never NaN garbage)
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) {
-                const float2 x = ffma2(make_float2(__uint_as_float(v[c][i]), __uint_as_float(v[c][i + 1])), sc2, nm2);
-                const float e0 = c * 32 + i < valid ? ex2_approx(x.x) : 0.f;
-                const float e1 = c * 32 + i + 1 < valid ? ex2_approx(x.y) : 0.f;
-                lsum.x += e0;
-                lsum.y += e1;
-                pk[i >> 1] = pack_bf16x2(e0, e1);
-              }
-            }
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int chunk = c * 4 + q;  // 16-byte chunk inside the 128-byte row
-              *reinterpret_cast<uint4*>(prow + ((chunk ^ rsw) << 4)) = make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-            }
-          }
-          l += lsum.x + lsum.y;
         }
-        tc_fence_before();
-        fence_proxy_async_smem();  // generic-proxy stores of P -> visible to the tensor core's async proxy
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[t * 2 + buf]);
+        // ---- O += P V ----
+        wgmma_fence();
+#pragma unroll
+        for (int hm = 0; hm < 2; ++hm) {
+          const uint64_t db = wgmma_desc_mn_sw128(smem_u32(smem_kv + st * 2 * kAtKTile + kAtKTile), 8192);
+#pragma unroll
+          for (int kk = 0; kk < kAtKV / 16; ++kk) wgmma_m64n64k16_rs_bf16<1>(o[hm], pa[hm][kk], db + 128u * kk, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o[0]);
+        wgmma_fence_regs(o[1]);
+        if (lane == 0) mbar_arrive(&kv_empty[st]);  // K_j / V_j free
       }
-      // ---- epilogue: O / l -> bf16 row ----
-      mbar_wait(&p_empty[t * 2 + ((gt - 1) & 1)], ((gt - 1) >> 1) & 1);
-      tc_fence_after();
-      const float inv = 1.0f / l;
-      // tcgen05.ld is .sync.aligned: EVERY lane of the warp executes it (rows beyond N included); only the stores are predicated
-      __nv_bfloat16* dst = p.out + (static_cast<size_t>(b) * p.N + (row < p.N ? row : 0)) * (static_cast<size_t>(p.H) * kAtD) + h * kAtD;
+      // ---- epilogue: O / l -> bf16 rows ----
 #pragma unroll
-      for (int hc = 0; hc < kAtD / 32; ++hc) {
-        uint32_t o[32];
-        tmem_ld_32x32b_x32(o_addr + hc * 32, o);
-        tmem_ld_wait();
-        if (row < p.N) {
+      for (int hm = 0; hm < 2; ++hm)
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 w;
-            w.x = pack_bf16x2(__uint_as_float(o[8 * q]) * inv, __uint_as_float(o[8 * q + 1]) * inv);
-            w.y = pack_bf16x2(__uint_as_float(o[8 * q + 2]) * inv, __uint_as_float(o[8 * q + 3]) * inv);
-            w.z = pack_bf16x2(__uint_as_float(o[8 * q + 4]) * inv, __uint_as_float(o[8 * q + 5]) * inv);
-            w.w = pack_bf16x2(__uint_as_float(o[8 * q + 6]) * inv, __uint_as_float(o[8 * q + 7]) * inv);
-            *reinterpret_cast<uint4*>(dst + hc * 32 + q * 8) = w;
+        for (int i = 0; i < 2; ++i) {
+          float lt = l[hm][i];
+          lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+          lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+          const float inv = 1.0f / lt;
+          const int row = (qt0 + t) * kAtQM + hm * 64 + wl * 16 + (lane >> 2) + 8 * i;  // token index of this query
+          if (row < N) {
+            __nv_bfloat16* dst = p.out + (static_cast<size_t>(b) * N + row) * (static_cast<size_t>(p.H) * kAtD) + h * kAtD;
+#pragma unroll
+            for (int jb = 0; jb < 8; ++jb)
+              *reinterpret_cast<uint32_t*>(dst + jb * 8 + fcol) =
+                  pack_bf16x2(o[hm][4 * jb + 2 * i] * inv, o[hm][4 * jb + 2 * i + 1] * inv);
+            if (p.lse2 && (lane & 3) == 0) p.lse2[(static_cast<size_t>(b) * p.H + h) * N + row] = m_ref[hm][i] + log2f(lt);
           }
         }
-      }
-      if (row < p.N && p.lse2) p.lse2[(static_cast<size_t>(b) * p.H + h) * p.N + row] = m_ref + log2f(l);
-      tc_fence_before();  // this item's O reads are ordered before the p_full arrival that lets the next item's P V overwrite O
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc<kAtTmemCols>(tmem_base);
   }
 }
 

@@ -4,7 +4,7 @@
 //   models/faceX/backbone/timm_wrapper.py:51-54 (TimmWrapper.forward), :30-38 (output_layer),
 //   models/faceX/face_model.py:137-139 (extract_cbir: model(x) then F.normalize).
 //
-// Dense contractions run on the tcgen05 GEMM (gemm.cu) with fused epilogues; everything around them is an
+// Dense contractions run on the wgmma GEMM (gemm.cu) with fused epilogues; everything around them is an
 // HBM-bound kernel written here:
 //   stem_patchify     NCHW fp32 image -> 4x4 patch rows [B*H/4*W/4, 48] bf16          (then GEMM + bias + LayerNorm)
 //   dwconv7_ln        depthwise 7x7 (pad 3) + bias + LayerNorm over C, NHWC bf16      (then GEMM+GELU, GEMM+gamma+res)
@@ -304,7 +304,7 @@ dwconv7_chunk_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, in
   __syncthreads();
   constexpr int pix_stride = chunk * 2;
   const bool active = has_c && warp < TH && oy0 + warp < H;
-  float2 acc[kDwTW][2];  // channel pairs (c0, c0+1), (c0+2, c0+3): the tap loop runs on FFMA2
+  float2 acc[kDwTW][2];  // channel pairs (c0, c0+1), (c0+2, c0+3)
 #pragma unroll
   for (int p = 0; p < kDwTW; ++p) {
     acc[p][0] = make_float2(bc.x, bc.y);
@@ -430,16 +430,14 @@ dwconv7_chunk_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, in
 // ------------------------------------------------------------------------------------------------
 // the same operator, PERSISTENT and software-pipelined (the default): latency was the limiter of the kernel above
 // ------------------------------------------------------------------------------------------------
-// Measured on B200 (tools/ubench_fma.cu): FFMA2 sustains 118 FMA/clk/SM at one issue slot per 2.17 clk, i.e. the tap loop's
-// 98 FFMA2 : 83 other instructions per filter row fits the FP32 pipe's shadow — yet the one-tile-per-CTA kernel ran at 25 %
-// of that rate (IPC 0.25 per scheduler): every CTA paid tensormap prefetch + barrier init + a 43 KB TMA load + 25 KB of tap
+// The one-tile-per-CTA kernel above is limited by latency, not by the FP32 pipe: every CTA pays tensormap prefetch + barrier init + a 43 KB TMA load + 25 KB of tap
 // staging + a cluster barrier + remote partial reads, with nothing to overlap them but two sibling CTAs in the same phase.
 // Here a CTA lives for the whole launch and keeps ONE channel chunk: the chunk's taps / bias / LayerNorm affine are staged
 // once, a producer warp streams halo tiles (TH x 7 output pixels) through a two-deep TMA / mbarrier ring, TH compute warps
 // (one output row each) run the tap loop of tile i+1 while the LayerNorm statistics of tile i cross the cluster
 // (split-phase barrier.cluster: arrive after publishing the chunk's (mean, M2), wait only after the next tile's taps).
 // LayerNorm numerics are unchanged: two-pass statistics per chunk, Chan's combination across the chunks of a pixel.
-template <int MODE, int CHUNK, int TH, bool F2>
+template <int MODE, int CHUNK, int TH>
 __global__ void __launch_bounds__((TH + 1) * 32, TH == 7 ? 2 : 1)
 dwconv7_pipe_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W, int C, int nchunks, int n_tiles,
                     const float* __restrict__ w49, const float* __restrict__ bias, const float* __restrict__ ln_w,
@@ -530,7 +528,7 @@ dwconv7_pipe_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int
   constexpr int pix_stride = CHUNK * 2;
   const float inv_chunk = 1.0f / static_cast<float>(CHUNK), inv_c = 1.0f / static_cast<float>(C);
 
-  // tap loop of one tile row: acc[p] = bias + sum over the 7x7 window (FFMA2 over channel pairs)
+  // tap loop of one tile row: acc[p] = bias + sum over the 7x7 window (FMAs over channel pairs)
   auto conv_row = [&](const uint8_t* tile, float2 (&acc)[kDwTW][2]) {
 #pragma unroll
     for (int p = 0; p < kDwTW; ++p) {
@@ -558,15 +556,8 @@ dwconv7_pipe_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int
         for (int p = 0; p < kDwTW; ++p) {
           const int dx = ix - p;
           if (dx >= 0 && dx < 7) {
-            if (F2) {
-              acc[p][0] = ffma2(a, wlo[dx], acc[p][0]);
-              acc[p][1] = ffma2(c, whi[dx], acc[p][1]);
-            } else {  // scalar FFMA form of the same arithmetic (tools/ubench_fma.cu: which form sustains more with these operands)
-              acc[p][0].x = fmaf(a.x, wlo[dx].x, acc[p][0].x);
-              acc[p][0].y = fmaf(a.y, wlo[dx].y, acc[p][0].y);
-              acc[p][1].x = fmaf(c.x, whi[dx].x, acc[p][1].x);
-              acc[p][1].y = fmaf(c.y, whi[dx].y, acc[p][1].y);
-            }
+            acc[p][0] = ffma2(a, wlo[dx], acc[p][0]);
+            acc[p][1] = ffma2(c, whi[dx], acc[p][1]);
           }
         }
       }
@@ -887,7 +878,7 @@ static int launch_dwconv_tw(const CUtensorMap& mx, int batch, int H, int W, int 
 
 
 // Persistent launch: one CTA per SM (two for the 7-row tile), grid = co-resident clusters x chunks.
-template <int MODE, int CHUNK, int TH, bool F2>
+template <int MODE, int CHUNK, int TH>
 static int launch_dwconv7_pipe_t(const __nv_bfloat16* x, int batch, int H, int W, int C, const float* w49, const float* bias,
                                  const float* ln_w, const float* ln_b, float eps, __nv_bfloat16* y, float* rstd_out,
                                  const __nv_bfloat16* addend, cudaStream_t s) {
@@ -898,7 +889,7 @@ static int launch_dwconv7_pipe_t(const __nv_bfloat16* x, int batch, int H, int W
   CUtensorMap mx;
   int rc = make_tma_nhwc_16bit(&mx, x, batch, H, W, C, TH + 6, kDwTW + 6, CHUNK);
   if (rc != VDK_OK) return rc;
-  auto kern = dwconv7_pipe_kernel<MODE, CHUNK, TH, F2>;
+  auto kern = dwconv7_pipe_kernel<MODE, CHUNK, TH>;
   const int cluster = (MODE == 0) ? nchunks : 1;
   struct Fit { int clusters; };
   static Fit fit[17] = {};  // per cluster size: co-resident clusters of this instantiation (queried once)
@@ -943,16 +934,9 @@ static int launch_dwconv7_pipe(int mode, const __nv_bfloat16* x, int batch, int 
                                const float* bias, const float* ln_w, const float* ln_b, float eps, __nv_bfloat16* y, float* rstd_out,
                                const __nv_bfloat16* addend, cudaStream_t s) {
   const bool tall = H > 7;  // 14-row tiles (15 warps, one CTA per SM) unless the map is 7 rows high
-  static const bool f2 = [] {
-    const char* e = getenv("VDK_DWCONV_FFMA2");
-    return e ? atoi(e) != 0 : true;
-  }();
 #define VDK_DWP(MODEV, CHV)                                                                                                           \
-  if (f2)                                                                                                                             \
-    return tall ? launch_dwconv7_pipe_t<MODEV, CHV, 14, true>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)  \
-                : launch_dwconv7_pipe_t<MODEV, CHV, 7, true>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s);  \
-  return tall ? launch_dwconv7_pipe_t<MODEV, CHV, 14, false>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)   \
-              : launch_dwconv7_pipe_t<MODEV, CHV, 7, false>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)
+  return tall ? launch_dwconv7_pipe_t<MODEV, CHV, 14>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)          \
+              : launch_dwconv7_pipe_t<MODEV, CHV, 7>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)
   if (mode == 0) {
     if (chunk == 128) { VDK_DWP(0, 128); }
     if (chunk == 96) { VDK_DWP(0, 96); }
@@ -1130,7 +1114,7 @@ extern "C" int vdk_convnext_forward(const vdk_convnext_net* net, const float* im
   int M = batch * H * W;
   {
     const int64_t total = static_cast<int64_t>(M) * 12;
-    const int blocks = static_cast<int>(std::min<int64_t>((total + 255) / 256, 148 * 16));
+    const int blocks = static_cast<int>(std::min<int64_t>((total + 255) / 256, 132 * 16));
     stem_patchify_kernel<<<blocks, 256, 0, s>>>(images, batch, S, S, hbuf);
     VDK_CUDA_OK(cudaGetLastError());
     rc = gemm(hbuf, net->stem_w, xbuf, M, C, 48, VDK_EPI_LAYERNORM, net->stem_b, net->stem_ln_w, net->stem_ln_b, nullptr,

@@ -1,5 +1,5 @@
 // convnext_train.cu — ConvNeXt + neck training forward (activations saved) and backward, orchestrated in C++ over the
-// tcgen05 GEMM (gemm.cu: K-major and MN-major operands, so dgrad / wgrad need no transposed copies) and the HBM-bound
+// wgmma GEMM (gemm.cu: K-major and MN-major operands, so dgrad / wgrad need no transposed copies) and the HBM-bound
 // kernels of convnext.cu / train_ops.cu.
 //
 // Replaces, for the faceX train step (engine/procedure/train.py:196,206): the forward of TimmWrapper in train mode
@@ -190,7 +190,7 @@ extern "C" size_t vdk_convnext_train_workspace_bytes(const vdk_convnext_net* net
 }
 
 // ---- weight packing, batched: the blocks of a stage have identical shapes, so ONE launch per (stage, kind) walks a table
-// of per-block pointers passed by value (the per-tensor kernels were launch-bound: ~190 launches of 3-5 us per step) ----
+// of per-block pointers passed by value (instead of ~190 small per-tensor launches per step) ----
 constexpr int kPackTab = 32;
 struct PackTab {
   const float* src[kPackTab];
@@ -348,7 +348,7 @@ extern "C" int vdk_convnext_train_forward(const vdk_convnext_net* net, const vdk
   {
     const int M0 = static_cast<int>(L.st[0].M), C0 = L.st[0].C;
     const int64_t total = static_cast<int64_t>(M0) * 12;
-    stem_patchify_train_kernel<<<static_cast<int>(std::min<int64_t>((total + 255) / 256, 148 * 16)), 256, 0, s>>>(images, batch, S, S,
+    stem_patchify_train_kernel<<<static_cast<int>(std::min<int64_t>((total + 255) / 256, 132 * 16)), 256, 0, s>>>(images, batch, S, S,
                                                                                                              B16(L.p0));
     VDK_CUDA_OK(cudaGetLastError());
     RC(G.run(B16(L.p0), net->stem_w, B16(L.z0), M0, C0, 48, 48, 48, C0, VDK_EPI_NONE, net->stem_b, nullptr, nullptr, 0,
@@ -415,8 +415,7 @@ extern "C" int vdk_convnext_train_backward_units(const vdk_convnext_net* net) {
 // (shared-memory-free) column-sum kernel — so the sum runs UNDER the weight- and data-gradient GEMMs of fc1 instead of in
 // front of them.  Fork: the side stream waits for the event recorded after the GEMM that produced dH; join: the caller's stream
 // waits for the side stream's last event before the call returns (the gradients it wrote are then ordered before anything the
-// caller enqueues next: the optimizer, an all-reduce, the next forward that overwrites dH).  Measured (profiles/r02_train.md): no
-// gain — 30.26 ms with it, 30.20 ms without: the single resident block per SM reads too slowly to hide — so it is OFF unless
+// caller enqueues next: the optimizer, an all-reduce, the next forward that overwrites dH).  It is OFF unless
 // VDK_TRAIN_SIDE_STREAM=1.
 struct SideStream {
   cudaStream_t stream = nullptr;

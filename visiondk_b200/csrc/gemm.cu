@@ -1,14 +1,15 @@
-// gemm.cu — D = epilogue(A . B^T) on tcgen05 tensor cores, operands staged by TMA, accumulators in TMEM.
+// gemm.cu — D = epilogue(A . B^T) on sm_90a warpgroup tensor cores (wgmma), operands staged by TMA.
 //
 // Replaces the library GEMMs behind timm's ConvNeXt/ViT Linear layers and patchify convolutions that
 // models/faceX/backbone/timm_wrapper.py:52 runs, and the neck Linear of timm_wrapper.py:36 (SURVEY K1-K5).
 //
-// One persistent CTA per SM, 320 threads:
-//   warp 0      : TMA producer   (A tile 128x64, B tile BNx64 per stage, 128-byte swizzle)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128 x BN x 16, fp32 accumulate)
-//   warps 2..9  : epilogue       (tcgen05.ld -> bias / GELU / layer-scale+residual / LayerNorm -> 16-byte global
-//                 stores); two warps share each TMEM lane quarter and take alternate 32-column chunks
-// Two accumulator stages in TMEM (2 x BN columns) let the epilogue of tile i overlap the MMAs of tile i+1.
+// One persistent CTA per SM, 384 threads:
+//   warpgroup 0    : TMA producer (one thread; A tile 128x64, B tile BNx64 per stage, 128-byte swizzle), registers
+//                    handed to the consumers with setmaxnreg
+//   warpgroups 1-2 : consumers, 64 rows each: wgmma m64 x BN x 16 into registers (fp32), then the epilogue.  The
+//                    accumulator leaves the registers 64 columns at a time through shared memory so that each thread
+//                    finishes 32 consecutive columns of one row (bias / GELU / layer-scale+residual / LayerNorm /
+//                    GELU' -> 16-byte global stores) while the producer already fills the stages of the next tile.
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
 
@@ -18,7 +19,8 @@ namespace vdk {
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;  // 64 x 16-bit = one 128-byte swizzle row
-constexpr int kGemmThreads = 320;  // TMA warp, MMA warp, 8 epilogue warps
+constexpr int kGemmThreads = 384;  // producer warpgroup, two consumer warpgroups
+constexpr int kAccLd = 64 + 4;     // fp32 row pitch of the staged 128 x 64 accumulator chunk (conflict-free row reads)
 
 struct GemmParams {
   int M, N, K;
@@ -27,16 +29,14 @@ struct GemmParams {
   const float* bias;
   const float* gamma;  // layer-scale (SCALE_RESIDUAL) or LayerNorm weight (LAYERNORM)
   const float* beta;   // LayerNorm bias
-  const void* residual;
+  const void* residual;  // SCALE_RESIDUAL: added; MUL_GELU_GRAD: the saved 16-bit pre-activation whose GELU' scales the output
   int ldr;
   int out_dtype;
   int epilogue;
   float ln_eps;
   int split_k;  // > 1: each tile's K range is split over split_k work items, fp32 partials are atomically added
-  int tma_store;  // 16-bit outputs: stage 128x64 sub-tiles in smem and write them with TMA (full-line stores)
-  int a_mn, b_mn;  // operand stored with the contraction index as the slow dimension ([K,M] / [K,N] row-major)
   long long split_stride;  // > 0: split s writes its partial tile to D + s*split_stride with plain stores (deterministic)
-  int aux_out;  // GELU only: also store the pre-activation (acc + bias) through map_d2 (saved for the backward)
+  void* aux;  // GELU only: also store the pre-activation (acc + bias) here, pitch ldd (saved for the backward)
   int partial_out;  // the caller asked for split-K: raw fp32 partials are added / slab-stored even if one split remains
 };
 
@@ -45,11 +45,11 @@ struct GemmCfg {
   static constexpr int kStageA = kBM * kBK * 2;
   static constexpr int kStageB = BN * kBK * 2;
   static constexpr int kStageBytes = kStageA + kStageB;
-  static constexpr int kStages = (BN == 256) ? 4 : 6;
-  static constexpr int kTmemCols = 2 * BN;
-  // stages + barriers (full, empty: kStages each; tmem_full, tmem_empty: 2 each) + tmem ptr + 1 KB align slack
-  static constexpr int kStoreStageBytes = kBM * 64 * 2;  // one 128 x 64 16-bit sub-tile per epilogue half
-  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kStoreStageBytes + (2 * kStages + 6) * 8 + 16 + 1024;
+  static constexpr int kStages = (BN == 256) ? 3 : 5;
+  static constexpr int kAccBytes = kBM * kAccLd * 4;
+  // stages + staged accumulator chunk + bias [BN] + LayerNorm mean / rstd [2][128] + barriers + 1 KB align slack
+  static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + BN * 4 + 2 * kBM * 4 + 2 * kStages * 8 + 1024;
+  static_assert(kSmemBytes <= 227 * 1024, "GEMM shared memory budget");
 };
 
 __device__ __forceinline__ float rcp_approx(float x) {
@@ -62,9 +62,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// erf-GELU for the forward epilogue.  The fc1 epilogue applies 4C x tokens GELUs per block while the tensor core
-// needs only 4096 cycles per 128 x 256 tile, so the activation has to cost ~5 issue slots and half an SFU op per
-// element or the epilogue, not the MMA, sets the pace (measured: two MUFU per element saturate the 16/cycle SFU).
+// erf-GELU for the forward epilogue.  The fc1 epilogue applies 4C x tokens GELUs per block, so the activation has to
+// cost few issue slots and at most one SFU op per pair of elements or the epilogue, not the MMA, sets the pace.
 // y = 0.5 x (1 + tanh(u)), u = x (c1 + c3 x^2) with (c1, c3) refitted to the erf form (max |dev| 3.1e-4 instead of the
 // textbook tanh-GELU's 4.7e-4); u and tanh are evaluated two elements at a time in fp16x2 (tanh.approx.f16x2,
 // rel. error 2^-11), the final multiply in fp32 so that y -> x exactly for large x.  Absolute error <= 6e-4 |x|:
@@ -132,9 +131,25 @@ __device__ __forceinline__ void add_bias32(float (&v)[32], const float* bsm) {
   }
 }
 __device__ __forceinline__ void epi_math(const GemmParams& p, float (&v)[32], int row, int col0, int ncols, float ln_mean,
-                                         float ln_rstd, const float* bsm, bool residual_from_smem = false) {
+                                         float ln_rstd, const float* bsm) {
   if (p.bias != nullptr) add_bias32(v, bsm);
-  if (p.epilogue == VDK_EPI_GELU) {
+  if (p.epilogue == VDK_EPI_MUL_GELU_GRAD) {
+    if (row < p.M) {
+      const uint16_t* pre = reinterpret_cast<const uint16_t*>(p.residual) + static_cast<size_t>(row) * p.ldr + col0;
+#pragma unroll
+      for (int j = 0; j < 32; j += 8) {
+        if (j < ncols) {
+          const uint4 t = *reinterpret_cast<const uint4*>(pre + j);
+          const float2 a0 = unpack2(t.x, p.out_dtype), a1 = unpack2(t.y, p.out_dtype);
+          const float2 a2 = unpack2(t.z, p.out_dtype), a3 = unpack2(t.w, p.out_dtype);
+          const float2 g0 = gelu_grad_pair(a0.x, a0.y), g1 = gelu_grad_pair(a1.x, a1.y);
+          const float2 g2 = gelu_grad_pair(a2.x, a2.y), g3 = gelu_grad_pair(a3.x, a3.y);
+          v[j] *= g0.x; v[j + 1] *= g0.y; v[j + 2] *= g1.x; v[j + 3] *= g1.y;
+          v[j + 4] *= g2.x; v[j + 5] *= g2.y; v[j + 6] *= g3.x; v[j + 7] *= g3.y;
+        }
+      }
+    }
+  } else if (p.epilogue == VDK_EPI_GELU) {
 #pragma unroll
     for (int j = 0; j < 32; j += 2) gelu_pair(v[j], v[j + 1]);
   } else if (p.epilogue == VDK_EPI_LAYERNORM) {
@@ -157,7 +172,7 @@ __device__ __forceinline__ void epi_math(const GemmParams& p, float (&v)[32], in
         v[j] *= g.x; v[j + 1] *= g.y; v[j + 2] *= g.z; v[j + 3] *= g.w;
       }
     }
-    if (row < p.M && !residual_from_smem) {
+    if (row < p.M) {
       if (p.out_dtype == VDK_DTYPE_FP32) {
         const float* res = reinterpret_cast<const float*>(p.residual) + static_cast<size_t>(row) * p.ldr + col0;
 #pragma unroll
@@ -183,587 +198,272 @@ __device__ __forceinline__ void epi_math(const GemmParams& p, float (&v)[32], in
     }
   }
 }
-
-// kAux: the epilogue streams a second 16-bit tile per output tile (the residual / saved pre-activation it reads, or the
-// pre-activation copy it writes).  That variant trades one mainloop stage for two more 16 KB staging buffers, so the
-// auxiliary input of the NEXT sub-tile is prefetched by TMA while this one is computed and stored, and the two output
-// streams never wait on each other's staging buffer (these GEMMs have short K loops: the epilogue sets their pace).
-// kPair: the CTAs of a 2-cluster (one TPC) run ONE UMMA of M = 256 (tcgen05 cta_group::2): each CTA stages its own 128
-// rows of A and HALF of the B tile, the leader's MMA thread reads both shared memories, and each CTA's TMEM receives
-// its 128 accumulator rows.  Per output tile that halves the B bytes every SM pulls through L2 and shrinks a stage to
-// 32 KB, so six stages (instead of four) cover the TMA latency at the same shared-memory budget.
-template <int BN, bool kBf16, bool kAux, bool kPair>
+// kTA / kTB: operand stored with the contraction index as the slow dimension ([K,M] / [K,N] row-major: MN-major)
+template <int BN, bool kBf16, int kTA, int kTB>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_r,
-               const __grid_constant__ CUtensorMap map_d2, const GemmParams p) {
+gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
   using Cfg = GemmCfg<BN>;
-  constexpr int kStageB = kPair ? Cfg::kStageB / 2 : Cfg::kStageB;  // B rows staged by this CTA
-  constexpr int kStageBytes = Cfg::kStageA + kStageB;
-  constexpr int kStages = kPair ? (kAux ? 5 : 6) : Cfg::kStages - (kAux ? 1 : 0);
-  constexpr int kStoreBufs = kAux ? 4 : 2;
-  constexpr int kTM = kPair ? 2 * kBM : kBM;  // rows of one work item (both CTAs of a pair)
-  const int rank = kPair ? static_cast<int>(cluster_ctarank()) : 0;
-  const int tile0 = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int tile_step = kPair ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   // align inside the dynamic smem window without a pointer->integer->pointer round trip (which would demote every
   // later access to generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* smem_store = smem + kStages * kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_store + kStoreBufs * Cfg::kStoreStageBytes);
+  float* acc_sm = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);  // [128][kAccLd]
+  float* bias_sm = acc_sm + kBM * kAccLd;                                      // [BN] bias of the tile being finished
+  float* ln_sm = bias_sm + BN;                                                 // [2][128] LayerNorm mean, rstd per row
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ln_sm + 2 * kBM);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint64_t* res_bar = tmem_empty + 2;  // residual sub-tile landed in the staging buffer (one per epilogue half)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(res_bar + 2);
-  float* bias_sm = reinterpret_cast<float*>(tmem_ptr + 4);  // [BN] bias of the tile being finished (16-byte aligned)
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  const int num_m = (p.M + kTM - 1) / kTM;
+  const int num_m = (p.M + kBM - 1) / kBM;
   const int num_n = (p.N + BN - 1) / BN;
   const int num_kb_total = (p.K + kBK - 1) / kBK;
   const int kb_per_split = (num_kb_total + p.split_k - 1) / p.split_k;
   const int num_tiles = num_m * num_n * p.split_k;  // work items; split index is the slowest dimension
-  (void)num_m;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tensormap(&map_a);
     prefetch_tensormap(&map_b);
-    if (p.tma_store) prefetch_tensormap(&map_d);
-    if (p.tma_store && (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD)) prefetch_tensormap(&map_r);
-    if (p.aux_out) prefetch_tensormap(&map_d2);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kPair ? 16 : 256);  // pair: one arrival per epilogue warp of both CTAs
-      mbar_init(&res_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if (kPair) tmem_alloc_pair<Cfg::kTmemCols>(tmem_ptr);
-    else tmem_alloc<Cfg::kTmemCols>(tmem_ptr);
-  }
-  tc_fence_before();
-  if (kPair) cluster_sync_all();  // the peer's barriers are initialised before any TMA / commit signals them
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  __syncthreads();
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int mn = tile % (num_m * num_n), split = tile / (num_m * num_n);
-        const int m0 = (mn / num_n) * kTM + rank * kBM;
-        const int n0 = (mn % num_n) * BN + (kPair ? rank * (BN / 2) : 0);  // first B row this CTA stages
+        const int m0 = (mn / num_n) * kBM;
+        const int n0 = (mn % num_n) * BN;
         const int kb0 = split * kb_per_split;
         const int kb1 = min(kb0 + kb_per_split, num_kb_total);
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait_relaxed(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * kStageBytes;
+          mbar_wait_relaxed<true>(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kStageA;
-          if (kPair) {
-            // both CTAs' bytes are credited to the LEADER's full barrier, which its MMA thread waits on
-            if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * kStageBytes);
-            if (p.a_mn) {
-#pragma unroll
-              for (int j = 0; j < kBM / 64; ++j)
-                tma_load_2d_pair(sa + j * 8192, &map_a, &full_bar[stage], m0 + j * 64, kb * kBK, kEvictNormal);
-            } else {
-              tma_load_2d_pair(sa, &map_a, &full_bar[stage], kb * kBK, m0, kEvictNormal);
-            }
-            if (p.b_mn) {
-#pragma unroll
-              for (int j = 0; j < BN / 128; ++j)
-                tma_load_2d_pair(sb + j * 8192, &map_b, &full_bar[stage], n0 + j * 64, kb * kBK, kEvictLast);
-            } else {
-              tma_load_2d_pair(sb, &map_b, &full_bar[stage], kb * kBK, n0, kEvictLast);
-            }
-          } else {
-          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-          if (p.a_mn) {  // [K,M] storage: 64-wide M blocks x 64 contraction rows, 8 KB each
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          if (kTA) {  // [K,M] storage: 64-wide M blocks x 64 contraction rows, 8 KB each
 #pragma unroll
             for (int j = 0; j < kBM / 64; ++j) tma_load_2d(sa + j * 8192, &map_a, &full_bar[stage], m0 + j * 64, kb * kBK, kEvictNormal);
           } else {
             tma_load_2d(sa, &map_a, &full_bar[stage], kb * kBK, m0, kEvictNormal);
           }
-          if (p.b_mn) {
+          if (kTB) {
 #pragma unroll
             for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &map_b, &full_bar[stage], n0 + j * 64, kb * kBK, kEvictLast);
           } else {
             tma_load_2d(sb, &map_b, &full_bar[stage], kb * kBK, n0, kEvictLast);
           }
-          }
           if (++stage == kStages) {
             stage = 0;
             phase ^= 1;
           }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0 && rank == 0) {  // pair: only the leader CTA issues (for both)
-      const uint32_t idesc = umma_idesc_f16<kBf16>(kTM, BN, p.a_mn ? 1u : 0u, p.b_mn ? 1u : 0u);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait_relaxed(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        const int split = tile / (num_m * num_n);
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb0 + kb_per_split, num_kb_total);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-          const uint32_t sb = sa + Cfg::kStageA;
-          const uint64_t da = p.a_mn ? umma_desc_mn_sw128(sa, 8192) : umma_desc_k_sw128(sa);
-          const uint64_t db = p.b_mn ? umma_desc_mn_sw128(sb, 8192) : umma_desc_k_sw128(sb);
-          // one UMMA consumes 16 contraction elements: K-major = 32 bytes inside the swizzle row (+2 in 16-byte
-          // units); MN-major = two 8-row groups of 1024 bytes (+128)
-          const uint32_t step_a = p.a_mn ? 128u : 2u, step_b = p.b_mn ? 128u : 2u;
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            if (kPair) umma_f16_ss_pair(tmem_d, da + step_a * k, db + step_b * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else umma_f16_ss(tmem_d, da + step_a * k, db + step_b * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // smem slot reusable once these MMAs retire (pair: in both CTAs)
-          if (kPair) umma_commit_pair(&empty_bar[stage]);
-          else umma_commit(&empty_bar[stage]);
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        // accumulator complete -> epilogue (pair: of both CTAs)
-        if (kPair) umma_commit_pair(&tmem_full[acc]);
-        else umma_commit(&tmem_full[acc]);
       }
     }
   } else {
-    // ===================== epilogue =====================
-    const int lane_base = (warp & 3) * 32;  // TMEM lanes this warp may touch
-    const int half = (warp - 2) >> 2;       // which of the two warps sharing this lane quarter
-    bool stores_issued = false;
-    uint32_t res_phase = 0;
-    int it = 0;
-    // (tile, 64-column sub-tile) sequence of this epilogue half: sub-tiles half, half + 2 of every tile of this CTA
-    auto next_sub = [&](int& t, int& sub) -> bool {
-      sub += 2;
-      while (t < num_tiles) {
-        if (sub < BN / 64 && ((t % (num_m * num_n)) % num_n) * BN + sub * 64 < p.N) return true;
-        t += tile_step;
-        sub = half;
-      }
-      return false;
-    };
-    if (kAux && p.tma_store && (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD) &&
-        threadIdx.x == 64 + half * 128) {
-      int nt = tile0, ns = half - 2;
-      if (next_sub(nt, ns)) {
-        const int nmn = nt % (num_m * num_n);
-        mbar_arrive_expect_tx(&res_bar[half], Cfg::kStoreStageBytes);
-        tma_load_2d(smem_store + (2 + half) * Cfg::kStoreStageBytes, &map_r, &res_bar[half], (nmn % num_n) * BN + ns * 64,
-                    (nmn / num_n) * kTM + rank * kBM, kEvictFirst);
-      }
-    }
-    for (int tile = tile0; tile < num_tiles; tile += tile_step, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int mn = tile % (num_m * num_n);
-      const int m0 = (mn / num_n) * kTM + rank * kBM;
+    // ===================== consumers: mainloop + epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int ct = threadIdx.x - 128;  // 0..255
+    const int cg = ct >> 7;            // consumer warpgroup: accumulator rows cg*64 .. cg*64+63 of the tile
+    const int wl = (ct >> 5) & 3, lane = ct & 31;
+    const int frow = cg * 64 + wl * 16 + (lane >> 2);  // first of this thread's two fragment rows (the other is + 8)
+    const int fcol = (lane & 3) * 2;
+    const int erow = ct & 127, half = ct >> 7;         // epilogue: row and 32-column half of a staged chunk
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int mn = tile % (num_m * num_n), split = tile / (num_m * num_n);
+      const int m0 = (mn / num_n) * kBM;
       const int n0 = (mn % num_n) * BN;
-      const int row = m0 + lane_base + lane;
-      if (p.bias != nullptr) {  // while the accumulator is still being produced
-        const int te = static_cast<int>(threadIdx.x) - 64;
-        named_bar_sync(3, 256);  // the previous tile's bias has been consumed by both halves
-        if (te < BN) bias_sm[te] = (n0 + te < p.N) ? __ldg(p.bias + n0 + te) : 0.f;
-        named_bar_sync(3, 256);
-      }
-      mbar_wait_relaxed(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + (static_cast<uint32_t>(lane_base) << 16) + acc * BN;
-      float ln_mean = 0.f, ln_rstd = 1.f;
-      if (p.epilogue == VDK_EPI_LAYERNORM) {
-        // the tile spans the whole row (N <= BN): this thread owns every channel of its row in TMEM.
-        // pass 1: mean, pass 2: centred variance; the write pass below re-reads TMEM (cheap) instead of
-        // holding BN values in registers.
-        float sum = 0.f;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(tacc + c * 32, r);
-          tmem_ld_wait();
+      const int kb0 = split * kb_per_split;
+      const int kb1 = min(kb0 + kb_per_split, num_kb_total);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait<true>(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes) + cg * 8192;  // K-major: 64 rows x 128 B; MN-major: 64-wide block
+        const uint32_t sb = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kStageA);
+        const uint64_t da = kTA ? wgmma_desc_mn_sw128(sa, 8192) : wgmma_desc_k_sw128(sa);
+        const uint64_t db = kTB ? wgmma_desc_mn_sw128(sb, 8192) : wgmma_desc_k_sw128(sb);
+        // one k16 step: K-major = 32 bytes inside the swizzle row (+2 in 16-byte units); MN-major = two 8-row groups (+128)
+        constexpr uint32_t step_a = kTA ? 128u : 2u, step_b = kTB ? 128u : 2u;
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int col = c * 32 + j;
-            if (col < p.N) sum += __uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + col) : 0.f);
-          }
+        for (int k = 0; k < kBK / 16; ++k) {
+          if constexpr (BN == 256) wgmma_m64n256k16_ss<kBf16, kTA, kTB>(acc, da + step_a * k, db + step_b * k, (kb > kb0 || k > 0) ? 1u : 0u);
+          else wgmma_m64n128k16_ss<kBf16, kTA, kTB>(acc, da + step_a * k, db + step_b * k, (kb > kb0 || k > 0) ? 1u : 0u);
         }
-        ln_mean = sum / static_cast<float>(p.N);
-        float sq = 0.f;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(tacc + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int col = c * 32 + j;
-            if (col < p.N) {
-              const float d = __uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + col) : 0.f) - ln_mean;
-              sq = fmaf(d, d, sq);
-            }
-          }
-        }
-        ln_rstd = rsqrtf(sq / static_cast<float>(p.N) + p.ln_eps);
-      }
-      if (kAux && p.tma_store) {
-        // pipelined variant of the staged epilogue below: `stg` stages the output sub-tile, `stg2` holds the auxiliary
-        // INPUT sub-tile (prefetched: the load of the next one is issued as soon as this one sits in registers) or
-        // stages the auxiliary OUTPUT (the saved pre-activation)
-        uint8_t* stg = smem_store + half * Cfg::kStoreStageBytes;
-        uint8_t* stg2 = smem_store + (2 + half) * Cfg::kStoreStageBytes;
-        const bool leader = threadIdx.x == 64 + half * 128;
-        const int rit = lane_base + lane;  // row inside the tile
-        const bool aux_in = p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD;
-#pragma unroll 1
-        for (int sc = half; sc < BN / 64; sc += 2) {
-          const int colS = n0 + sc * 64;
-          if (colS >= p.N) break;
-          uint32_t packed[32], ain[32];
-          if (aux_in) {
-            mbar_wait(&res_bar[half], res_phase);
-            res_phase ^= 1;
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const uint4 t = *reinterpret_cast<const uint4*>(stg2 + rit * 128 + ((q ^ (rit & 7)) << 4));
-              ain[4 * q] = t.x; ain[4 * q + 1] = t.y; ain[4 * q + 2] = t.z; ain[4 * q + 3] = t.w;
-            }
-            named_bar_sync(1 + half, 128);  // every row of the input sub-tile is in registers: stg2 may be refilled
-            if (leader) {
-              int nt = tile, ns = sc;
-              if (next_sub(nt, ns)) {
-                const int nmn = nt % (num_m * num_n);
-                mbar_arrive_expect_tx(&res_bar[half], Cfg::kStoreStageBytes);
-                tma_load_2d(stg2, &map_r, &res_bar[half], (nmn % num_n) * BN + ns * 64, (nmn / num_n) * kTM + rank * kBM,
-                            kEvictFirst);
-              }
-            }
-          }
-          // both 32-column halves of the sub-tile leave TMEM before the first is touched: one exposed TMEM latency per
-          // 64 columns, and two independent instruction streams for the scheduler
-          uint32_t rr[2][32];
-          tmem_ld_32x32b_x32(tacc + sc * 64, rr[0]);
-          tmem_ld_32x32b_x32(tacc + sc * 64 + 32, rr[1]);
-          tmem_ld_wait();
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[hh][j]);
-            const int col0 = colS + hh * 32;
-            const int ncols = max(0, min(32, p.N - col0));
-            if (p.aux_out) {  // GELU with a saved pre-activation: bias only here; the activation follows the aux store
-              if (p.bias != nullptr) add_bias32(v, bias_sm + (col0 - n0));
-            } else if (ncols > 0) {
-              epi_math(p, v, row, col0, ncols, ln_mean, ln_rstd, bias_sm + (col0 - n0), aux_in);
-            }
-            if (aux_in) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const int w0 = (hh * 4 + q) * 4;
-                const float2 a0 = unpack2(ain[w0], p.out_dtype), a1 = unpack2(ain[w0 + 1], p.out_dtype);
-                const float2 a2 = unpack2(ain[w0 + 2], p.out_dtype), a3 = unpack2(ain[w0 + 3], p.out_dtype);
-                if (p.epilogue == VDK_EPI_SCALE_RESIDUAL) {
-                  v[q * 8] += a0.x; v[q * 8 + 1] += a0.y; v[q * 8 + 2] += a1.x; v[q * 8 + 3] += a1.y;
-                  v[q * 8 + 4] += a2.x; v[q * 8 + 5] += a2.y; v[q * 8 + 6] += a3.x; v[q * 8 + 7] += a3.y;
-                } else {
-                  const float2 g0 = gelu_grad_pair(a0.x, a0.y), g1 = gelu_grad_pair(a1.x, a1.y);
-                  const float2 g2 = gelu_grad_pair(a2.x, a2.y), g3 = gelu_grad_pair(a3.x, a3.y);
-                  v[q * 8] *= g0.x; v[q * 8 + 1] *= g0.y; v[q * 8 + 2] *= g1.x; v[q * 8 + 3] *= g1.y;
-                  v[q * 8 + 4] *= g2.x; v[q * 8 + 5] *= g2.y; v[q * 8 + 6] *= g3.x; v[q * 8 + 7] *= g3.y;
-                }
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) packed[hh * 16 + (j >> 1)] = pack2(v[j], v[j + 1], p.out_dtype);
-          }
-          if (p.aux_out) {
-            // bulk groups of the leader alternate aux, main, aux, main ...: "at most one pending" means the previous
-            // store out of the buffer about to be rewritten has been read
-            if (stores_issued) {
-              if (leader) tma_store_wait_read<1>();
-              named_bar_sync(1 + half, 128);
-            }
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              *reinterpret_cast<uint4*>(stg2 + rit * 128 + ((q ^ (rit & 7)) << 4)) =
-                  make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-            fence_proxy_async_smem();
-            named_bar_sync(1 + half, 128);
-            if (leader) {
-              tma_store_2d(&map_d2, stg2, colS, m0);
-              tma_store_commit();
-            }
-            // the activation is applied to the ROUNDED pre-activation (what the backward will see, and what autocast's
-            // 16-bit Linear output hands to nn.GELU)
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              float2 a = unpack2(packed[i], p.out_dtype);
-              gelu_pair(a.x, a.y);
-              packed[i] = pack2(a.x, a.y, p.out_dtype);
-            }
-          }
-          if (stores_issued) {  // the previous output sub-tile must have been read out of `stg`
-            if (leader) {
-              if (p.aux_out) tma_store_wait_read<1>();
-              else tma_store_wait_read<0>();
-            }
-            named_bar_sync(1 + half, 128);
-          }
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<uint4*>(stg + rit * 128 + ((q ^ (rit & 7)) << 4)) =
-                make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-          fence_proxy_async_smem();
-          named_bar_sync(1 + half, 128);
-          if (leader) {
-            tma_store_2d(&map_d, stg, colS, m0);
-            tma_store_commit();
-          }
-          stores_issued = true;
-        }
-      } else if (p.tma_store) {
-        // 16-bit outputs: each half stages 128 x 64 sub-tiles (128-byte rows, 128B swizzle) and one thread hands
-        // them to TMA, so global memory sees full-line stores instead of 32 row-strided 16-byte pieces per warp
-        uint8_t* stg = smem_store + half * Cfg::kStoreStageBytes;
-        const bool leader = threadIdx.x == 64 + half * 128;
-        const int rit = lane_base + lane;  // row inside the tile
-#pragma unroll 1
-        for (int sc = half; sc < BN / 64; sc += 2) {
-          const int colS = n0 + sc * 64;
-          if (colS >= p.N) break;
-          uint32_t packed[32];
-          // auxiliary INPUT tile (residual to add, or the saved pre-activation whose GELU' scales the gradient): fetched
-          // by TMA into the staging buffer (full-line reads instead of 32 row-strided 16-byte loads per warp)
-          const bool aux_in = p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD;
-          if (aux_in) {
-            if (leader) {
-              if (stores_issued) tma_store_wait_read<0>();
-              mbar_arrive_expect_tx(&res_bar[half], Cfg::kStoreStageBytes);
-              tma_load_2d(stg, &map_r, &res_bar[half], colS, m0, kEvictFirst);
-            }
-          }
-          // both 32-column halves of the sub-tile leave TMEM before the first is touched: one exposed TMEM latency per
-          // 64 columns, and two independent instruction streams for the scheduler
-          uint32_t rr[2][32];
-          tmem_ld_32x32b_x32(tacc + sc * 64, rr[0]);
-          tmem_ld_32x32b_x32(tacc + sc * 64 + 32, rr[1]);
-          tmem_ld_wait();
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(rr[hh][j]);
-            const int col0 = colS + hh * 32;
-            const int ncols = max(0, min(32, p.N - col0));
-            if (p.aux_out) {  // GELU with a saved pre-activation: bias only here; the activation follows the aux store
-              if (p.bias != nullptr) add_bias32(v, bias_sm + (col0 - n0));
-            } else if (ncols > 0) {
-              epi_math(p, v, row, col0, ncols, ln_mean, ln_rstd, bias_sm + (col0 - n0), aux_in);
-            }
-            if (aux_in) {
-              if (hh == 0) {
-                mbar_wait(&res_bar[half], res_phase);
-                res_phase ^= 1;
-              }
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const uint4 t = *reinterpret_cast<const uint4*>(stg + rit * 128 + (((hh * 4 + q) ^ (rit & 7)) << 4));
-                const float2 a0 = unpack2(t.x, p.out_dtype), a1 = unpack2(t.y, p.out_dtype);
-                const float2 a2 = unpack2(t.z, p.out_dtype), a3 = unpack2(t.w, p.out_dtype);
-                if (p.epilogue == VDK_EPI_SCALE_RESIDUAL) {
-                  v[q * 8] += a0.x; v[q * 8 + 1] += a0.y; v[q * 8 + 2] += a1.x; v[q * 8 + 3] += a1.y;
-                  v[q * 8 + 4] += a2.x; v[q * 8 + 5] += a2.y; v[q * 8 + 6] += a3.x; v[q * 8 + 7] += a3.y;
-                } else {
-                  const float2 g0 = gelu_grad_pair(a0.x, a0.y), g1 = gelu_grad_pair(a1.x, a1.y);
-                  const float2 g2 = gelu_grad_pair(a2.x, a2.y), g3 = gelu_grad_pair(a3.x, a3.y);
-                  v[q * 8] *= g0.x; v[q * 8 + 1] *= g0.y; v[q * 8 + 2] *= g1.x; v[q * 8 + 3] *= g1.y;
-                  v[q * 8 + 4] *= g2.x; v[q * 8 + 5] *= g2.y; v[q * 8 + 6] *= g3.x; v[q * 8 + 7] *= g3.y;
-                }
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) packed[hh * 16 + (j >> 1)] = pack2(v[j], v[j + 1], p.out_dtype);
-          }
-          if (p.aux_out) {  // first the pre-activation copy, through the same staging buffer
-            if (stores_issued) {
-              if (leader) tma_store_wait_read<0>();
-              named_bar_sync(1 + half, 128);
-            }
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              *reinterpret_cast<uint4*>(stg + rit * 128 + ((q ^ (rit & 7)) << 4)) =
-                  make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-            fence_proxy_async_smem();
-            named_bar_sync(1 + half, 128);
-            if (leader) {
-              tma_store_2d(&map_d2, stg, colS, m0);
-              tma_store_commit();
-            }
-            stores_issued = true;
-            // the activation is applied to the ROUNDED pre-activation (what the backward will see, and what autocast's
-            // 16-bit Linear output hands to nn.GELU) while TMA drains the staging buffer
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              float2 a = unpack2(packed[i], p.out_dtype);
-              gelu_pair(a.x, a.y);
-              packed[i] = pack2(a.x, a.y, p.out_dtype);
-            }
-          }
-          if (stores_issued && !aux_in) {  // the previous sub-tile must have been read out of the staging buffer
-            if (leader) tma_store_wait_read<0>();
-            named_bar_sync(1 + half, 128);
-          }
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<uint4*>(stg + rit * 128 + ((q ^ (rit & 7)) << 4)) =
-                make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-          fence_proxy_async_smem();
-          named_bar_sync(1 + half, 128);
-          if (leader) {
-            tma_store_2d(&map_d, stg, colS, m0);
-            tma_store_commit();
-          }
-          stores_issued = true;
-        }
-      } else {
-#pragma unroll 1
-        for (int c = half; c < BN / 32; c += 2) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(tacc + c * 32, r);
-          tmem_ld_wait();
-          const int col0 = n0 + c * 32;
-          if (row < p.M && col0 < p.N && p.partial_out) {
-            // split-K: raw fp32 partial sums.  With a slab stride every split owns its own copy of D (plain stores,
-            // the consumer adds the slabs in a fixed order: deterministic); otherwise they are atomically added
-            // into a D the caller zeroed.
-            const int ncols = min(32, p.N - col0);
-            if (p.split_stride > 0) {
-              float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(tile / (num_m * num_n)) * p.split_stride +
-                           static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                if (j < ncols)
-                  *reinterpret_cast<float4*>(out + j) = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                                    __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-            } else {
-              float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (j < ncols) atomicAdd(out + j, __uint_as_float(r[j]));
-            }
-          } else if (row < p.M && col0 < p.N) {
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-            const int ncols = min(32, p.N - col0);  // multiple of 8 (N % 8 == 0 is required)
-            epi_math(p, v, row, col0, ncols, ln_mean, ln_rstd, bias_sm + (col0 - n0));
-            if (p.out_dtype == VDK_DTYPE_FP32) {
-              float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                if (j < ncols) *reinterpret_cast<float4*>(out + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            } else {
-              uint16_t* out = reinterpret_cast<uint16_t*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                if (j < ncols) {
-                  uint4 t;
-                  t.x = pack2(v[j], v[j + 1], p.out_dtype);
-                  t.y = pack2(v[j + 2], v[j + 3], p.out_dtype);
-                  t.z = pack2(v[j + 4], v[j + 5], p.out_dtype);
-                  t.w = pack2(v[j + 6], v[j + 7], p.out_dtype);
-                  *reinterpret_cast<uint4*>(out + j) = t;
-                }
-              }
-            }
-          }
+        wgmma_commit();
+        // the previous stage's MMAs have retired once at most this one is pending: its slot may be refilled
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
         }
       }
-      tc_fence_before();
-      if (kPair) {  // one arrival per warp on the LEADER's barrier (its MMA thread owns both CTAs' accumulators)
-        __syncwarp();
-        if (lane == 0) mbar_arrive_leader(&tmem_empty[acc]);
-      } else {
-        mbar_arrive(&tmem_empty[acc]);
-      }
-    }
-    if (p.tma_store && stores_issued && threadIdx.x == 64 + half * 128) tma_store_wait<0>();
-  }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 
-  tc_fence_before();
-  if (kPair) cluster_sync_all();  // neither CTA frees TMEM / exits while the pair's MMAs or remote arrivals are in flight
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (kPair) tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
-    else tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+      if (p.epilogue == VDK_EPI_LAYERNORM) {
+        // the tile spans the whole row (N <= BN): the four threads of a fragment quad hold every column of its two rows
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float sum = 0.f;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = n0 + j * 8 + fcol + e;
+              if (col < p.N) sum += acc[4 * j + 2 * r + e] + (p.bias ? __ldg(p.bias + col) : 0.f);
+            }
+          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+          const float mean = sum / static_cast<float>(p.N);
+          float sq = 0.f;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = n0 + j * 8 + fcol + e;
+              if (col < p.N) {
+                const float d = acc[4 * j + 2 * r + e] + (p.bias ? __ldg(p.bias + col) : 0.f) - mean;
+                sq = fmaf(d, d, sq);
+              }
+            }
+          sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+          sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+          if ((lane & 3) == 0) {
+            ln_sm[frow + 8 * r] = mean;
+            ln_sm[kBM + frow + 8 * r] = rsqrtf(sq / static_cast<float>(p.N) + p.ln_eps);
+          }
+        }
+      }
+      if (p.bias != nullptr && ct < BN) bias_sm[ct] = (n0 + ct < p.N) ? __ldg(p.bias + n0 + ct) : 0.f;
+      const int row = m0 + erow;
+#pragma unroll
+      for (int sc = 0; sc < BN / 64; ++sc) {
+        if (n0 + sc * 64 < p.N) {  // block-uniform
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = sc * 8 + jj;
+            *reinterpret_cast<float2*>(acc_sm + frow * kAccLd + jj * 8 + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(acc_sm + (frow + 8) * kAccLd + jj * 8 + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+          named_bar_sync(1, 256);  // the chunk (and, before the first one, the bias and LayerNorm statistics) is in smem
+          float v[32];
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 t = *reinterpret_cast<const float4*>(acc_sm + erow * kAccLd + half * 32 + j);
+            v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
+          }
+          named_bar_sync(1, 256);  // every thread holds its piece: the buffer may take the next chunk
+          const float ln_mean = p.epilogue == VDK_EPI_LAYERNORM ? ln_sm[erow] : 0.f;
+          const float ln_rstd = p.epilogue == VDK_EPI_LAYERNORM ? ln_sm[kBM + erow] : 1.f;
+          const int col0 = n0 + sc * 64 + half * 32;
+          const int ncols = min(32, p.N - col0);  // multiple of 8 (N % 8 == 0 is required)
+          if (row < p.M && ncols > 0) {
+            if (p.partial_out) {
+              // split-K: raw fp32 partial sums.  With a slab stride every split owns its own copy of D (plain stores,
+              // the consumer adds the slabs in a fixed order: deterministic); otherwise they are atomically added
+              // into a D the caller zeroed.
+              if (p.split_stride > 0) {
+                float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(split) * p.split_stride +
+                             static_cast<size_t>(row) * p.ldd + col0;
+#pragma unroll
+                for (int j = 0; j < 32; j += 4)
+                  if (j < ncols) *reinterpret_cast<float4*>(out + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+              } else {
+                float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
+#pragma unroll
+                for (int j = 0; j < 32; ++j)
+                  if (j < ncols) atomicAdd(out + j, v[j]);
+              }
+            } else {
+              if (p.aux != nullptr) {
+                // GELU with a saved pre-activation: store acc + bias, then apply the activation to the ROUNDED
+                // pre-activation (what the backward will see, and what autocast's 16-bit Linear output hands to nn.GELU)
+                if (p.bias != nullptr) add_bias32(v, bias_sm + (col0 - n0));
+                uint16_t* aux = reinterpret_cast<uint16_t*>(p.aux) + static_cast<size_t>(row) * p.ldd + col0;
+#pragma unroll
+                for (int j = 0; j < 32; j += 8) {
+                  if (j < ncols) {
+                    uint4 t;
+                    t.x = pack2(v[j], v[j + 1], p.out_dtype);
+                    t.y = pack2(v[j + 2], v[j + 3], p.out_dtype);
+                    t.z = pack2(v[j + 4], v[j + 5], p.out_dtype);
+                    t.w = pack2(v[j + 6], v[j + 7], p.out_dtype);
+                    *reinterpret_cast<uint4*>(aux + j) = t;
+                  }
+                }
+#pragma unroll
+                for (int j = 0; j < 32; j += 2) {
+                  float2 a = unpack2(pack2(v[j], v[j + 1], p.out_dtype), p.out_dtype);
+                  gelu_pair(a.x, a.y);
+                  v[j] = a.x;
+                  v[j + 1] = a.y;
+                }
+              } else {
+                epi_math(p, v, row, col0, ncols, ln_mean, ln_rstd, bias_sm + (col0 - n0));
+              }
+              if (p.out_dtype == VDK_DTYPE_FP32) {
+                float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
+#pragma unroll
+                for (int j = 0; j < 32; j += 4)
+                  if (j < ncols) *reinterpret_cast<float4*>(out + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+              } else {
+                uint16_t* out = reinterpret_cast<uint16_t*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
+#pragma unroll
+                for (int j = 0; j < 32; j += 8) {
+                  if (j < ncols) {
+                    uint4 t;
+                    t.x = pack2(v[j], v[j + 1], p.out_dtype);
+                    t.y = pack2(v[j + 2], v[j + 3], p.out_dtype);
+                    t.z = pack2(v[j + 4], v[j + 5], p.out_dtype);
+                    t.w = pack2(v[j + 6], v[j + 7], p.out_dtype);
+                    *reinterpret_cast<uint4*>(out + j) = t;
+                  }
+                }
+              }
+            }
+          }
+        }
+      }
+      named_bar_sync(1, 256);  // bias and LayerNorm statistics of this tile are consumed
+    }
   }
 }
 
-template <int BN, bool kBf16, bool kAux, bool kPair>
-static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md, const CUtensorMap& mr,
-                       const CUtensorMap& md2, const GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
-  constexpr int kStageBytes = Cfg::kStageA + (kPair ? Cfg::kStageB / 2 : Cfg::kStageB);
-  constexpr int kStages = kPair ? (kAux ? 5 : 6) : Cfg::kStages - (kAux ? 1 : 0);
-  constexpr int kSmem = kStages * kStageBytes + (kAux ? 4 : 2) * Cfg::kStoreStageBytes + (2 * kStages + 6) * 8 + 16 + BN * 4 + 1024;
-  static_assert(kSmem <= 227 * 1024, "GEMM shared memory budget");
-  auto kern = gemm_tn_kernel<BN, kBf16, kAux, kPair>;
-  static bool attr_set = false;  // per (BN, dtype, variant) instantiation
+template <int BN, bool kBf16, int kTA, int kTB>
+static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, cudaStream_t stream) {
+  constexpr int kSmem = GemmCfg<BN>::kSmemBytes;
+  auto kern = gemm_tn_kernel<BN, kBf16, kTA, kTB>;
+  static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
     attr_set = true;
   }
-  const int tm = kPair ? 2 * kBM : kBM;
-  const int num_tiles = ((p.M + tm - 1) / tm) * ((p.N + BN - 1) / BN) * p.split_k;
-  if (kPair) {
-    const int pairs = std::min(num_tiles, sm_count() / 2);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * pairs);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = kSmem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    VDK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, ma, mb, md, mr, md2, p));
-    return VDK_OK;
-  }
+  const int num_tiles = ((p.M + kBM - 1) / kBM) * ((p.N + BN - 1) / BN) * p.split_k;
   const int grid = num_tiles < sm_count() ? num_tiles : sm_count();
-  kern<<<grid, kGemmThreads, kSmem, stream>>>(ma, mb, md, mr, md2, p);
+  kern<<<grid, kGemmThreads, kSmem, stream>>>(ma, mb, p);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
+}
+
+template <int BN, bool kBf16>
+static int launch_gemm_major(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, bool ta, bool tb,
+                             cudaStream_t s) {
+  if (ta) return tb ? launch_gemm<BN, kBf16, 1, 1>(ma, mb, p, s) : launch_gemm<BN, kBf16, 1, 0>(ma, mb, p, s);
+  return tb ? launch_gemm<BN, kBf16, 0, 1>(ma, mb, p, s) : launch_gemm<BN, kBf16, 0, 0>(ma, mb, p, s);
 }
 
 }  // namespace vdk
@@ -818,7 +518,7 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
                 "vdk_gemm: split_k > 1 needs fp32 output, no bias and no epilogue (partials are atomically added)");
 
   // LayerNorm needs the whole row in one tile; otherwise narrow outputs use 128-column tiles (more tiles to
-  // balance over 148 SMs) and wide ones 256.
+  // balance over 132 SMs) and wide ones 256.
   bool wide = (g.N % 256 == 0) || g.N > 512;
   if (g.epilogue == VDK_EPI_LAYERNORM) wide = g.N > 128;
   const int BN = wide ? 256 : 128;
@@ -828,37 +528,16 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   int rc = g.trans_a ? make_tma_2d_16bit(&ma, g.A, (uint64_t)g.K, (uint64_t)g.M, (uint64_t)g.lda, kBK, 64)
                      : make_tma_2d_16bit(&ma, g.A, (uint64_t)g.M, (uint64_t)g.K, (uint64_t)g.lda, kBM, kBK);
   if (rc != VDK_OK) return rc;
-  // CTA pairs (one UMMA of M = 256 per 2-cluster) for the wide tile whenever there are at least two row blocks
-  static const int pair_mode = [] {
-    const char* e = getenv("VDK_GEMM_PAIR");
-    return e ? atoi(e) : 1;
-  }();
-  // VDK_GEMM_PAIR: 0 never, 2 whenever possible, 1 (default) where it measured faster at ConvNeXt-B shapes: long K loops
-  // over many row blocks (+4..5 %); short-K GEMMs are paced by their epilogue and lose 2..5 % to the pair's barriers
-  const bool pair = wide && g.M > kBM && (pair_mode == 2 || (pair_mode == 1 && g.K >= 1024 && g.M >= 16384));
   rc = g.trans_b ? make_tma_2d_16bit(&mb, g.B, (uint64_t)g.K, (uint64_t)g.N, (uint64_t)g.ldb, kBK, 64)
-                 : make_tma_2d_16bit(&mb, g.B, (uint64_t)g.N, (uint64_t)g.K, (uint64_t)g.ldb, pair ? BN / 2 : BN, kBK);
+                 : make_tma_2d_16bit(&mb, g.B, (uint64_t)g.N, (uint64_t)g.K, (uint64_t)g.ldb, BN, kBK);
   if (rc != VDK_OK) return rc;
-  const int tma_store = (g.out_dtype != VDK_DTYPE_FP32 && g.split_k <= 1) ? 1 : 0;
-  CUtensorMap md = ma;  // placeholder when unused
-  if (tma_store) {
-    rc = make_tma_2d_16bit(&md, g.D, (uint64_t)g.M, (uint64_t)g.N, (uint64_t)g.ldd, kBM, 64);
-    if (rc != VDK_OK) return rc;
-  }
-  CUtensorMap mr = md, md2 = md;
-  if (tma_store && (g.epilogue == VDK_EPI_SCALE_RESIDUAL || g.epilogue == VDK_EPI_MUL_GELU_GRAD)) {
-    rc = make_tma_2d_16bit(&mr, g.residual, (uint64_t)g.M, (uint64_t)g.N, (uint64_t)g.ldr, kBM, 64);
-    if (rc != VDK_OK) return rc;
-  }
-  const int aux_out = (g.aux_out != nullptr) ? 1 : 0;
-  if (aux_out) {
-    VDK_REQUIRE(tma_store && g.epilogue == VDK_EPI_GELU, "vdk_gemm: aux_out needs the GELU epilogue and a 16-bit output");
-    rc = make_tma_2d_16bit(&md2, g.aux_out, (uint64_t)g.M, (uint64_t)g.N, (uint64_t)g.ldd, kBM, 64);
-    if (rc != VDK_OK) return rc;
+  if (g.aux_out != nullptr) {
+    VDK_REQUIRE(g.out_dtype != VDK_DTYPE_FP32 && g.split_k <= 1 && g.epilogue == VDK_EPI_GELU,
+                "vdk_gemm: aux_out needs the GELU epilogue and a 16-bit output");
+    VDK_REQUIRE((reinterpret_cast<uintptr_t>(g.aux_out) & 15) == 0, "vdk_gemm: aux_out must be 16-byte aligned");
   }
   GemmParams p{g.M, g.N, g.K, g.D, g.ldd, g.bias, g.gamma, g.beta, g.residual, g.ldr, g.out_dtype, g.epilogue,
-               g.ln_eps, split, tma_store, g.trans_a ? 1 : 0, g.trans_b ? 1 : 0, g.split_k > 1 ? (long long)g.split_stride : 0ll,
-               aux_out, (g.split_k > 1) ? 1 : 0};
+               g.ln_eps, split, g.split_k > 1 ? (long long)g.split_stride : 0ll, g.aux_out, (g.split_k > 1) ? 1 : 0};
   const bool bf = g.in_dtype == VDK_DTYPE_BF16;
   // algorithmic bytes: both operands once, the output once (x2 for an auxiliary 16-bit output), a 16-bit residual / saved tile once
   const double osz = g.out_dtype == VDK_DTYPE_FP32 ? 4.0 : 2.0;
@@ -866,26 +545,9 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
                  2.0 * (static_cast<double>(g.M) * g.K + static_cast<double>(g.N) * g.K) + osz * g.M * g.N * (g.split_k > 1 ? split : 1) +
                      (g.aux_out ? 2.0 * g.M * g.N : 0.0) + (g.residual ? osz * g.M * g.N : 0.0),
                  s);
-  // which epilogues take the pipelined auxiliary-tile variant (VDK_GEMM_AUXPIPE: bit 0 aux_out, bit 1 MUL_GELU_GRAD,
-  // bit 2 SCALE_RESIDUAL; a tuning switch.  Measured at ConvNeXt-B
-  // shapes: the GELU' data gradient gains 24 %, the layer-scale + residual GEMM (K = 4C: mainloop-bound) loses 8 % to the
-  // missing stage, so the default is 3)
-  static const int aux_mask = [] {
-    const char* e = getenv("VDK_GEMM_AUXPIPE");
-    return e ? atoi(e) : 3;
-  }();
-  const bool aux = tma_store && ((aux_out && (aux_mask & 1)) || (g.epilogue == VDK_EPI_MUL_GELU_GRAD && (aux_mask & 2)) ||
-                                 (g.epilogue == VDK_EPI_SCALE_RESIDUAL && (aux_mask & 4)));
-  if (pair) {
-    if (aux) return bf ? launch_gemm<256, true, true, true>(ma, mb, md, mr, md2, p, s) : launch_gemm<256, false, true, true>(ma, mb, md, mr, md2, p, s);
-    return bf ? launch_gemm<256, true, false, true>(ma, mb, md, mr, md2, p, s) : launch_gemm<256, false, false, true>(ma, mb, md, mr, md2, p, s);
-  }
-  if (aux) {
-    if (wide) return bf ? launch_gemm<256, true, true, false>(ma, mb, md, mr, md2, p, s) : launch_gemm<256, false, true, false>(ma, mb, md, mr, md2, p, s);
-    return bf ? launch_gemm<128, true, true, false>(ma, mb, md, mr, md2, p, s) : launch_gemm<128, false, true, false>(ma, mb, md, mr, md2, p, s);
-  }
-  if (wide) return bf ? launch_gemm<256, true, false, false>(ma, mb, md, mr, md2, p, s) : launch_gemm<256, false, false, false>(ma, mb, md, mr, md2, p, s);
-  return bf ? launch_gemm<128, true, false, false>(ma, mb, md, mr, md2, p, s) : launch_gemm<128, false, false, false>(ma, mb, md, mr, md2, p, s);
+  const bool ta = g.trans_a != 0, tb = g.trans_b != 0;
+  if (wide) return bf ? launch_gemm_major<256, true>(ma, mb, p, ta, tb, s) : launch_gemm_major<256, false>(ma, mb, p, ta, tb, s);
+  return bf ? launch_gemm_major<128, true>(ma, mb, p, ta, tb, s) : launch_gemm_major<128, false>(ma, mb, p, ta, tb, s);
 }
 
 }  // namespace vdk

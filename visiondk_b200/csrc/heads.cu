@@ -7,7 +7,7 @@
 // and their autograd backward.
 //
 // The reference runs this path in fp32 (no autocast, train.py:227).  The class-logit contraction cos = f~ . W~ and the
-// two gradient contractions run on the tcgen05 GEMM with a 3-way bf16 split of every fp32 operand
+// two gradient contractions run on the wgmma GEMM with a 3-way bf16 split of every fp32 operand
 // (x = p0 + p1 + p2, 8 mantissa bits each; the six products with i + j <= 2 are laid side by side along K), which
 // reproduces fp32 accuracy (~2^-22 relative) on 16-bit tensor cores.  Everything else (row/column normalisation,
 // margins, online softmax, the normalisation backward) is fused into a few HBM-bound kernels.
@@ -392,7 +392,7 @@ static int split_gemm(const __nv_bfloat16* a, const __nv_bfloat16* b, float* d, 
   return gemm_run(g, s);
 }
 
-static int blocks_for(int64_t n, int per_block) { return static_cast<int>(std::min<int64_t>((n + per_block - 1) / per_block, 148 * 32)); }
+static int blocks_for(int64_t n, int per_block) { return static_cast<int>(std::min<int64_t>((n + per_block - 1) / per_block, 132 * 32)); }
 
 // cos = normalize(f) . normalize(W, dim 0) into ws.cosm (pitch Cp); also fills inv_f, inv_w, fn
 static int head_cos(const vdk_head_desc* d, const float* feats, const float* weight, const HeadWs& w, cudaStream_t s) {

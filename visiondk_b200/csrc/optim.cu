@@ -12,7 +12,7 @@
 namespace vdk {
 
 constexpr int kRedThreads = 256;
-constexpr int kRedBlocksMax = 1184;  // 8 x 148
+constexpr int kRedBlocksMax = 1184;  // fixed partial count: the order of the final sum does not depend on the device
 
 __global__ void __launch_bounds__(kRedThreads) sumsq_partial_kernel(const float* __restrict__ g, int64_t n,
                                                                      double* __restrict__ partial) {
@@ -119,7 +119,7 @@ extern "C" int vdk_sgd_clip_ema_step(float* params, float* grads, float* momentu
   if (n == 0) return VDK_OK;
   StepArgs a{params, grads, momentum_buf, ema, n, total_sumsq, max_norm, lr, momentum, weight_decay, ema_decay,
              ema_one_minus_decay, first_step, zero_grad};
-  const int blocks = static_cast<int>(std::min<int64_t>((n + 255) / 256, 148 * 16));
+  const int blocks = static_cast<int>(std::min<int64_t>((n + 255) / 256, 132 * 16));
   sgd_clip_ema_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
@@ -128,7 +128,7 @@ extern "C" int vdk_sgd_clip_ema_step(float* params, float* grads, float* momentu
 extern "C" int vdk_ema_update(float* ema, const float* src, int64_t n, float decay, float one_minus_decay, void* stream) {
   VDK_REQUIRE(ema && src && n >= 0, "vdk_ema_update: null operand");
   if (n == 0) return VDK_OK;
-  const int blocks = static_cast<int>(std::min<int64_t>((n + 255) / 256, 148 * 16));
+  const int blocks = static_cast<int>(std::min<int64_t>((n + 255) / 256, 132 * 16));
   ema_only_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(ema, src, n, decay, one_minus_decay);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;

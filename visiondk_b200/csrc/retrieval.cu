@@ -5,8 +5,8 @@
 //
 // Pipeline (all on device, nothing leaves HBM):
 //   rows_prepare   fp32 rows -> canonical unit rows (fp32) + fp16 copy + per-row rounding-error norm
-//   score_filter   fp16 tcgen05 GEMM of a 128-query tile (resident in smem) against streamed gallery tiles;
-//                  the epilogue never writes the score matrix: each thread owns one query row in TMEM and
+//   score_filter   fp16 wgmma GEMM of a 128-query tile (resident in smem) against streamed gallery tiles;
+//                  the epilogue never writes the score matrix: each thread owns one query row of a staged chunk and
 //                  appends only scores >= tau[row] to a segment of that row's candidate list that this CTA
 //                  owns exclusively (plain stores, a register counter — no atomics on the scan path)
 //   select         per query: k-th largest approximate score A_k (radix select), keep a >= A_k - 2*eps
@@ -96,17 +96,18 @@ __global__ void reduce_max_kernel(const float* __restrict__ x, int64_t n, float*
 }
 
 // ------------------------------------------------------------------------------------------------
-// score_filter: fp16 tcgen05 GEMM with a threshold-filter epilogue
+// score_filter: fp16 wgmma GEMM with a threshold-filter epilogue
 // ------------------------------------------------------------------------------------------------
-constexpr int kQM = 128;          // queries per tile (TMEM lanes)
-constexpr int kGN = 256;          // gallery rows per tile (UMMA N)
+constexpr int kQM = 128;          // queries per tile (two consumer warpgroups of 64 rows)
+constexpr int kGN = 256;          // gallery rows per tile (wgmma N)
 constexpr int kSBK = 64;          // K per smem block (128-byte swizzle row of fp16)
 constexpr int kQBlockBytes = kQM * kSBK * 2;   // 16 KB
 constexpr int kGStageBytes = kGN * kSBK * 2;   // 32 KB
-constexpr int kGStages = 3;
-constexpr int kScoreThreads = 320;  // TMA warp, MMA warp, 8 epilogue warps
+constexpr int kGStages = 2;       // with a resident 512-dim query tile (128 KB) two gallery stages fit beside the staging buffer
+constexpr int kScoreThreads = 384;  // producer warpgroup, two consumer warpgroups
+constexpr int kStageLd = 64 + 1;  // fp32 pitch of the staged 128 x 64 score chunk (odd: conflict-free row reads)
 constexpr int kMaxKB = 8;         // dim <= 512
-constexpr int kMaxSeg = 32;       // candidate segments per query = 2 x gallery splits per range (two epilogue warps per row)
+constexpr int kMaxSeg = 32;       // candidate segments per query = 2 x gallery splits per range (two epilogue threads per row)
 
 struct ScoreParams {
   int n_query;
@@ -121,7 +122,7 @@ struct ScoreParams {
 };
 
 static int score_smem_bytes(int num_kb) {
-  return num_kb * kQBlockBytes + kGStages * kGStageBytes + (2 * kGStages + 6) * 8 + 16 + 1024;
+  return num_kb * kQBlockBytes + kGStages * kGStageBytes + kQM * kStageLd * 4 + (2 * kGStages + 2) * 8 + 1024;
 }
 
 template <bool kDense>
@@ -134,42 +135,31 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_q = smem;
   uint8_t* smem_g = smem + p.num_kb * kQBlockBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_g + kGStages * kGStageBytes);
+  uint32_t* stage_sm = reinterpret_cast<uint32_t*>(smem_g + kGStages * kGStageBytes);  // [128][kStageLd] score bits
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_sm + kQM * kStageLd);  // 128 x 65 words: 8-byte aligned
   uint64_t* empty_bar = full_bar + kGStages;
-  uint64_t* tmem_full = empty_bar + kGStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint64_t* q_full = tmem_empty + 2;
+  uint64_t* q_full = empty_bar + kGStages;
   uint64_t* q_empty = q_full + 1;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(q_empty + 1);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   const int n_units = p.n_qtiles * p.n_splits;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tensormap(&map_q);
     prefetch_tensormap(&map_g);
     for (int i = 0; i < kGStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 256);
+      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
     mbar_init(q_full, 1);
-    mbar_init(q_empty, 1);
+    mbar_init(q_empty, 8);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0, uphase = 0;
       for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
@@ -178,7 +168,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
         if (t0 >= t1) continue;
         // the query tile stays resident for the whole unit
-        mbar_wait(q_empty, uphase ^ 1);
+        mbar_wait<true>(q_empty, uphase ^ 1);
         mbar_arrive_expect_tx(q_full, p.num_kb * kQBlockBytes);
         for (int kb = 0; kb < p.num_kb; ++kb)
           tma_load_2d(smem_q + kb * kQBlockBytes, &map_q, q_full, kb * kSBK, qt * kQM, kEvictLast);
@@ -186,7 +176,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         for (int t = t0; t < t1; ++t) {
           const int grow = static_cast<int>(p.g_lo) + t * kGN;
           for (int kb = 0; kb < p.num_kb; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_wait<true>(&empty_bar[stage], phase ^ 1);
             mbar_arrive_expect_tx(&full_bar[stage], kGStageBytes);
             tma_load_2d(smem_g + stage * kGStageBytes, &map_g, &full_bar[stage], kb * kSBK, grow, kEvictNormal);
             if (++stage == kGStages) {
@@ -197,75 +187,75 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16<false>(kQM, kGN);
-      int stage = 0, it = 0;
-      uint32_t phase = 0, uphase = 0;
-      for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        const int sp = u / p.n_qtiles;
-        const int t0 = sp * p.tiles_per_split;
-        const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-        if (t0 >= t1) continue;
-        mbar_wait(q_full, uphase);
-        uphase ^= 1;
-        tc_fence_after();
-        for (int t = t0; t < t1; ++t, ++it) {
-          const int acc = it & 1;
-          mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + acc * kGN;
-          for (int kb = 0; kb < p.num_kb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint64_t da = umma_desc_k_sw128(smem_u32(smem_q + kb * kQBlockBytes));
-            const uint64_t db = umma_desc_k_sw128(smem_u32(smem_g + stage * kGStageBytes));
-#pragma unroll
-            for (int k = 0; k < kSBK / 16; ++k)
-              umma_f16_ss(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_commit(&empty_bar[stage]);
-            if (++stage == kGStages) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-          umma_commit(&tmem_full[acc]);
-        }
-        umma_commit(q_empty);  // query tile may be overwritten once every MMA of this unit has retired
-      }
-    }
   } else {
-    // ===================== epilogue: one query row per TMEM lane =====================
-    // Eight warps: two per TMEM lane quarter, taking alternate 32-column chunks (two warps per scheduler hide
-    // each other's TMEM-load and ALU latency).  Each (row, split, half) has exactly one writer thread.
-    const int lane_base = (warp & 3) * 32;
-    const int half = (warp - 2) >> 2;
-    int it = 0;
+    // ===================== consumers: scores of 64 query rows each, then the filter =====================
+    // The accumulator leaves the registers in 64-column chunks through shared memory; thread (row, half) then examines 32
+    // consecutive gallery columns of one query row, so each (row, split, half) has exactly one writer thread.
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int ct = threadIdx.x - 128;
+    const int cg = ct >> 7;
+    const int wl = (ct >> 5) & 3, lane = ct & 31;
+    const int frow = cg * 64 + wl * 16 + (lane >> 2);
+    const int fcol = (lane & 3) * 2;
+    const int erow = ct & 127, half = ct >> 7;
+    int stage = 0;
+    uint32_t phase = 0, uphase = 0;
+    float acc[kGN / 2];
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
       const int qt = u % p.n_qtiles, sp = u / p.n_qtiles;
       const int t0 = sp * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
       if (t0 >= t1) continue;
-      const int row = qt * kQM + lane_base + lane;
+      mbar_wait<true>(q_full, uphase);
+      uphase ^= 1;
+      const int row = qt * kQM + erow;
       const bool row_ok = row < p.n_query;
       float tau = INFINITY;
       if (!kDense && row_ok) tau = p.tau[row];
       uint2* seg = p.seg + static_cast<size_t>(row_ok ? row : 0) * p.seg_stride + (kDense ? 0 : (sp * 2 + half) * p.seg_cap);
       unsigned cnt = 0;
-      for (int t = t0; t < t1; ++t, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&tmem_full[acc], (it >> 1) & 1);
-        tc_fence_after();
+      for (int t = t0; t < t1; ++t) {
+        int prev = -1;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait<true>(&full_bar[stage], phase);
+          const uint64_t da = wgmma_desc_k_sw128(smem_u32(smem_q + kb * kQBlockBytes) + cg * 8192);
+          const uint64_t db = wgmma_desc_k_sw128(smem_u32(smem_g + stage * kGStageBytes));
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kSBK / 16; ++k)
+            wgmma_m64n256k16_ss<false, 0, 0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == kGStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (lane == 0) {
+          mbar_arrive(&empty_bar[prev]);
+          if (t + 1 == t1) mbar_arrive(q_empty);  // every MMA of this unit has retired: the query tile may be overwritten
+        }
         const int64_t gbase = p.g_lo + static_cast<int64_t>(t) * kGN;
-        const uint32_t tacc = tmem_base + (static_cast<uint32_t>(lane_base) << 16) + acc * kGN;
-        uint32_t r[32], rn[32];
-        tmem_ld_32x32b_x32(tacc + half * 32, r);
-#pragma unroll 1
-        for (int c = half; c < kGN / 32; c += 2) {
-          tmem_ld_wait();
-          // prefetch this warp's next chunk while the current one is examined
-          if (c + 2 < kGN / 32) tmem_ld_32x32b_x32(tacc + (c + 2) * 32, rn);
+#pragma unroll
+        for (int cc = 0; cc < kGN / 64; ++cc) {
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = cc * 8 + jj;
+            stage_sm[frow * kStageLd + jj * 8 + fcol] = __float_as_uint(acc[4 * j]);
+            stage_sm[frow * kStageLd + jj * 8 + fcol + 1] = __float_as_uint(acc[4 * j + 1]);
+            stage_sm[(frow + 8) * kStageLd + jj * 8 + fcol] = __float_as_uint(acc[4 * j + 2]);
+            stage_sm[(frow + 8) * kStageLd + jj * 8 + fcol + 1] = __float_as_uint(acc[4 * j + 3]);
+          }
+          named_bar_sync(1, 256);
+          uint32_t r[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) r[j] = stage_sm[erow * kStageLd + half * 32 + j];
+          named_bar_sync(1, 256);  // the staging buffer may take the next chunk
+          const int c = cc * 2 + half;  // 32-column chunk of the tile
           const int64_t g0 = gbase + c * 32;
           if (kDense) {
             if (row_ok && g0 < p.g_hi) {
@@ -311,21 +301,10 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
               }
             }
           }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = rn[j];
         }
-        tc_fence_before();
-        mbar_arrive(&tmem_empty[acc]);
       }
       if (!kDense && row_ok) p.seg_cnt[static_cast<size_t>(row) * kMaxSeg + sp * 2 + half] = cnt;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -362,8 +341,7 @@ struct SelectParams {
 constexpr int kSelStage = 4096;
 
 // kPre: the prefilter of dense ranges, 1 = two sweeps over the entries, 2 = entries held in registers (default).  Its own
-// instantiation: the 64 registers of the entry array would otherwise cut the occupancy of every sparse-range launch — measured:
-// 120 -> 225 us per sparse select.
+// instantiation: the 64 registers of the entry array would otherwise cut the occupancy of every sparse-range launch.
 template <bool kAgg, int kPre>
 __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectParams p) {
   extern __shared__ uint2 s_stage[];  // [p.stage_cap]
@@ -409,7 +387,7 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectParams 
   };
   const bool staged = n <= static_cast<unsigned>(p.stage_cap);
   // Dense range (thousands of scores per row, all of one sign and exponent: the first radix digits barely discriminate and
-  // their histogram atomics pile up on 2-3 bins — 290-430 us per launch).  Prefilter instead: thread t takes the maximum of
+  // their histogram atomics pile up on 2-3 bins).  Prefilter instead: thread t takes the maximum of
   // entries t, t + 128, ...; >= k threads hold a maximum >= F (the k-th largest of the 128 maxima), so the
   // k-th largest score of the row is >= F and only entries >= F - 2 eps can survive the select.  They (a few hundred) are
   // compacted into shared memory and the radix passes run on them.
@@ -534,7 +512,7 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectParams 
       // 30+ nearly empty lists do not cost 30+ CTA-wide loop trips
       // warp-aggregated histogram: candidate scores share sign and exponent, so the first digit of most keys falls into a
       // handful of bins — one shared-memory atomic per (warp, distinct bin) instead of one per key (the 4096-entry dense
-      // range serialised ~1000 deep on a single bin: 287 us per select)
+      // range would serialise ~1000 deep on a single bin)
       for (int l = 0; l < n_lists; ++l) {
         const unsigned c = s_cnt[l];
         if (c <= kShortList) continue;
@@ -824,7 +802,7 @@ __global__ void topk_merge_kernel(const float* __restrict__ scores, const int64_
 // shards).  Lane l of a group walks list l and holds its head as ONE 64-bit key (order-preserving score bits << 32 | ~id: larger
 // is better — score desc, id asc; 0 = list exhausted) with the next entry already loaded, so a step is log2(group) 64-bit
 // max-shuffles and the winner's register move: no load on the critical path (the general kernel above re-loads 32 heads and
-// runs a five-round three-field tournament per step: 169 us for 8 x 10 000 x 100 against ~15 us here).
+// runs a five-round three-field tournament per step).
 __global__ void __launch_bounds__(256) topk_merge_packed_kernel(const unsigned long long* __restrict__ packed, int n_lists,
                                                                 int group, int64_t n_query, int k,
                                                                 float* __restrict__ out_scores, int64_t* __restrict__ out_ids) {
@@ -1292,7 +1270,7 @@ static int topk_filter(const vdk_topk_plan* plan, const void* qh, const float* q
       sp.stage_cap = dense ? kSelStage : kSelStage / 2;
       static const int prefilter = [] {  // VDK_SELECT_PREFILTER: 0 plain staged select on dense ranges too, 1 two sweeps, 2 registers
         const char* e = getenv("VDK_SELECT_PREFILTER");
-        return e ? atoi(e) : 2;  // measured on 8 emulated shards, same box: 2.11 ms per shard (registers) / 2.19 ms (two sweeps)
+        return e ? atoi(e) : 2;
       }();
       sp.prefilter = prefilter;
       const bool pre = prefilter && dense && k <= kSelThreads;  // what is left after the prefilter needs no aggregation

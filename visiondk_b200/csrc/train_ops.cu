@@ -325,7 +325,7 @@ dwconv7_wgrad_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
   const bool active = plane < planes;
   const int hh = plane / 7, dy = plane - hh * 7;
   const int px0 = hh * kWgR;
-  float2 acc[7][2];  // channel pairs: the product loop runs on FFMA2
+  float2 acc[7][2];  // channel pairs
 #pragma unroll
   for (int dx = 0; dx < 7; ++dx) {
     acc[dx][0] = make_float2(0.f, 0.f);
@@ -751,7 +751,7 @@ __global__ void add_f32_kernel(float* __restrict__ dst, const float* __restrict_
     dst[i] += src[i];
 }
 
-static int blocks_for(int64_t n) { return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 148 * 16))); }
+static int blocks_for(int64_t n) { return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 132 * 16))); }
 
 int launch_permute021(const float* in, int A, int Bd, int Cd, const float* row_scale, __nv_bfloat16* out_bf16,
                       float* out_f32, int accumulate, cudaStream_t s) {

@@ -129,8 +129,8 @@ int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -191,10 +191,12 @@ int vdk_device_check(void) {
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n == 0)
     return vdk::fail(VDK_ERR_CUDA, "no CUDA device: %s", e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   VDK_CUDA_OK(cudaGetDevice(&dev));
   VDK_CUDA_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 10) return vdk::fail(VDK_ERR_CUDA, "device compute capability %d.x; this library is sm_100a only", major);
+  VDK_CUDA_OK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  if (major != 9 || minor != 0)
+    return vdk::fail(VDK_ERR_CUDA, "device compute capability %d.%d; this library is sm_90a only", major, minor);
   return VDK_OK;
 }
 

@@ -1,6 +1,6 @@
-// vdk_ptx.cuh — thin inline-PTX wrappers for the sm_100a primitives the hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), cluster helpers.
-// Written for sm_100a only; there is deliberately no fallback for other architectures.
+// vdk_ptx.cuh — thin inline-PTX wrappers for the sm_90a primitives the hot path uses:
+// mbarrier, TMA (cp.async.bulk.tensor), cluster helpers; the warpgroup MMA lives in vdk_wgmma.cuh.
+// Written for sm_90a only; there is deliberately no fallback for other architectures.
 #pragma once
 #include <cstdint>
 #include <cstdio>
@@ -8,6 +8,8 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+
+#include "vdk_wgmma.cuh"
 
 namespace vdk {
 
@@ -67,13 +69,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // Bounded wait: a protocol bug must surface as a trap (a CUDA error the caller reports), never as a
-// hung GPU.  The bound (~4e9 cycles, >2 s at any clock) is far beyond any legitimate wait.
+// hung GPU.  The bound (~4e9 cycles, >2 s at any clock) is far beyond any legitimate wait.  kQuiet: trap without the
+// message, for kernels that keep wgmma in flight (a call to printf anywhere in a kernel makes ptxas serialize its wgmma).
+template <bool kQuiet = false>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > 4000000000LL) {
-      printf("vdk: mbarrier wait timed out (block %d, thread %d, parity %u)\n", (int)blockIdx.x, (int)threadIdx.x, parity);
+      if (!kQuiet) printf("vdk: mbarrier wait timed out (block %d, thread %d, parity %u)\n", (int)blockIdx.x, (int)threadIdx.x, parity);
       __trap();
     }
   }
@@ -82,6 +86,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // The same wait for threads that are expected to wait LONG (a producer out of free slots, an epilogue waiting for the
 // next accumulator): after a few polls the warp sleeps between polls, so that its spin loop stops competing for issue
 // slots with the warps that share its scheduler.
+template <bool kQuiet = false>
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
@@ -89,7 +94,7 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity
   while (!mbar_try_wait(bar, parity)) {
     if (++polls > 4) __nanosleep(64);
     if (clock64() - t0 > 4000000000LL) {
-      printf("vdk: mbarrier wait timed out (block %d, thread %d, parity %u)\n", (int)blockIdx.x, (int)threadIdx.x, parity);
+      if (!kQuiet) printf("vdk: mbarrier wait timed out (block %d, thread %d, parity %u)\n", (int)blockIdx.x, (int)threadIdx.x, parity);
       __trap();
     }
   }
@@ -153,115 +158,8 @@ __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// cluster helpers
 // ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: pow2 in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (tile rows are 128 B = 64 x 16-bit;
-// 8-row groups are 1024 B apart).  Field layout: cute/arch/mma_sm100_desc.hpp (SmemDescriptor).
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // start address      [0,14)
-  d |= static_cast<uint64_t>(1) << 16;                      // leading byte offs  [16,30) (unused w/ swizzle)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;              // stride byte offset [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                      // descriptor version [46,48) = 1 on sm_100
-  d |= static_cast<uint64_t>(2) << 61;                      // layout type        [61,64) = SWIZZLE_128B
-  return d;
-}
-
-// MN-major operand (the contraction index is the SLOW dimension in memory), 128-byte swizzle: the tile is stored as
-// blocks of 64 MN-elements (one 128-byte swizzle row) x kBK contraction rows; inside a block groups of 8 contraction
-// rows are 1024 B apart (stride byte offset), and the next block of 64 MN-elements starts `mn_block_bytes` later
-// (leading byte offset).  One UMMA (K = 16) spans two 8-row groups: advance the start address by 2048 B per step.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t mn_block_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((mn_block_bytes >> 4) & 0x3FFFu) << 16;  // leading byte offset
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;                        // stride byte offset
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 (A/B fp16 or bf16, fp32 accumulate, both operands K-major).
-// Field layout: cute/arch/mma_sm100_desc.hpp (InstrDescriptor).
-template <bool kBf16>
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t m, uint32_t n, uint32_t a_mn = 0, uint32_t b_mn = 0) {
-  return (1u << 4)                      // c_format = F32
-         | ((kBf16 ? 1u : 0u) << 7)     // a_format
-         | ((kBf16 ? 1u : 0u) << 10)    // b_format
-         | (a_mn << 15) | (b_mn << 16)  // a_major, b_major: 0 = K-major, 1 = MN-major
-         | ((n >> 3) << 17)             // n_dim
-         | ((m >> 4) << 24);            // m_dim
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; single-CTA, issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this thread's lane (row), 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM: this thread's lane (row), 32 consecutive 32-bit columns (the accumulator rescale of the attention kernel)
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-      "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-      "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// CTA pairs (cta_group::2): two CTAs of a 2-cluster share one UMMA (M = 256); forms as in cute/arch/copy_sm100_tma.hpp
-// and cutlass/arch/barrier.h
-// ----------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> the even CTA
-
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -271,65 +169,12 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// TMA load into THIS CTA's shared memory whose completion bytes are credited to the LEADER (even) CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
-                                                 uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "l"(policy)
-      : "memory");
-}
-// arrive on the LEADER CTA's copy of `bar` (same offset in its shared memory) from either CTA of the pair
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: pow2 in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[256 rows: 128 per CTA] * B[N rows: N/2 per CTA]^T ; issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on `bar` in BOTH CTAs of the pair once all previously issued pair-MMAs have completed
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b16 m;\n\t"
-      "mov.b16 m, 3;\n\t"
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], m;\n\t"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
 
 // ----------------------------------------------------------------------------------------------
-// packed fp32 pairs.  Measured on B200 (tools/ubench_fma.cu): FFMA issues every 1.01 clk per scheduler (126 FMA/clk/SM), FFMA2
-// every 2.17 clk (118 FMA/clk/SM): the same FP32 rate at half the issue slots, which leaves every other slot to the loads /
-// conversions of an FMA-bound CUDA-core loop
+// fp32 pairs: two independent FMAs (sm_90 has no packed fp32 instruction; the pair form keeps the call sites' shape)
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra = *reinterpret_cast<unsigned long long*>(&a), rb = *reinterpret_cast<unsigned long long*>(&b),
-                     rc = *reinterpret_cast<unsigned long long*>(&c), rd;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  return *reinterpret_cast<float2*>(&rd);
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
 // ----------------------------------------------------------------------------------------------

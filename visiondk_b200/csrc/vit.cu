@@ -1,4 +1,4 @@
-// vit.cu — ViT inference forward (CBIR extract path with a Transformer backbone) on the same tcgen05 GEMM, plus the one
+// vit.cu — ViT inference forward (CBIR extract path with a Transformer backbone) on the same wgmma GEMM, plus the one
 // kernel the ConvNeXt path does not have: softmax(Q K^T / sqrt(d)) V.
 //
 // Replaces, for `timm-vit_*` backbones, the eval forward of TimmWrapper (models/faceX/backbone/timm_wrapper.py:51-54: timm's
@@ -13,7 +13,7 @@
 //
 // Attention: one CTA = 64 query rows of one (image, head), 4 warps x 16 rows, K/V streamed in 64-row tiles through
 // swizzled shared memory, mma.sync m16n8k16 (bf16 in, fp32 accumulate) with the online-softmax recurrence in registers
-// (scores never leave the SM).  Attention is 4 % of a ViT-B's FLOPs; the tcgen05 version is the next step for it.
+// (scores never leave the SM).  Attention is 4 % of a ViT-B's FLOPs.
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
 #include "convnext_internal.h"
@@ -280,8 +280,8 @@ int launch_attention_tc(const __nv_bfloat16* qkv, int B, int N, int H, __nv_bflo
 static int launch_attention_mma_sync(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
                                      cudaStream_t s);
 
-// Forward attention: the tcgen05 kernel (attention_tc.cu) by default; VDK_ATT_TC=0 selects the earlier mma.sync kernel (kept as
-// the comparison baseline of profiles/ and for A/B parity tests).
+// Forward attention: the wgmma kernel (attention_tc.cu) by default; VDK_ATT_TC=0 selects the earlier mma.sync kernel (kept as
+// the comparison baseline and for A/B parity tests).
 static int launch_attention(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
                             cudaStream_t s) {
   static const bool use_tc = [] {
@@ -306,7 +306,7 @@ static int launch_attention_mma_sync(const __nv_bfloat16* qkv, int B, int N, int
   const int row_groups = (N + 15) / 16;
   static const int warp_cap = [] {  // tuning switch: query-row groups (warps) per CTA
     const char* e = getenv("VDK_ATT_WARPS");
-    const int v = e ? atoi(e) : 8;  // measured on ViT-B/16 batch 256: 16 -> 13.06 ms, 8 -> 12.68 ms, 4 -> 12.87 ms per forward
+    const int v = e ? atoi(e) : 8;
     return v < 1 ? 1 : (v > kAttMaxWarps ? kAttMaxWarps : v);
   }();
   const int ctas = (row_groups + warp_cap - 1) / warp_cap;
@@ -644,13 +644,13 @@ extern "C" int vdk_vit_forward(const vdk_vit_net* net, const float* images, int 
     __nv_bfloat16* rows = big;                                                        // [B*N, Kp]
     __nv_bfloat16* tok = big + (static_cast<size_t>(batch) * N * L.Kp + 127) / 128 * 128;  // [B*N, C]
     const int64_t total = static_cast<int64_t>(batch) * N * L.Kp;
-    vit_patchify_kernel<<<static_cast<int>(std::min<int64_t>((total + 255) / 256, 148 * 32)), 256, 0, s>>>(images, batch, net->image_size,
+    vit_patchify_kernel<<<static_cast<int>(std::min<int64_t>((total + 255) / 256, 132 * 32)), 256, 0, s>>>(images, batch, net->image_size,
                                                                                                          net->patch, L.Kp, rows);
     VDK_CUDA_OK(cudaGetLastError());
     rc = gemm(rows, net->patch_w, tok, batch * N, C, L.Kp, L.Kp, VDK_EPI_NONE, net->patch_b, nullptr, nullptr);
     if (rc != VDK_OK) return rc;
     const int64_t tot2 = static_cast<int64_t>(M) * (C / 2);
-    vit_assemble_kernel<<<static_cast<int>(std::min<int64_t>((tot2 + 255) / 256, 148 * 32)), 256, 0, s>>>(tok, net->cls_token, net->pos_embed,
+    vit_assemble_kernel<<<static_cast<int>(std::min<int64_t>((tot2 + 255) / 256, 132 * 32)), 256, 0, s>>>(tok, net->cls_token, net->pos_embed,
                                                                                                         batch, N, C, x);
     VDK_CUDA_OK(cudaGetLastError());
     if (net->norm_pre_w) {  // timm pre_norm=True (CLIP towers): LayerNorm over every token before the first block
@@ -857,13 +857,13 @@ extern "C" int vdk_vit_train_forward(const vdk_vit_net* net, const vdk_vit_tenso
 
   {
     const int64_t total = static_cast<int64_t>(batch) * N * L.Kp;
-    vit_patchify_kernel<<<static_cast<int>(std::min<int64_t>((total + 255) / 256, 148 * 32)), 256, 0, s>>>(images, batch, net->image_size,
+    vit_patchify_kernel<<<static_cast<int>(std::min<int64_t>((total + 255) / 256, 132 * 32)), 256, 0, s>>>(images, batch, net->image_size,
                                                                                                          net->patch, L.Kp, B16(L.rows));
     VDK_CUDA_OK(cudaGetLastError());
     RC(G.run(B16(L.rows), net->patch_w, B16(L.tok), batch * N, C, L.Kp, L.Kp, L.Kp, C, VDK_EPI_NONE, net->patch_b, nullptr, nullptr, 0,
              VDK_DTYPE_BF16, 1, 0, 0, 0));
     const int64_t tot2 = static_cast<int64_t>(M) * (C / 2);
-    vit_assemble_kernel<<<static_cast<int>(std::min<int64_t>((tot2 + 255) / 256, 148 * 32)), 256, 0, s>>>(B16(L.tok), net->cls_token,
+    vit_assemble_kernel<<<static_cast<int>(std::min<int64_t>((tot2 + 255) / 256, 132 * 32)), 256, 0, s>>>(B16(L.tok), net->cls_token,
                                                                                                         net->pos_embed, batch, N, C, B16(L.x0));
     VDK_CUDA_OK(cudaGetLastError());
   }
@@ -970,7 +970,7 @@ static int vit_backward_range(const vdk_vit_net* net, const vdk_vit_tensors* p, 
   // ---- cls / position embeddings, patch embedding ----
   if (active(net->depth + 1)) {
     const int64_t tot = static_cast<int64_t>(T) * C;
-    vit_assemble_bwd_kernel<<<static_cast<int>(std::min<int64_t>((tot + 255) / 256, 148 * 8)), 256, 0, s>>>(B16(dx), batch, N, C, B16(L.dtok),
+    vit_assemble_bwd_kernel<<<static_cast<int>(std::min<int64_t>((tot + 255) / 256, 132 * 8)), 256, 0, s>>>(B16(dx), batch, N, C, B16(L.dtok),
                                                                                                            g->pos_embed, g->cls_token);
     VDK_CUDA_OK(cudaGetLastError());
     RC(launch_col_sum(B16(L.dtok), static_cast<int64_t>(batch) * N, C, C, g->patch_b, s));

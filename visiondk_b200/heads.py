@@ -1,9 +1,9 @@
-"""Head seam of the faceX train step on B200 (SURVEY.md §8b, Seam 2 and Seam 4).
+"""Head seam of the faceX train step on H100 (SURVEY.md §8b, Seam 2 and Seam 4).
 
 `HeadFactory(model_cfg['head']).get_head()` (models/faceX/head/head_def.py:14-56) returns an nn.Module with
 `.weight: Parameter[feat_dim, num_class]` and `forward(feats[B,D], labels[B]) -> logits[B,C]`.  ArcFace and
 CircleLoss here keep that surface and parameter initialisation (arcface.py:11-12) while the arithmetic — both
-normalisations, the cos(theta) contraction on tcgen05, the margin, and (in the fused form the trainer uses) the
+normalisations, the cos(theta) contraction on wgmma, the margin, and (in the fused form the trainer uses) the
 cross-entropy with label smoothing and the whole backward — is csrc/heads.cu.
 
 `margin_ce_loss(head, feats, labels, label_smooth)` is criterion∘head fused: the two are only ever called
@@ -47,7 +47,7 @@ def _workspace(desc, device):
 
 def _check_inputs(feats, weight, labels):
     if feats.device.type != "cuda":
-        raise RuntimeError("visiondk_b200 heads run on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("visiondk_b200 heads run on CUDA (sm_90a) only; there is no CPU fallback")
     if feats.dim() != 2 or feats.shape[1] != weight.shape[0]:
         raise ValueError(f"feats must be [B, {weight.shape[0]}], got {tuple(feats.shape)}")
     if labels.shape != (feats.shape[0],):
@@ -181,5 +181,5 @@ class HeadFactory:
             return CircleLoss(p["feat_dim"], p["num_class"], p["margin"], p["gamma"])
         if self.head_type == "mv-softmax":
             return MV_Softmax(p["feat_dim"], p["num_class"], p["is_am"], p["margin"], p["mv_weight"], p["scale"])
-        raise NotImplementedError(f"head '{self.head_type}': arcface, circleloss and mv-softmax are built for B200; magface returns "
+        raise NotImplementedError(f"head '{self.head_type}': arcface, circleloss and mv-softmax are built for H100; magface returns "
                                   f"a (logits, loss) tuple the reference's own train loop cannot consume (magface.py:47 vs train.py:196)")

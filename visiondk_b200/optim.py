@@ -1,4 +1,4 @@
-"""Optimizer half of the faceX train step on B200 (SURVEY.md §8b, Seam 4).
+"""Optimizer half of the faceX train step on H100 (SURVEY.md §8b, Seam 4).
 
 Reference: `Trainer.update(model, loss, scaler, optimizer, ema)` (engine/procedure/train.py:203-215) =
 backward -> clip_grad_norm_(10) -> SGD step -> zero_grad -> ModelEMA.update, with param groups from
@@ -54,7 +54,7 @@ class FusedSGDClipEMA:
             groups = [(list(param_groups), float(lr))]
         for ps, _ in groups:
             if any(p.device.type != "cuda" for p in ps):
-                raise RuntimeError("FusedSGDClipEMA runs on CUDA (sm_100a) parameters only; there is no CPU fallback")
+                raise RuntimeError("FusedSGDClipEMA runs on CUDA (sm_90a) parameters only; there is no CPU fallback")
         self.groups = [_FlatGroup([p for p in ps if p.requires_grad], g_lr) for ps, g_lr in groups]
         self.param_groups = [{"lr": g.lr, "initial_lr": g.lr, "momentum": momentum, "weight_decay": weight_decay}
                              for g in self.groups]  # scheduler-facing view (torch LR schedulers mutate 'lr')

@@ -27,7 +27,7 @@ class ImagePreprocessor:
         self.size = int(size)
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("visiondk_b200 preprocessing runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200 preprocessing runs on CUDA (sm_90a) only; there is no CPU fallback")
         self.mean = (C.c_float * 3)(*[float(np.float32(m)) for m in mean])
         self.std = (C.c_float * 3)(*[float(np.float32(s)) for s in std])
         self._pinned = None

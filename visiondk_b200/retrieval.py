@@ -1,10 +1,10 @@
-"""Flat inner-product index on B200: the drop-in for the faiss objects of the reference's CBIR path.
+"""Flat inner-product index on H100: the drop-in for the faiss objects of the reference's CBIR path.
 
 Seam (SURVEY.md §8b, Seam 6): engine/cbir/evaluation.py:155-168 builds
 `faiss.index_factory(dim, "Flat", faiss.METRIC_INNER_PRODUCT)`, clones it to the GPUs, then calls
 `.train(x)`, `.add(x)` and (evaluation.py:193) `.search(x, k) -> (scores float32 [n,k] desc, ids int64 [n,k])`.
 FlatIPIndex answers exactly those calls with numpy in / numpy out, and adds `search_device` for callers that
-keep embeddings on the GPU (what extract -> search should do on a B200; the reference's per-batch
+keep embeddings on the GPU (what extract -> search should do on an H100; the reference's per-batch
 `.cpu().numpy()` at face_model.py:140 is a host round trip the hot path does not need).
 
 Results are EXACT inner-product top-k under the canonical score / tie rule of oracle/retrieval.py
@@ -28,7 +28,7 @@ FLT_LOWEST = -3.4028234663852886e38
 def _dev(device) -> torch.device:
     d = torch.device(device if device is not None else "cuda")
     if d.type != "cuda":
-        raise RuntimeError("visiondk_b200 runs on CUDA (sm_100a) devices only; there is no CPU path")
+        raise RuntimeError("visiondk_b200 runs on CUDA (sm_90a) devices only; there is no CPU path")
     return d
 
 
@@ -408,9 +408,7 @@ def shard_schedule(ng_max: int, world: int, k: int):
     """Gallery range ends every shard of a `world`-way search follows (computed from the LARGEST shard).  After a range every
     shard knows (from the rank sketches) about the k-th score of the union of `world` prefixes, so the next range may grow `world`
     times faster at the same expected admissions per query: 2 ranges per shard on 8 GPUs instead of 3.
-    Measured on 2 GPUs (profiles/r02_retrieval.md): shrinking the dense first range to 8192 / world rows and growing by
-    1 + 15 * world costs more in admissions than the smaller dense write saves (6.90 ms against 6.21 ms): so the single-GPU first
-    range, growth 1 + 7 * world.  VDK_SHARD_FIRST / VDK_SHARD_GROWTH override (tuning)."""
+    The first range is the single-GPU one and the growth 1 + 7 * world.  VDK_SHARD_FIRST / VDK_SHARD_GROWTH override (tuning)."""
     first = int(os.environ.get("VDK_SHARD_FIRST", min(max(4096, (4 * k + 255) // 256 * 256), 16384)))
     first = min(first, (max(ng_max, 1) + 255) // 256 * 256)
     growth = int(os.environ.get("VDK_SHARD_GROWTH", 1 + 7 * world))

@@ -1,4 +1,4 @@
-"""faceX train step on B200 (SURVEY.md §8a rows a1-a3, a9-a12): the reference's model container and step, same names.
+"""faceX train step on H100 (SURVEY.md §8a rows a1-a3, a9-a12): the reference's model container and step, same names.
 
   FaceTrainingModel      models/faceX/face_model.py:28-54   (trainingwrapper = ModuleDict{'backbone','head'})
   cosine_with_warm       engine/scheduler.py:47-57          (LinearLR 0.1->1 then CosineAnnealingLR, stepped per batch)
@@ -6,7 +6,7 @@
   FaceTrainer.step       engine/procedure/train.py:196-215,230  (criterion∘model, backward, clip, SGD, zero_grad, EMA, LR)
   DDP                    engine/vision_engine.py:509-510    -> one NCCL all-reduce(mean) of the flat gradient buffers
 
-All arithmetic is the sm_100a kernels: backbone forward/backward (csrc/convnext_train.cu), fused margin head + CE
+All arithmetic is the sm_90a kernels: backbone forward/backward (csrc/convnext_train.cu), fused margin head + CE
 (csrc/heads.cu), fused clip + SGD + EMA (csrc/optim.cu).
 """
 from __future__ import annotations
@@ -65,7 +65,7 @@ def layer_wise_groups(model: FaceTrainingModel, layer_wise: bool, lr: float):
 
 
 class FaceTrainer:
-    """The per-batch body of Trainer.train_one_epoch_face (engine/procedure/train.py:217-233) on B200."""
+    """The per-batch body of Trainer.train_one_epoch_face (engine/procedure/train.py:217-233) on H100."""
 
     def __init__(self, model: FaceTrainingModel, lr0: float, momentum: float, weight_decay: float, label_smooth: float = 0.0,
                  layer_wise: bool = True, warm_steps: int = 0, total_steps: int = 1, lrf_ratio: Optional[float] = None,

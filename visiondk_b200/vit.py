@@ -1,4 +1,4 @@
-"""ViT backbones for the CBIR extract path (inference) on the B200 kernels.
+"""ViT backbones for the CBIR extract path (inference) on the H100 kernels.
 
 Mirrors what `TimmWrapper(model_name='vit_*', feat_dim, image_size)` builds in the reference
 (models/faceX/backbone/timm_wrapper.py:16-21 + the Transformer neck of :39-47): the parameter tree and state_dict keys of
@@ -125,12 +125,12 @@ class ViTWrapper(nn.Module):
         super().__init__()
         if dim is None:
             if model_name not in VIT_ARCHS:
-                raise ValueError(f"backbone '{model_name}' is not built for B200 yet; available: {sorted(VIT_ARCHS)}")
+                raise ValueError(f"backbone '{model_name}' is not built for H100 yet; available: {sorted(VIT_ARCHS)}")
             patch, dim, depth, heads = VIT_ARCHS[model_name]
         if pre_norm is None:
             pre_norm = model_name in VIT_PRE_NORM
         if image_size % patch != 0 or dim != heads * 64 or depth > MAX_BLOCKS:
-            raise ValueError("ViT on B200: image_size must be a multiple of patch, head_dim must be 64, depth <= 48")
+            raise ValueError("ViT on H100: image_size must be a multiple of patch, head_dim must be 64, depth <= 48")
         self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
         self.model = ViTParams(image_size, patch, dim, depth, heads, pre_norm=pre_norm)
         tokens = (image_size // patch) ** 2 + 1
@@ -229,7 +229,7 @@ class ViTWrapper(nn.Module):
     def _train_forward(self, x: torch.Tensor) -> torch.Tensor:
         lib = _lib.load()
         if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.ViTWrapper runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200.ViTWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
         x = x.contiguous().float()
         B = x.shape[0]
         st, net, params = self._train_structs(x.device)
@@ -347,7 +347,7 @@ class ViTWrapper(nn.Module):
         """[B,3,S,S] fp32 NCHW -> fp32 [B, feat_dim] (TimmWrapper.forward in eval mode; optionally F.normalize fused)."""
         lib = _lib.load()
         if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.ViTWrapper runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("visiondk_b200.ViTWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
         if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
             raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
         x = x.contiguous().float()
