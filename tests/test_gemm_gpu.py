@@ -1,42 +1,185 @@
-"""GPU parity of vdk_gemm_tn (wgmma/TMA GEMM) against a plain fp32 torch reference of the same op.
+"""GPU parity of vdk_gemm (wgmma/TMA GEMM) and its epilogues against an fp64 reference of the same 16-bit inputs.
 
-Inputs are drawn already rounded to the 16-bit input type, so the only differences are the fp32
-accumulation order (tolerance 2e-3 relative to the row scale) and, for 16-bit outputs, one final rounding.
+Bounds are elementwise.  The fp32 accumulation follows the model of DESIGN.md §3: a K-long dot product on wgmma is off by at
+most (ceil(K/16) + 17) 2^-23 (|A| |B|^T)_mn.  Each fp32 operation of the epilogue adds one rounding (2^-24 relative to its
+result), the 16-bit output one ulp of the output type at |ref|, and the activations their documented approximation error.
+
+The kernel is persistent (min(tiles, SM count) CTAs, each looping over tiles 128 x BN), so the regime cases size M from the
+device's SM count to give every CTA at least three tiles, and one case exactly SM + 1 tiles.  Outputs sit in NaN-guarded
+buffers (padding columns for ldd > N, trailing rows, a tail); a failure names the wrong tiles and the CTA that ran them.
 """
+import ctypes as C
+import math
+
 import pytest
 import torch
 
+from kernel_ref import U32, Guarded, check_within, ulp
 from visiondk_b200 import _lib
 
 pytestmark = pytest.mark.gpu
 
 DT = {"bf16": (torch.bfloat16, _lib.DTYPE_BF16), "fp16": (torch.float16, _lib.DTYPE_FP16),
       "fp32": (torch.float32, _lib.DTYPE_FP32)}
+CODE = {torch.bfloat16: _lib.DTYPE_BF16, torch.float16: _lib.DTYPE_FP16, torch.float32: _lib.DTYPE_FP32}
+
+# Documented accuracy of the fp16x2 activations (gemm.cu, include/vdk_b200.h).  The sweeps below run every finite 16-bit
+# pre-activation through them: on an H100 the worst GELU error was 4.3e-4 |x|, the worst GELU' error 7.6e-3 (near |x| = 3, where
+# the error of tanh.approx.f16 in 1 - tanh^2 is multiplied by x (c1 + 3 c3 x^2) ~ 5)
+GELU_REL_ERR = 6e-4     # |gelu~(x) - gelu(x)| <= GELU_REL_ERR |x|
+GELU_GRAD_ERR = 8e-3    # |gelu~'(x) - gelu'(x)| <= GELU_GRAD_ERR
+GELU_GRAD_MAX = 1.13    # max |gelu'(x)| = 1.1289...
 
 
-def run_gemm(a, b, out_dtype, epilogue=_lib.EPI_NONE, bias=None, gamma=None, residual=None):
+def sm_count():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def tile_n(N, epilogue):
+    wide = N % 256 == 0 or N > 512
+    if epilogue == _lib.EPI_LAYERNORM:
+        wide = N > 128
+    return 256 if wide else 128
+
+
+def gelu64(x):
+    return 0.5 * x * (1.0 + torch.special.erf(x / math.sqrt(2.0)))
+
+
+def gelu_grad64(x):
+    return 0.5 * (1.0 + torch.special.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
+
+
+def out_rounding(ref, dtype):
+    return torch.zeros_like(ref) if dtype == torch.float32 else ulp(ref, dtype)
+
+
+def describe_tiles(M, N, BN):
+    """bad [M, N] -> the (tile row, tile column) tiles holding failures, the CTAs that ran them (tile % grid) and how many
+    wrong tiles each round of the persistent loop (tile // grid) had."""
+    num_n = -(-N // BN)
+    tiles = -(-M // 128) * num_n
+    grid = min(tiles, sm_count())
+
+    def describe(bad):
+        idx = bad.nonzero()
+        t = torch.unique((idx[:, 0] // 128) * num_n + idx[:, 1] // BN)
+        return (f"{t.numel()}/{tiles} tiles wrong (BN {BN}, grid {grid}); wrong tiles per CTA round "
+                f"{torch.bincount(t // grid).tolist()}; first (tile row, tile col, CTA) "
+                f"{[(int(x) // num_n, int(x) % num_n, int(x) % grid) for x in t[:6]]}; first element {idx[0].tolist()}")
+    return describe
+
+
+def run(a, b, out_dtype, epilogue=_lib.EPI_NONE, bias=None, gamma=None, beta=None, residual=None, ldr_pad=0, ldd_pad=0,
+        aux=False, ta=0, tb=0, ln_eps=1e-6, in_place=False):
+    """vdk_gemm of logical a [M, K] and b [N, K] (stored transposed when ta / tb) into a guarded D [M, N] with pitch
+    N + ldd_pad.  `residual` holds the values of the residual (SCALE_RESIDUAL) or saved pre-activation (MUL_GELU_GRAD): copied
+    into D itself when in_place, else into a guarded [M, N] buffer of pitch N + ldr_pad.  Returns (D, aux or None)."""
     lib = _lib.load()
     M, K = a.shape
     N = b.shape[0]
-    d = torch.full((M, N), float("nan"), dtype=DT[out_dtype][0], device=a.device)
-    in_code = _lib.DTYPE_BF16 if a.dtype == torch.bfloat16 else _lib.DTYPE_FP16
-    rc = lib.vdk_gemm_tn(a.data_ptr(), b.data_ptr(), d.data_ptr(), M, N, K, a.stride(0), b.stride(0), d.stride(0),
-                         in_code, DT[out_dtype][1], epilogue, _lib.ptr(bias), _lib.ptr(gamma), _lib.ptr(residual),
-                         residual.stride(0) if residual is not None else 0, _lib.stream_ptr())
-    _lib.check(rc, "vdk_gemm_tn")
+    a_st = a.t().contiguous() if ta else a
+    b_st = b.t().contiguous() if tb else b
+    d = Guarded(M, N, N + ldd_pad, out_dtype)
+    res, ldr = None, 0
+    if residual is not None:
+        if in_place:
+            d.fill_(residual)
+            res, ldr = d, N + ldd_pad
+        else:
+            res, ldr = Guarded(M, N, N + ldr_pad, residual.dtype).fill_(residual), N + ldr_pad
+    ax = Guarded(M, N, N + ldd_pad, out_dtype) if aux else None
+    g = _lib.GemmDesc(A=a_st.data_ptr(), B=b_st.data_ptr(), D=d.ptr(), M=M, N=N, K=K, lda=a_st.stride(0), ldb=b_st.stride(0),
+                      ldd=N + ldd_pad, in_dtype=CODE[a.dtype], out_dtype=CODE[out_dtype], epilogue=epilogue,
+                      bias=_lib.ptr(bias), gamma=_lib.ptr(gamma), beta=_lib.ptr(beta), residual=res.ptr() if res else 0,
+                      ldr=ldr, ln_eps=ln_eps, split_k=1, split_stride=0, aux_out=ax.ptr() if ax else 0, trans_a=ta, trans_b=tb)
+    _lib.check(lib.vdk_gemm(C.byref(g), _lib.stream_ptr()), "vdk_gemm")
     torch.cuda.synchronize()
-    return d
+    for name, buf in (("D", d), ("aux", ax), ("residual", res if res is not d else None)):
+        if buf is not None:
+            assert not buf.guard_errors(), f"{name}: {buf.guard_errors()}"
+    return d, ax
 
 
-def describe_mismatch(got, ref, tol):
-    bad = (got.float() - ref).abs() > tol
-    idx = bad.nonzero()
-    rows = idx[:, 0]
-    cols = idx[:, 1]
-    return (f"{int(bad.sum())}/{bad.numel()} wrong; rows%8 hist {torch.bincount(rows % 8, minlength=8).tolist()} "
-            f"cols%8 hist {torch.bincount(cols % 8, minlength=8).tolist()} "
-            f"row tiles {torch.unique(rows // 128).tolist()[:8]} col tiles {torch.unique(cols // 128).tolist()[:8]} "
-            f"first {idx[:4].tolist()} got {got[bad][:4].tolist()} ref {ref[bad][:4].tolist()} nan {int(torch.isnan(got.float()).sum())}")
+def acc_reference(a, b):
+    """fp64 A . B^T of the 16-bit operands and the fp32 accumulation bound (ceil(K/16) + 17) 2^-23 (|A| |B|^T)."""
+    A, Bm = a.double(), b.double()
+    K = A.shape[1]
+    return A @ Bm.t(), (-(-K // 16) + 17) * U32 * (A.abs() @ Bm.abs().t())
+
+
+def check_epilogue(a, b, out_dtype, epilogue, d, ax, bias=None, gamma=None, beta=None, residual=None, ln_eps=1e-6, name=""):
+    """Compares D (and the saved pre-activation) with the fp64 epilogue of the exact accumulator.
+
+      x = acc + bias in fp32:         |x~ - x| <= ex = e_acc + 2^-24 |x|  (no rounding without a bias)
+      NONE                            ref = x, bound ex
+      GELU                            ref = gelu(x), bound max|gelu'| ex + GELU_REL_ERR |x| + 2^-24 |ref|
+      GELU + aux_out                  aux: ref x, bound ex + ulp(x); out: ref gelu(aux), bound GELU_REL_ERR |aux| + 2^-24 |ref|
+      SCALE_RESIDUAL                  ref = res + gamma x, bound |gamma| ex + 2^-24 (|gamma x| + |ref|)
+      MUL_GELU_GRAD                   ref = acc gelu'(pre), bound (|gelu'(pre)| + GELU_GRAD_ERR) e_acc + GELU_GRAD_ERR |acc|
+                                      + 2^-24 |ref|
+      LAYERNORM (row of n = N values, E = max_j ex_j, r = 1/sqrt(var + eps), d_i = x_i - mean):
+        mean: ~n/4 sequential fp32 adds per thread, 2 shuffles, a divide: |dmean| <= E + (n/4 + 3) 2^-24 mean|x| = dm
+        d~_i off by D_i = ex_i + dm + 2^-24 |d_i|; the two-pass variance off by the relative
+        rho = (2 max D sqrt(var) + max D^2) / (var + eps) + (n/4 + 4) 2^-24, rsqrtf adds 2^-22:
+        bound |g_i| r D_i + |g_i d_i| r (rho / 2 + 2^-22) + 2^-24 (3 |g_i d_i| r + |ref|)
+    plus one ulp of a 16-bit output type at |ref| everywhere.
+    """
+    M, N = d.view.shape
+    acc, e = acc_reference(a, b)
+    bias64 = bias.double() if bias is not None else torch.zeros(N, dtype=torch.float64, device=acc.device)
+    x = acc + bias64
+    ex = e + (2.0 ** -24 * x.abs() if bias is not None else 0.0)
+    describe = describe_tiles(M, N, tile_n(N, epilogue))
+    got = d.view.double()
+    if epilogue == _lib.EPI_NONE:
+        ref, bound = x, ex
+    elif epilogue == _lib.EPI_GELU and ax is not None:
+        check_within(ax.view, x, ex + ulp(x, out_dtype), f"{name} aux", describe)
+        pre = ax.view.double()
+        ref = gelu64(pre)
+        bound = GELU_REL_ERR * pre.abs() + 2.0 ** -24 * ref.abs()
+    elif epilogue == _lib.EPI_GELU:
+        ref = gelu64(x)
+        bound = GELU_GRAD_MAX * ex + GELU_REL_ERR * x.abs() + 2.0 ** -24 * ref.abs()
+    elif epilogue == _lib.EPI_SCALE_RESIDUAL:
+        g = gamma.double()
+        ref = residual.double() + g * x
+        bound = g.abs() * ex + 2.0 ** -24 * ((g * x).abs() + ref.abs())
+    elif epilogue == _lib.EPI_MUL_GELU_GRAD:
+        gp = gelu_grad64(residual.double())
+        ref = acc * gp
+        bound = (gp.abs() + GELU_GRAD_ERR) * e + GELU_GRAD_ERR * acc.abs() + 2.0 ** -24 * ref.abs()
+    elif epilogue == _lib.EPI_LAYERNORM:
+        mean = x.mean(1, keepdim=True)
+        dv = x - mean
+        var = (dv * dv).mean(1, keepdim=True)
+        r = 1.0 / torch.sqrt(var + ln_eps)
+        g, bt = gamma.double(), beta.double()
+        ref = dv * r * g + bt
+        E = ex.amax(1, keepdim=True) if torch.is_tensor(ex) else torch.zeros_like(mean)
+        dm = E + (N / 4 + 3) * 2.0 ** -24 * x.abs().mean(1, keepdim=True)
+        Di = ex + dm + 2.0 ** -24 * dv.abs()
+        Dmax = Di.amax(1, keepdim=True)
+        rho = (2 * Dmax * var.sqrt() + Dmax * Dmax) / (var + ln_eps) + (N / 4 + 4) * 2.0 ** -24
+        gd = (g * dv).abs()
+        bound = g.abs() * r * Di + gd * r * (rho / 2 + 2.0 ** -22) + 2.0 ** -24 * (3 * gd * r + ref.abs())
+    else:
+        raise ValueError(epilogue)
+    check_within(got, ref, bound + out_rounding(ref, out_dtype), f"{name} D", describe)
+    return got, ref
+
+
+def operands(M, N, K, in_dtype, seed, a_scale=1.0, b_scale=1.0):
+    torch.manual_seed(seed)
+    dt = DT[in_dtype][0]
+    a = (a_scale * torch.randn(M, K, device="cuda")).to(dt)
+    b = (b_scale * torch.randn(N, K, device="cuda")).to(dt)
+    return a, b
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# plain products (shapes of the original suite) on the fp64 reference
 
 
 @pytest.mark.parametrize("in_dtype", ["bf16", "fp16"])
@@ -44,15 +187,9 @@ def describe_mismatch(got, ref, tol):
                                    (1000, 384, 200), (300, 1000, 512), (4096, 512, 128), (77, 8, 8),
                                    (20000, 1024, 256)])
 def test_gemm_plain_fp32_out(lib, in_dtype, M, N, K):
-    torch.manual_seed(M * 7 + N * 3 + K)
-    dt = DT[in_dtype][0]
-    a = torch.randn(M, K, device="cuda").to(dt)
-    b = torch.randn(N, K, device="cuda").to(dt)
-    ref = a.float() @ b.float().t()
-    got = run_gemm(a, b, "fp32")
-    tol = 2e-3 * (K ** 0.5)
-    assert torch.isfinite(got).all(), describe_mismatch(got, ref, tol)
-    assert (got - ref).abs().max().item() <= tol, describe_mismatch(got, ref, tol)
+    a, b = operands(M, N, K, in_dtype, M * 7 + N * 3 + K)
+    d, _ = run(a, b, torch.float32)
+    check_epilogue(a, b, torch.float32, _lib.EPI_NONE, d, None, name="plain")
 
 
 def test_gemm_exact_small_integers(lib):
@@ -60,9 +197,8 @@ def test_gemm_exact_small_integers(lib):
     torch.manual_seed(0)
     a = torch.randint(-4, 5, (256, 192), device="cuda").to(torch.bfloat16)
     b = torch.randint(-4, 5, (384, 192), device="cuda").to(torch.bfloat16)
-    ref = a.float() @ b.float().t()
-    got = run_gemm(a, b, "fp32")
-    assert torch.equal(got, ref), describe_mismatch(got, ref, 0.0)
+    d, _ = run(a, b, torch.float32)
+    assert torch.equal(d.view.double(), a.double() @ b.double().t())
 
 
 def test_gemm_strided_operands(lib):
@@ -70,38 +206,27 @@ def test_gemm_strided_operands(lib):
     abuf = torch.randn(500, 320, device="cuda").to(torch.bfloat16)
     bbuf = torch.randn(264, 448, device="cuda").to(torch.bfloat16)
     a, b = abuf[:, :256], bbuf[:, 64:320]  # pitches 320 / 448, 16-byte aligned starts
-    ref = a.float() @ b.float().t()
-    got = run_gemm(a, b, "fp32")
-    assert (got - ref).abs().max().item() <= 2e-3 * 16, describe_mismatch(got, ref, 2e-3 * 16)
+    d, _ = run(a, b, torch.float32)
+    check_epilogue(a, b, torch.float32, _lib.EPI_NONE, d, None, name="strided")
 
 
 @pytest.mark.parametrize("out_dtype", ["bf16", "fp32"])
 def test_gemm_bias_gelu(lib, out_dtype):
-    torch.manual_seed(2)
-    M, N, K = 1568, 512, 128
-    a = (0.5 * torch.randn(M, K, device="cuda")).to(torch.bfloat16)
-    b = (0.2 * torch.randn(N, K, device="cuda")).to(torch.bfloat16)
-    bias = torch.randn(N, device="cuda")
-    ref = torch.nn.functional.gelu(a.float() @ b.float().t() + bias)
-    got = run_gemm(a, b, out_dtype, _lib.EPI_GELU, bias=bias).float()
-    # the epilogue's GELU is a half-precision tanh form fitted to erf-GELU: |err| <= 1.2e-3 |x| (gemm.cu), |x| < ~6 here
-    tol = 3e-2 if out_dtype == "bf16" else 8e-3
-    assert (got - ref).abs().max().item() <= tol, describe_mismatch(got, ref, tol)
+    a, b = operands(1568, 512, 128, "bf16", 2, 0.5, 0.2)
+    bias = torch.randn(512, device="cuda")
+    d, _ = run(a, b, DT[out_dtype][0], _lib.EPI_GELU, bias=bias)
+    check_epilogue(a, b, DT[out_dtype][0], _lib.EPI_GELU, d, None, bias=bias, name="bias_gelu")
 
 
 @pytest.mark.parametrize("out_dtype", ["bf16", "fp32"])
 def test_gemm_layerscale_residual(lib, out_dtype):
-    torch.manual_seed(3)
-    M, N, K = 784, 256, 1024
-    a = (0.3 * torch.randn(M, K, device="cuda")).to(torch.bfloat16)
-    b = (0.1 * torch.randn(N, K, device="cuda")).to(torch.bfloat16)
-    bias = torch.randn(N, device="cuda")
-    gamma = torch.rand(N, device="cuda")
-    res = torch.randn(M, N, device="cuda").to(DT[out_dtype][0])
-    ref = res.float() + gamma * (a.float() @ b.float().t() + bias)
-    got = run_gemm(a, b, out_dtype, _lib.EPI_SCALE_RESIDUAL, bias=bias, gamma=gamma, residual=res).float()
-    tol = 4e-2 if out_dtype == "bf16" else 3e-3
-    assert (got - ref).abs().max().item() <= tol, describe_mismatch(got, ref, tol)
+    a, b = operands(784, 256, 1024, "bf16", 3, 0.3, 0.1)
+    bias = torch.randn(256, device="cuda")
+    gamma = torch.rand(256, device="cuda")
+    res = torch.randn(784, 256, device="cuda").to(DT[out_dtype][0])
+    d, _ = run(a, b, DT[out_dtype][0], _lib.EPI_SCALE_RESIDUAL, bias=bias, gamma=gamma, residual=res)
+    check_epilogue(a, b, DT[out_dtype][0], _lib.EPI_SCALE_RESIDUAL, d, None, bias=bias, gamma=gamma, residual=res,
+                   name="layerscale")
 
 
 def test_gemm_rejects_bad_arguments(lib):
@@ -115,44 +240,40 @@ def test_gemm_rejects_bad_arguments(lib):
 @pytest.mark.parametrize("M,N,K", [(128, 128, 64), (256, 512, 192), (512, 2048, 50176 // 49), (1000, 384, 200), (2048, 512, 3000)])
 def test_gemm_transposed_storage(lib, ta, tb, M, N, K):
     """MN-major operands (contraction index slow): the forms the backward GEMMs use (dgrad: trans_b, wgrad: both)."""
-    import ctypes as C
-    torch.manual_seed(M + N + K + ta * 2 + tb)
-    a = torch.randn(M, K, device="cuda").to(torch.bfloat16)
-    b = torch.randn(N, K, device="cuda").to(torch.bfloat16)
-    ref = a.float() @ b.float().t()
-    a_st = a.t().contiguous() if ta else a          # [K, M] storage when transposed
-    b_st = b.t().contiguous() if tb else b          # [K, N]
-    d = torch.full((M, N), float("nan"), device="cuda")
-    g = _lib.GemmDesc(A=a_st.data_ptr(), B=b_st.data_ptr(), D=d.data_ptr(), M=M, N=N, K=K, lda=a_st.stride(0),
-                      ldb=b_st.stride(0), ldd=N, in_dtype=_lib.DTYPE_BF16, out_dtype=_lib.DTYPE_FP32, epilogue=_lib.EPI_NONE,
-                      bias=0, gamma=0, beta=0, residual=0, ldr=0, ln_eps=0.0, split_k=1, trans_a=ta, trans_b=tb)
-    _lib.check(lib.vdk_gemm(C.byref(g), _lib.stream_ptr()), "vdk_gemm")
-    torch.cuda.synchronize()
-    tol = 2e-3 * K ** 0.5
-    assert torch.isfinite(d).all(), describe_mismatch(d, ref, tol)
-    assert (d - ref).abs().max().item() <= tol, describe_mismatch(d, ref, tol)
+    a, b = operands(M, N, K, "bf16", M + N + K + ta * 2 + tb)
+    d, _ = run(a, b, torch.float32, ta=ta, tb=tb)
+    check_epilogue(a, b, torch.float32, _lib.EPI_NONE, d, None, name="transposed")
+
+
+def split_k_bound(a, b, n_split):
+    """Each split's partial is one wgmma chain over its K range; adding n_split partials (atomics or the slab sum) adds at most
+    n_split more roundings, each 2^-23 of the running |sum|: (ceil(K/16) + 17 + n_split) 2^-23 (|A| |B|^T).  At K = 12544 and
+    50176 the measured error is a few 1e-4 of this bound: the bound takes every one of the ~800 / ~3200 roundings at its maximum
+    and of one sign, and |A| |B|^T of random-sign operands exceeds |A B^T| by ~sqrt(K), while the rounding errors of the real
+    sums cancel like a random walk.  It stays the worst-case model; a lost or doubled split (one partial, ~sqrt(K / n_split)
+    times the operand scales) is still several times larger than it."""
+    A, Bm = a.double(), b.double()
+    return A @ Bm.t(), (-(-A.shape[1] // 16) + 17 + n_split) * U32 * (A.abs() @ Bm.abs().t())
 
 
 def test_gemm_wgrad_form_split_k(lib):
     """dW[N_out, K_in] = dY^T . X with the token index (M = 50k) as the contraction: both operands MN-major, split-K."""
-    import ctypes as C
     torch.manual_seed(9)
     tokens, n_out, k_in = 50176, 512, 256
     dy = (0.1 * torch.randn(tokens, n_out, device="cuda")).to(torch.bfloat16)
     x = torch.randn(tokens, k_in, device="cuda").to(torch.bfloat16)
-    ref = dy.float().t() @ x.float()
     d = torch.zeros(n_out, k_in, device="cuda")
     g = _lib.GemmDesc(A=dy.data_ptr(), B=x.data_ptr(), D=d.data_ptr(), M=n_out, N=k_in, K=tokens, lda=n_out, ldb=k_in,
                       ldd=k_in, in_dtype=_lib.DTYPE_BF16, out_dtype=_lib.DTYPE_FP32, epilogue=_lib.EPI_NONE, bias=0, gamma=0,
                       beta=0, residual=0, ldr=0, ln_eps=0.0, split_k=37, trans_a=1, trans_b=1)
     _lib.check(lib.vdk_gemm(C.byref(g), _lib.stream_ptr()), "vdk_gemm")
     torch.cuda.synchronize()
-    assert (d - ref).abs().max().item() <= 2e-3 * tokens ** 0.5 * 0.1 + 1e-2, describe_mismatch(d, ref, 0.05)
+    ref, bound = split_k_bound(dy.t(), x.t(), lib.vdk_gemm_effective_splits(tokens, 37))
+    check_within(d, ref, bound, "split-K atomics", describe_tiles(n_out, k_in, tile_n(k_in, _lib.EPI_NONE)))
 
 
 def test_gemm_split_k_slabs_are_deterministic(lib):
     """split_stride > 0: every split writes its own slab (no atomics); the slab sum is bitwise reproducible."""
-    import ctypes as C
     torch.manual_seed(4)
     M, N, K = 200, 512, 12544
     a = torch.randn(M, K, device="cuda").to(torch.bfloat16)
@@ -169,5 +290,169 @@ def test_gemm_split_k_slabs_are_deterministic(lib):
         assert torch.isfinite(d).all()
         outs.append(d.sum(0))
     assert torch.equal(outs[0], outs[1])
-    ref = a.float() @ w.float().t()
-    assert (outs[0] - ref).abs().max().item() <= 2e-3 * K ** 0.5 * 0.05 + 1e-3
+    ref, bound = split_k_bound(a, w, n_split)
+    check_within(outs[0], ref, bound, "split-K slabs", describe_tiles(M, N, tile_n(N, _lib.EPI_NONE)))
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# every epilogue in the persistent regime: >= 3 tiles per CTA, both tile widths, ragged M and ragged last 64-column chunk,
+# fp16 inputs, every output type an epilogue accepts, ldd / ldr > N, the transposed operand forms
+
+E = _lib
+# (id, in, out, epilogue, N, K, options); M is derived from the SM count (ragged: 37 rows short of a full tile row)
+REGIME = [
+    ("none_bias_bf16_fp32_N512", "bf16", "fp32", E.EPI_NONE, 512, 96, dict(bias=True, ldd_pad=8)),
+    ("none_bias_fp16_fp16_N200", "fp16", "fp16", E.EPI_NONE, 200, 80, dict(bias=True, ldd_pad=24)),
+    ("none_bf16_bf16_N520_ta", "bf16", "bf16", E.EPI_NONE, 520, 136, dict(ta=1)),
+    ("none_bf16_fp32_N512_tb", "bf16", "fp32", E.EPI_NONE, 512, 200, dict(tb=1)),
+    ("none_bf16_fp32_N136_ta_tb", "bf16", "fp32", E.EPI_NONE, 136, 72, dict(ta=1, tb=1, ldd_pad=4)),
+    ("gelu_bf16_bf16_N520", "bf16", "bf16", E.EPI_GELU, 520, 64, dict(bias=True)),
+    ("gelu_fp16_fp32_N136", "fp16", "fp32", E.EPI_GELU, 136, 96, dict(bias=True, ldd_pad=4)),
+    ("gelu_fp16_fp16_N200", "fp16", "fp16", E.EPI_GELU, 200, 64, dict(bias=True)),
+    ("gelu_aux_bf16_bf16_N512", "bf16", "bf16", E.EPI_GELU, 512, 64, dict(bias=True, aux=True, ldd_pad=16)),
+    ("gelu_aux_fp16_fp16_N200", "fp16", "fp16", E.EPI_GELU, 200, 128, dict(bias=True, aux=True)),
+    ("scale_res_inplace_bf16_bf16_N512", "bf16", "bf16", E.EPI_SCALE_RESIDUAL, 512, 64, dict(bias=True, in_place=True, ldd_pad=8)),
+    ("scale_res_inplace_fp16_fp16_N136", "fp16", "fp16", E.EPI_SCALE_RESIDUAL, 136, 64, dict(bias=True, in_place=True)),
+    ("scale_res_bf16_fp32_N200", "bf16", "fp32", E.EPI_SCALE_RESIDUAL, 200, 96, dict(bias=True, ldr_pad=12, ldd_pad=4)),
+    ("scale_res_fp16_fp16_N520", "fp16", "fp16", E.EPI_SCALE_RESIDUAL, 520, 64, dict(bias=True, ldr_pad=8)),
+    ("layernorm_bf16_bf16_N200", "bf16", "bf16", E.EPI_LAYERNORM, 200, 64, dict(bias=True, ldd_pad=8)),
+    ("layernorm_fp16_fp32_N136", "fp16", "fp32", E.EPI_LAYERNORM, 136, 96, dict(bias=True)),
+    ("layernorm_bf16_fp16_N8", "bf16", "fp16", E.EPI_LAYERNORM, 8, 64, dict(bias=True)),
+    ("layernorm_bf16_bf16_N256", "bf16", "bf16", E.EPI_LAYERNORM, 256, 64, dict()),
+    ("gelu_grad_bf16_bf16_N512_tb", "bf16", "bf16", E.EPI_MUL_GELU_GRAD, 512, 64, dict(tb=1, ldr_pad=8)),
+    ("gelu_grad_fp16_fp16_N200", "fp16", "fp16", E.EPI_MUL_GELU_GRAD, 200, 96, dict(ldr_pad=8, ldd_pad=8)),
+    ("gelu_grad_bf16_fp16_N136_tb", "bf16", "fp16", E.EPI_MUL_GELU_GRAD, 136, 64, dict(tb=1)),
+]
+
+
+def regime_case(case_id, in_dtype, out_dtype, epilogue, N, K, opts, tiles_per_cta=3, exact_tiles=None):
+    sm = sm_count()
+    BN = tile_n(N, epilogue)
+    num_n = -(-N // BN)
+    if exact_tiles is not None:
+        row_tiles = -(-exact_tiles // num_n)
+        assert row_tiles * num_n == exact_tiles
+    else:
+        row_tiles = -(-tiles_per_cta * sm // num_n) + 1
+    M = row_tiles * 128 - 40 if opts.get("ta") else row_tiles * 128 - 37  # trans_a needs M % 8 == 0
+    tiles = row_tiles * num_n
+    if exact_tiles is None:
+        assert tiles >= tiles_per_cta * sm, (tiles, sm)
+    seed = sum(map(ord, case_id))
+    a, b = operands(M, N, K, in_dtype, seed, 0.5, 0.25)
+    odt = DT[out_dtype][0]
+    dev = "cuda"
+    bias = torch.randn(N, device=dev) if opts.get("bias") else None
+    gamma = beta = residual = None
+    if epilogue == E.EPI_SCALE_RESIDUAL:
+        gamma = torch.rand(N, device=dev) * 2 - 0.5
+        residual = torch.randn(M, N, device=dev).to(odt)
+    elif epilogue == E.EPI_LAYERNORM:
+        gamma = torch.rand(N, device=dev) + 0.5
+        beta = torch.randn(N, device=dev)
+    elif epilogue == E.EPI_MUL_GELU_GRAD:
+        residual = (3 * torch.randn(M, N, device=dev)).to(odt)
+    d, ax = run(a, b, odt, epilogue, bias=bias, gamma=gamma, beta=beta, residual=residual, ldr_pad=opts.get("ldr_pad", 0),
+                ldd_pad=opts.get("ldd_pad", 0), aux=opts.get("aux", False), ta=opts.get("ta", 0), tb=opts.get("tb", 0),
+                in_place=opts.get("in_place", False))
+    check_epilogue(a, b, odt, epilogue, d, ax, bias=bias, gamma=gamma, beta=beta, residual=residual, name=case_id)
+
+
+@pytest.mark.parametrize("case_id,in_dtype,out_dtype,epilogue,N,K,opts", REGIME, ids=[c[0] for c in REGIME])
+def test_gemm_epilogue_persistent_regime(lib, case_id, in_dtype, out_dtype, epilogue, N, K, opts):
+    regime_case(case_id, in_dtype, out_dtype, epilogue, N, K, opts)
+
+
+def test_gemm_exactly_one_tile_more_than_sms(lib):
+    """SM + 1 tiles of 128 x 128: one CTA runs a second tile, with the saved pre-activation and a bias."""
+    regime_case("gelu_aux_sm_plus_1", "bf16", "bf16", E.EPI_GELU, 128, 64, dict(bias=True, aux=True),
+                exact_tiles=sm_count() + 1)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# LayerNorm edges
+
+
+@pytest.mark.parametrize("offset", [0.0, 1e4])
+@pytest.mark.parametrize("N,out_dtype", [(8, "bf16"), (136, "fp32"), (200, "bf16"), (256, "fp16")])
+def test_gemm_layernorm_constant_rows_and_offset(lib, N, out_dtype, offset):
+    """Every third row of A is zero, so its row of acc + bias is the constant bias `offset + 3`: variance 0 and the output is
+    beta exactly.  With offset 1e4 the other rows have mean ~1e4 and spread ~1 (the fp32 rounding of x = acc + bias at 1e4 is
+    what the bound's 2^-24 |x| term carries).  Multi-tile M (>= 3 tiles per CTA)."""
+    sm = sm_count()
+    M = (3 * sm + 1) * 128 - 5
+    a, b = operands(M, N, 64, "bf16", N, 0.5, 0.25)
+    a[::3] = 0
+    bias = torch.full((N,), offset + 3.0, device="cuda")
+    gamma = torch.rand(N, device="cuda") + 0.5
+    beta = torch.randn(N, device="cuda")
+    odt = DT[out_dtype][0]
+    d, _ = run(a, b, odt, E.EPI_LAYERNORM, bias=bias, gamma=gamma, beta=beta, ldd_pad=8)
+    check_epilogue(a, b, odt, E.EPI_LAYERNORM, d, None, bias=bias, gamma=gamma, beta=beta, name=f"layernorm N{N} +{offset}")
+    const = d.view[::3]
+    assert torch.equal(const, beta.to(odt).expand_as(const)), "rows of zero variance must equal beta"
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# activation sweeps: one-hot A rows make the accumulator equal chosen 16-bit values exactly
+
+
+def finite_values(dtype):
+    v = torch.arange(-32768, 32768, dtype=torch.int32, device="cuda").to(torch.int16).view(dtype)
+    return v[torch.isfinite(v)]
+
+
+def one_hot(M, K, dtype):
+    a = torch.zeros(M, K, device="cuda", dtype=dtype)
+    a[torch.arange(M), torch.arange(M) % K] = 1
+    return a
+
+
+@pytest.mark.parametrize("in_dtype,out_dtype,aux", [("bf16", "fp32", False), ("bf16", "bf16", True),
+                                                    ("fp16", "fp16", False), ("fp16", "fp16", True)])
+def test_gemm_gelu_sweeps_every_16bit_value(lib, in_dtype, out_dtype, aux):
+    """acc[m, n] = B[n, m % 64] runs through every finite value x of the input type.  The epilogue's GELU is within
+    GELU_REL_ERR |x| of fp64 erf-GELU plus the output rounding (fp32: 2^-24 |ref|, 16-bit: one ulp); y == x exactly for
+    x >= 8 and y == 0 for x <= -8 (tanh saturates to +-1 in fp16, gemm.cu); the saved pre-activation equals x."""
+    dt, odt = DT[in_dtype][0], DT[out_dtype][0]
+    vals = finite_values(dt)
+    K, N = 64, 1024
+    b = torch.zeros(N * K, dtype=dt, device="cuda")
+    b[:vals.numel()] = vals
+    b = b.view(N, K)
+    a = one_hot(128, K, dt)
+    d, ax = run(a, b, odt, E.EPI_GELU, aux=aux)
+    x = (a.double() @ b.double().t())
+    if aux:
+        assert torch.equal(ax.view.double(), x), "the saved pre-activation must equal the accumulator"
+    y = d.view.double()
+    ref = gelu64(x)
+    rnd = 2.0 ** -24 * ref.abs() if odt == torch.float32 else ulp(ref, odt)
+    err = (y - ref).abs()
+    measured = float(((err - rnd).clamp_min(0) / x.abs().clamp_min(1e-300)).max())
+    print(f"GELU {in_dtype}->{out_dtype}{' aux' if aux else ''}: max (|err| - rounding) / |x| = {measured:.3e}")
+    check_within(y, ref, GELU_REL_ERR * x.abs() + rnd, f"gelu sweep {in_dtype}", describe_tiles(128, N, 256))
+    assert torch.equal(y[x >= 8], x[x >= 8])
+    assert bool((y[x <= -8] == 0).all())
+
+
+@pytest.mark.parametrize("in_dtype,out_dtype", [("bf16", "bf16"), ("fp16", "fp16"), ("bf16", "fp16")])
+def test_gemm_gelu_grad_sweeps_every_16bit_value(lib, in_dtype, out_dtype):
+    """acc = 1 everywhere, the saved pre-activation runs through every finite value of the output type (|x| up to 3.4e38 for
+    bf16, where fp16 conversion gives inf before the clamp to [-8, 8]): D = gelu~'(x) within GELU_GRAD_ERR of fp64
+    d/dx erf-GELU, plus one ulp of the output."""
+    dt, odt = DT[in_dtype][0], DT[out_dtype][0]
+    vals = finite_values(odt)
+    M, N, K = 128, 512, 64
+    pre = torch.zeros(M * N, dtype=odt, device="cuda")
+    pre[:vals.numel()] = vals
+    pre = pre.view(M, N)
+    a = one_hot(M, K, dt)
+    b = torch.ones(N, K, dtype=dt, device="cuda")
+    d, _ = run(a, b, odt, E.EPI_MUL_GELU_GRAD, residual=pre)
+    ref = gelu_grad64(pre.double())
+    y = d.view.double()
+    rnd = ulp(ref, odt)
+    measured = float(((y - ref).abs() - rnd).clamp_min(0).max())
+    print(f"GELU' {out_dtype}: max |err| - rounding = {measured:.3e}")
+    check_within(y, ref, GELU_GRAD_ERR + rnd, f"gelu' sweep {out_dtype}", describe_tiles(M, N, 256))

@@ -3,6 +3,7 @@ pinned against HF ViTModel on CPU).  bf16 activations vs the fp32 oracle: tolera
 import pytest
 import torch
 
+from kernel_ref import attention_reference, check_attention, check_within
 from oracle.vit import ViTWrapperOracle, randomize_
 from visiondk_b200 import _lib
 from visiondk_b200.backbone import BackboneFactory
@@ -17,18 +18,12 @@ def rel(a, b):
 
 @pytest.mark.parametrize("B,N,H", [(2, 197, 12), (3, 64, 3), (1, 577, 4), (2, 50, 2), (2, 1, 1)])
 def test_attention_forward_matches_torch(lib, B, N, H):
-    """softmax(q k^T / 8) v per (image, head) on the qkv Linear's output layout [B, N, 3, H, 64]; reference in fp32 on the same
-    bf16-rounded inputs.  P is rounded to bf16 before P.V: |err| <= 2^-8 relative to the largest |v| of the row."""
+    """softmax(q k^T / 8) v per (image, head) on the qkv Linear's output layout [B, N, 3, H, 64] through vdk_attention_fwd,
+    against the fp64 reference of the same bf16 inputs within the elementwise bound derived in kernel_ref.attention_reference
+    (P rounded to bf16 before P.V, the bf16 output rounding, and the fp32 score and row-sum errors); NaN guards around out."""
     torch.manual_seed(N * 7 + H)
     qkv = (torch.randn(B, N, 3, H, 64, device="cuda") * 1.5).to(torch.bfloat16)
-    out = torch.full((B, N, H * 64), float("nan"), dtype=torch.bfloat16, device="cuda")
-    _lib.check(lib.vdk_attention_fwd(qkv.data_ptr(), B, N, H, 64, out.data_ptr(), _lib.stream_ptr()), "attention")
-    q, k, v = qkv.float().permute(2, 0, 3, 1, 4).unbind(0)  # [B, H, N, 64]
-    ref = torch.softmax((q @ k.transpose(-2, -1)) * 0.125, dim=-1) @ v
-    ref = ref.transpose(1, 2).reshape(B, N, H * 64)
-    assert torch.isfinite(out.float()).all()
-    assert (out.float() - ref).abs().max().item() <= 2e-2 * v.abs().max().item()
-    assert rel(out, ref) <= 1e-2
+    check_attention(lib, qkv, with_lse=False)
 
 
 def build(seed, **kw):
@@ -118,9 +113,9 @@ def test_attention_backward_matches_torch_autograd(lib, B, N, H):
     q, k, v = x.permute(2, 0, 3, 1, 4).unbind(0)
     ref = (torch.softmax((q @ k.transpose(-2, -1)) * 0.125, dim=-1) @ v).transpose(1, 2).reshape(B, N, H * 64)
     ref.backward(dout.float())
-    # the saved log-sum-exp (log2 domain) equals torch's logsumexp of the scaled scores
-    lse_ref = torch.logsumexp((q @ k.transpose(-2, -1)) * 0.125, dim=-1) * 1.4426950408889634
-    assert (lse - lse_ref.detach()).abs().max().item() <= 2e-2
+    # the saved log-sum-exp (log2 domain) against the fp64 logsumexp of the scaled scores, within its derived bound
+    _, _, lse_ref, lse_bound = attention_reference(qkv)
+    check_within(lse, lse_ref, lse_bound, "lse2", lambda bad: f"{int(bad.sum())} rows")
     assert torch.isfinite(dqkv.float()).all()
     for i, name in enumerate("qkv"):
         assert rel(dqkv[:, :, i], x.grad[:, :, i]) <= 2e-2, (name, rel(dqkv[:, :, i], x.grad[:, :, i]))

@@ -66,8 +66,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
 // cost few issue slots and at most one SFU op per pair of elements or the epilogue, not the MMA, sets the pace.
 // y = 0.5 x (1 + tanh(u)), u = x (c1 + c3 x^2) with (c1, c3) refitted to the erf form (max |dev| 3.1e-4 instead of the
 // textbook tanh-GELU's 4.7e-4); u and tanh are evaluated two elements at a time in fp16x2 (tanh.approx.f16x2,
-// rel. error 2^-11), the final multiply in fp32 so that y -> x exactly for large x.  Absolute error <= 6e-4 |x|:
-// below one bf16 ulp of the typical activation; stated in the tests.
+// rel. error 2^-11), the final multiply in fp32 so that y -> x exactly for large x.  Absolute error <= 6e-4 |x| before the
+// output rounding (4.3e-4 |x| measured over every finite bf16 / fp16 x, tests/test_gemm_gpu.py): below one bf16 ulp.
 __device__ __forceinline__ void gelu_pair(float& x0, float& x1) {
   const __half2 h = __floats2half2_rn(x0, x1);
   const __half2 t = __hmul2(h, h);
@@ -84,7 +84,9 @@ __device__ __forceinline__ void gelu_pair(float& x0, float& x1) {
 // d/dx of the forward's GELU form 0.5 x (1 + tanh(u)), u = x (c1 + c3 x^2), two elements at a time in fp16x2 like the
 // forward (the fc2 data-gradient epilogue evaluates 4C x tokens of these per block): x is clamped to [-8, 8], where
 // the derivative has reached 1 / 0 to fp16 precision, so that x^2 (1 - tanh^2) cannot overflow into inf * 0.
-// Absolute error <= 2e-3 (fp16 tanh.approx + fp16 arithmetic): below the bf16 rounding of the gradient it scales.
+// Absolute error <= 8e-3 before the output rounding (7.6e-3 measured over every finite bf16 / fp16 x, tests/test_gemm_gpu.py;
+// 7.4e-4 of it is the fitted form's own derivative error): the worst case is near |x| = 3, where the error of
+// tanh.approx.f16 in 1 - tanh^2 is multiplied by x (c1 + 3 c3 x^2) ~ 5.  About two bf16 ulps of a gradient of order 1.
 __device__ __forceinline__ float2 gelu_grad_pair(float x0, float x1) {
   const __half2 lim = __floats2half2_rn(8.0f, 8.0f);
   const __half2 h = __hmax2(__hmin2(__floats2half2_rn(x0, x1), lim), __hneg2(lim));
