@@ -213,8 +213,10 @@ int vdk_convnext_train_backward_range(const vdk_convnext_net* net, const vdk_con
 /* Building blocks of the backward, exported for unit parity tests (NHWC bf16 activations, fp32 parameter grads +=):
  *   vdk_dwconv7             mode 0: LayerNorm_C(dwconv7(x)+bias) (rstd_out optional); mode 1: dwconv7(x) with `w49` (+addend)
  *                           — with reversed taps this is the depthwise backward-data pass
- *   vdk_dwconv7_wgrad       dw49[tap][c] += sum dconv * shifted x; dbias[c] += sum dconv
- *   vdk_layernorm_bwd       LayerNorm backward from the saved OUTPUT y and 1/sigma (patch = 2: through the 2x2 regrouping)
+ *   vdk_dwconv7_wgrad       dw49[tap][c] += sum dconv * shifted x; dbias[c] += sum dconv (C a multiple of 8)
+ *   vdk_layernorm_bwd       LayerNorm backward from the saved OUTPUT y and 1/sigma (patch = 2: through the 2x2 regrouping;
+ *                           C a multiple of 8, <= 1536).  xhat = (y - beta) / gamma carries ulp(y) / (2 |gamma|) of error,
+ *                           |beta / gamma| / |xhat| times bf16 precision; gamma = 0 takes xhat = 0 (that dgamma gets nothing)
  *   vdk_batchnorm_train_*   BatchNorm over the rows of [rows, C] with batch statistics (running stats updated) */
 int vdk_dwconv7(int mode, const void* x, int batch, int H, int W, int C, const float* w49, const float* bias,
                 const float* ln_w, const float* ln_b, float eps, void* y, float* rstd_out, const void* addend, void* stream);

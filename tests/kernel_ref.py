@@ -189,3 +189,344 @@ def check_attention(lib, qkv, stats=None, with_lse=True):
         check_within(lse.view.view(B, H, N), lse_ref, lse_b, "attention lse2", lambda bad: describe_attention(bad, N, H, sm), stats)
         assert not lse.guard_errors(), "lse2: " + lse.guard_errors()
     return got
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# ConvNeXt HBM-bound kernels (csrc/convnext.cu, csrc/train_ops.cu): launch arithmetic, fp64 references and bounds.
+# Every reference takes the kernel's own bf16 / fp32 inputs and is computed in fp64 on the device.
+
+A32 = 2.0 ** -24   # fp32 unit roundoff
+WG_T, WG_C = 14, 64
+
+
+def wgrad_launch(B, H, W, C, sm_count):
+    """launch_dwconv7_wgrad: tile edge T, strips per tile row nh, images per CTA ipc, image groups, tiles per image, chunks."""
+    T = min(WG_T, max(H, W))
+    tiles = -(-H // T) * -(-W // T)
+    chunks = -(-C // WG_C)
+    ipc = max(1, min(16, tiles * chunks * B // (sm_count * 4)))
+    return dict(T=T, nh=-(-T // 7), ipc=ipc, groups=-(-B // ipc), tiles=tiles, chunks=chunks)
+
+
+def ln_bwd_launch(npix, C, sm_count):
+    """launch_ln_bwd: (LPP, IT, U), blocks, pixels per warp trip, and the fewest trips any warp makes."""
+    vecs = C // 8
+    lpp, it, u = next(cfg for lim, cfg in ((8, (8, 1, 4)), (16, (16, 1, 4)), (32, (32, 1, 4)), (64, (32, 2, 2)),
+                                          (96, (32, 3, 1)), (128, (32, 4, 1)), (192, (32, 6, 1))) if vecs <= lim)
+    ppt = (32 // lpp) * u
+    blocks = max(1, min(-(-npix // (8 * ppt)), sm_count * (1 if it >= 4 else 2)))
+    nwarps = 8 * blocks
+    last = npix - (nwarps - 1) * ppt  # pixels left to the last warp after its first base
+    return dict(lpp=lpp, it=it, u=u, blocks=blocks, ppt=ppt, nwarps=nwarps,
+                min_trips=max(0, -(-last // (nwarps * ppt))) if last > 0 else 0,
+                max_trips=-(-npix // (nwarps * ppt)))
+
+
+def dwconv7_reference(x, w49):
+    """fp64 correlation out[b, y, x, c] = sum_{dy, dx} w49[7 dy + dx, c] x[b, y + dy - 3, x + dx - 3, c] (zero padding)
+    of NHWC x with [49, C] taps, and sum |w x| over the same 49 products."""
+    B, H, W, C = x.shape
+    xp = torch.nn.functional.pad(x.double(), (0, 0, 3, 3, 3, 3))
+    w = w49.double()
+    out = torch.zeros(B, H, W, C, dtype=torch.float64, device=x.device)
+    mag = torch.zeros_like(out)
+    for t in range(49):
+        dy, dx = divmod(t, 7)
+        p = xp[:, dy:dy + H, dx:dx + W, :] * w[t]
+        out += p
+        mag += p.abs()
+    return out, mag
+
+
+def dwconv7_bwd_data_bound(ref, mag, addend):
+    """Bound of mode 1 (vdk_dwconv7(1, ...): out = bf16(sum_49 w x + addend)), whatever the order of its fp32 operations:
+      49 FMAs and one add of the addend, each one rounding of a partial sum bounded by sum |w x| + |addend|:
+        |fp32 result - exact| <= 50 * 2^-24 * (mag + |addend|)
+      bf16 store: half an ulp of the fp32 result, <= ulp_bf16(|ref| + e32) / 2."""
+    a = addend.double().abs() if addend is not None else 0.0
+    e32 = 50 * A32 * (mag + a) * 1.001
+    return e32 + 0.5 * ulp(ref.abs() + e32, torch.bfloat16)
+
+
+def wgrad_reference(x, g):
+    """fp64 dw49 [49, C] = sum_{b,y,x} g[b,y,x,c] x[b,y+dy-3,x+dx-3,c], dbias [C] = sum g, and their sums of |terms|."""
+    B, H, W, C = x.shape
+    xp = torch.nn.functional.pad(x.double(), (0, 0, 3, 3, 3, 3))
+    gd = g.double()
+    dw = torch.empty(49, C, dtype=torch.float64, device=x.device)
+    dw_mag = torch.empty_like(dw)
+    for t in range(49):
+        dy, dx = divmod(t, 7)
+        p = gd * xp[:, dy:dy + H, dx:dx + W, :]
+        dw[t] = p.sum((0, 1, 2))
+        dw_mag[t] = p.abs().sum((0, 1, 2))
+    return dw, dw_mag, gd.sum((0, 1, 2)), gd.abs().sum((0, 1, 2))
+
+
+def wgrad_bound(mag, init, launch):
+    """Bound of vdk_dwconv7_wgrad (dw49 += ..., dbias += ...) for one output element.
+    Kernel order (train_ops.cu): bf16 x bf16 products are exact in fp32.  A thread chains ipc x T x 7 FMAs (its images,
+    tile rows, strip pixels); nh strip partials are added in shared memory; every CTA (image group x tile) adds its
+    partial to the output with one fp32 atomic, starting from the output's initial value.  Each rounding is at most
+    2^-24 of a partial sum bounded by sum |terms| + |init|, and no term passes more than
+        n = ipc * T * 7 + nh + groups * tiles
+    roundings:  |got - (init + exact)| <= n 2^-24 (sum |terms| + |init|)."""
+    n = launch["ipc"] * launch["T"] * 7 + launch["nh"] + launch["groups"] * launch["tiles"]
+    return n * A32 * (mag + init.double().abs()) * 1.001
+
+
+def layernorm_bwd_reference(xhat, rstd64, gamma, dy, addend, patch):
+    """fp64 LayerNorm backward from the exact normalised input xhat [P, C] (pixel rows of NHWC order) and exact rstd64 [P]:
+    dx = rstd (g - mean_c g - xhat mean_c(g xhat)) + addend with g = dy gamma; dgamma = sum_p dy xhat; dbeta = sum_p dy.
+    dy [P, C] is given in pixel order (the caller undoes the patch layout)."""
+    g = dy.double() * gamma.double()
+    m1 = g.mean(-1, keepdim=True)
+    m2 = (g * xhat).mean(-1, keepdim=True)
+    dx = rstd64[:, None] * (g - m1 - xhat * m2)
+    if addend is not None:
+        dx = dx + addend.double()
+    return dx, (dy.double() * xhat).sum(0), dy.double().sum(0), m1, m2
+
+
+def layernorm_bwd_bound(xhat, rstd64, gamma, beta, y, dy, addend, m1, m2, launch, dg_init, db_init):
+    """Elementwise bounds of vdk_layernorm_bwd (dx, dgamma, dbeta), all fp64; a = 2^-24, n1 = 8 IT + log2(LPP).
+
+    Kernel order (train_ops.cu) per pixel, channel:
+      h = (y - beta) * fl(1/gamma): y is the SAVED bf16 output, e_y = |y - (gamma xhat + beta)| <= ulp(y) / 2, so
+          |h - xhat| <= dh = e_y / |gamma| + 3 a |y - beta| / |gamma|          (gamma = 0: h = 0, dh = |xhat|)
+          -- the recovered xhat loses |beta / gamma| / |xhat| times more than bf16 precision when beta dominates y --
+      g = fl(dy gamma): a |dy gamma|
+      s1 = sum_c g, s2 = sum_c g h: 8 IT sequential adds per lane + log2(LPP) shuffles, then x fl(1/C):
+          |m1 - M1| <= (n1 + 3) a mean|g|,  |m2 - M2| <= (n1 + 3) a mean(|g| (|xhat| + dh)) + mean(|g| dh)
+      o = fl(rstd) * (g - m1 - h m2) (+ addend), bf16 store:
+          |inner - INNER| <= a |g| + dm1 + dh |M2| + (|xhat| + dh) dm2 + 3 a (|g| + |M1| + |xhat M2|)
+          |o - dx| <= rstd |inner - INNER| + 3 a rstd (|g| + |M1| + |xhat M2|) + a |dx|, then half a bf16 ulp.
+      dgamma, dbeta: a lane chains U x trips pixels, then log2(32 / LPP) shuffles, 8 warps' shared atomics and one global
+          atomic per block onto the initial value: n = U trips + log2(32/LPP) + 8 + blocks + 1 roundings of partial sums
+          bounded by sum_p |dy| (|xhat| + dh) + |init| (dgamma; plus sum_p |dy| dh from h itself), sum_p |dy| + |init| (dbeta)."""
+    a = A32
+    gm = gamma.double()
+    zero = gm == 0
+    ag = gm.abs().masked_fill(zero, 1.0)
+    e_y = (y.double() - (gm * xhat + beta.double())).abs()
+    dh = torch.where(zero, xhat.abs(), e_y / ag + 3 * a * (y.double() - beta.double()).abs() / ag)
+    gabs = (dy.double() * gm).abs()
+    n1 = 8 * launch["it"] + int(math.log2(launch["lpp"]))
+    dm1 = (n1 + 3) * a * gabs.mean(-1, keepdim=True)
+    dm2 = (n1 + 3) * a * (gabs * (xhat.abs() + dh)).mean(-1, keepdim=True) + (gabs * dh).mean(-1, keepdim=True)
+    mag = gabs + m1.abs() + (xhat * m2).abs()
+    inner = a * gabs + dm1 + dh * m2.abs() + (xhat.abs() + dh) * dm2 + 3 * a * mag
+    dx_ref_abs = rstd64[:, None] * (gabs + m1.abs() + (xhat * m2).abs())
+    if addend is not None:
+        dx_ref_abs = dx_ref_abs + addend.double().abs()
+    e32 = (rstd64[:, None] * inner + 3 * a * rstd64[:, None] * mag + a * dx_ref_abs) * 1.01
+    dyd = dy.double().abs()
+    n = launch["u"] * launch["max_trips"] + int(math.log2(32 // launch["lpp"])) + 8 + launch["blocks"] + 1
+    dg_b = (n * a * ((dyd * (xhat.abs() + dh)).sum(0) + dg_init.double().abs()) + (dyd * dh).sum(0)) * 1.01
+    db_b = n * a * (dyd.sum(0) + db_init.double().abs()) * 1.01
+    return e32, dg_b, db_b
+
+
+def bf16_store_bound(ref, e32):
+    """e32 plus half a bf16 ulp of the (fp32) value that was rounded."""
+    return e32 + 0.5 * ulp(ref.abs() + e32, torch.bfloat16)
+
+
+def describe_pixels(bad_pix, npix, launch):
+    """bad_pix: bool [npix] -> the ln_bwd warps and grid-stride trips that wrote them."""
+    idx = bad_pix.nonzero().flatten()
+    slot = idx // launch["ppt"]
+    warp, trip = slot % launch["nwarps"], slot // launch["nwarps"]
+    return (f"{idx.numel()}/{npix} pixels wrong; first pixels {idx[:6].tolist()} on warps {warp[:6].tolist()} (blocks "
+            f"{(warp[:6] // 8).tolist()}) in trips {trip[:6].tolist()}; wrong pixels per trip {torch.bincount(trip).tolist()}")
+
+
+def describe_wgrad(bad, launch):
+    """bad: bool [49 or 1, C] -> the taps and 64-channel chunks whose atomics were wrong."""
+    idx = bad.nonzero()
+    chunks = torch.unique(idx[:, 1] // WG_C).tolist()
+    return (f"{idx.shape[0]} outputs wrong in 64-channel chunks {chunks[:8]} (launch {launch}); first (tap, channel) "
+            f"{idx[:6].tolist()}")
+
+
+# ---- depthwise forward / backward-data dispatch (launch_dwconv7) ----
+DW_TW = 7        # kDwTW: output columns of a persistent / chunk-kernel tile
+LN_NS = 32       # deepest fp32 reduction tree of a LayerNorm statistic in the three depthwise kernels (see dwconv7_ln_bound)
+
+
+def dwconv_launch(B, H, W, C, sm_count, pipe=True):
+    """The kernel launch_dwconv7 picks and its tiling.  Persistent kernel: CHUNK, nchunks, TH (14 unless H <= 7), tiles,
+    the most co-resident groups sm_count * (2 if TH == 7 else 1) // nchunks (the occupancy query can only give fewer),
+    and the fewest tiles any group then runs.  `pipe=False` is VDK_DWCONV_PIPE=0 (the round-1 chunk kernel, one tile per
+    CTA).  Otherwise the all-channel fallback with tile edge T = 7 / 4 / 2."""
+    chunk = next((c for c in (128, 96, 64) if C % c == 0), 0)
+    if chunk and C // chunk <= 16:
+        n = C // chunk
+        if pipe:
+            TH = 14 if H > 7 else 7
+            tiles = B * -(-H // TH) * -(-W // DW_TW)
+            gmax = max(1, min(tiles, sm_count * (2 if TH == 7 else 1) // n))
+            return dict(kind="pipe", chunk=chunk, nchunks=n, TH=TH, TW=DW_TW, tiles=tiles, groups_max=gmax,
+                        min_tiles_per_group=tiles // gmax)
+        TH = min(7, H)
+        return dict(kind="chunk", chunk=chunk, nchunks=n, TH=TH, TW=DW_TW, tiles=B * -(-H // TH) * -(-W // DW_TW))
+    T = 7
+    while T > 2 and (T + 6) ** 2 * C * 2 > 200 * 1024:
+        T = 4 if T == 7 else 2
+    return dict(kind="fallback", chunk=0, nchunks=1, T=T, TH=min(T, H), TW=T, tiles=B * -(-H // min(T, H)) * -(-W // T))
+
+
+def describe_dw_tiles(bad, launch):
+    """bad: bool [B, H, W, C] -> the tiles holding failures, and for the persistent kernel the group (CTA or cluster) and
+    round that ran them (tile t runs on group t % groups in round t // groups, at the largest possible grid)."""
+    B, H, W, _ = bad.shape
+    th, tw = launch["TH"], launch["TW"]
+    tiles_h, tiles_w = -(-H // th), -(-W // tw)
+    idx = bad.any(-1).nonzero()
+    t = torch.unique((idx[:, 0] * tiles_h + idx[:, 1] // th) * tiles_w + idx[:, 2] // tw)
+    msg = f"{int(bad.any(-1).sum())} pixels wrong in {t.numel()}/{launch['tiles']} {th}x{tw} tiles {t[:6].tolist()}"
+    if launch["kind"] == "pipe":
+        g = launch["groups_max"]
+        msg += f"; groups {(t[:6] % g).tolist()}, rounds {(t[:6] // g).tolist()}; wrong tiles per round {torch.bincount(t // g).tolist()}"
+    if launch.get("chunk"):
+        ch = torch.unique(bad.nonzero()[:, 3] // launch["chunk"]).tolist()
+        msg += f"; channel chunks {ch[:8]}"
+    return msg + f" ({launch['kind']})"
+
+
+def dwconv7_ln_reference(x, w49, bias, gamma, beta, eps):
+    """fp64 mode-0 forward: z = conv + bias, y = LayerNorm_C(z) gamma + beta and rstd = 1 / sqrt(var_C(z) + eps), plus
+    what dwconv7_ln_bound needs."""
+    conv, mag = dwconv7_reference(x, w49)
+    z = conv + bias.double()
+    mu = z.mean(-1, keepdim=True)
+    d = z - mu
+    var = d.pow(2).mean(-1)
+    r = (var + eps).rsqrt()
+    y = d * r[..., None] * gamma.double() + beta.double()
+    return dict(z=z, mag=mag + bias.double().abs(), mu=mu, d=d, var=var, rstd=r, y=y)
+
+
+def dwconv7_ln_bound(ref, gamma, beta, eps, chunk):
+    """Bounds of vdk_dwconv7 mode 0 (y = bf16(LayerNorm_C(conv + bias) gamma + beta)) and of rstd_out; a = 2^-24.
+
+    Kernel order (convnext.cu): z~ = bias + 49 FMAs in fp32:  |z~ - z| <= ez = 50 a mag.
+      Statistics, two-pass per channel chunk and Chan's combination across the chunks of a pixel (persistent and chunk
+      kernels), or two-pass over all of C (fallback).  Every sum is a tree of at most NS = 32 fp32 roundings (4 channels
+      per thread, 5 shuffle levels, <= 16 partials across warps or chunks, x 1/n and its rounding):
+        mean:  |mu~ - mu| <= e_mu = NS a mean|z| + mean(ez)
+        centred sum of squares Q = sum (z - mu)^2: the computed one differs by at most
+               (NS + 2) a Q + 2 sum |z - mu| ez + sum ez^2 + C e_mu^2     (a wrong mean adds C (mu~ - mu)^2 only)
+               + 2 CHUNK sum_k |m_k - mu| e_mu_k                           (Chan: d_k = m~_k - mu~ carries the chunk mean error)
+        rstd = rsqrtf(Q / C + eps): relative error e_r = e_Q / (2 (Q + C eps)) + 2^-22 + 2a   -> rstd_out's bound
+      y = (z~ - mu~) rstd gamma + beta: |dxhat| <= rstd (ez + e_mu) + |xhat| e_r, then 4 fp32 roundings on
+      |gamma xhat| + |beta| and half a bf16 ulp."""
+    a = A32
+    z, d, r = ref["z"], ref["d"], ref["rstd"]
+    C = z.shape[-1]
+    ez = 50 * a * ref["mag"]
+    e_mu = LN_NS * a * z.abs().mean(-1, keepdim=True) + ez.mean(-1, keepdim=True)
+    Q = d.pow(2).sum(-1)
+    eQ = (LN_NS + 2) * a * Q + 2 * (d.abs() * ez).sum(-1) + ez.pow(2).sum(-1) + C * e_mu[..., 0] ** 2
+    if chunk and C > chunk:
+        zk = z.unflatten(-1, (C // chunk, chunk))
+        e_mu_k = LN_NS * a * zk.abs().mean(-1) + ez.unflatten(-1, (C // chunk, chunk)).mean(-1)
+        eQ = eQ + 2 * chunk * ((zk.mean(-1) - ref["mu"]).abs() * e_mu_k).sum(-1)
+    e_r = (eQ / (2 * (Q + C * eps)) + 2.0 ** -22 + 2 * a) * 1.01
+    xhat = d * r[..., None]
+    dxh = r[..., None] * (ez + e_mu) + xhat.abs() * e_r[..., None]
+    g = gamma.double().abs()
+    e32 = (g * dxh + 4 * a * (g * xhat.abs() + beta.double().abs())) * 1.01
+    return e32 + 0.5 * ulp(ref["y"].abs() + e32, torch.bfloat16), r * e_r
+
+
+def layernorm_bwd_dgamma(y, beta, gamma, dy, launch, dg_init):
+    """dgamma of vdk_layernorm_bwd against the xhat the kernel can see, xh = (y - beta) / gamma in fp64 from the saved y
+    (channels with gamma = 0 excluded by the caller).  The kernel's h = (y - beta) * fl(1 / gamma) carries 3 a |xh|;
+    dy * h is chained over U x trips pixels per lane, log2(32 / LPP) shuffles, 8 shared and one global atomic per block:
+        |dgamma - init - sum dy xh| <= n a (sum |dy xh| + |init|) + 3 a sum |dy xh|,  n as in layernorm_bwd_bound."""
+    a = A32
+    gm = gamma.double()
+    xh = (y.double() - beta.double()) / gm.masked_fill(gm == 0, 1.0)
+    t = dy.double() * xh
+    n = launch["u"] * launch["max_trips"] + int(math.log2(32 // launch["lpp"])) + 8 + launch["blocks"] + 1
+    return dg_init.double() + t.sum(0), ((n * a) * (t.abs().sum(0) + dg_init.double().abs()) + 3 * a * t.abs().sum(0)) * 1.01
+
+
+# ---- BatchNorm with batch statistics over the rows of [R, C] (train_ops.cu) ----
+def bn_rows_depth(R):
+    """Roundings of a column sum: a thread chains ceil(R / 8) rows (generic kernels: 8 warps stride the rows; the vector
+    kernel's 256 threads chain fewer), then <= 5 shuffles and 8 per-warp partials."""
+    return -(-R // 8) + 16
+
+
+def batchnorm_fwd_reference(x, weight, bias, eps, momentum, rm, rv):
+    xd = x.double()
+    R = xd.shape[0]
+    mu = xd.mean(0)
+    d = xd - mu
+    var = d.pow(2).mean(0)
+    r = (var + eps).rsqrt()
+    y = d * r * weight.double() + bias.double()
+    return dict(x=xd, mu=mu, d=d, var=var, rstd=r, y=y, rm=(1 - momentum) * rm.double() + momentum * mu,
+                rv=(1 - momentum) * rv.double() + momentum * var * R / (R - 1))
+
+
+def batchnorm_fwd_bound(ref, weight, bias, eps, momentum, rm, rv, out_dtype):
+    """Bounds of vdk_batchnorm_train_fwd; a = 2^-24, n = bn_rows_depth(R).
+      mean: e_mu = (n + 2) a mean|x|;  Q = sum (x - mu)^2: e_Q = (n + 3) a Q + R e_mu^2 (a wrong mean adds R e_mu^2 only)
+      rstd = rsqrtf(Q / R + eps): e_r = e_Q / (2 (Q + R eps)) + 2^-22 + 2a relative
+      y: the generic kernels form (x - mu) rstd w + b; the vector kernel fma(x, rstd w, b - mu rstd w), which cancels
+      when |mu| >> std: |dy| <= |w| (rstd e_mu + |xhat| e_r) + 4 a (|x| + |mu|) rstd |w| + 4 a |b|, then the output
+      rounding (half a bf16 ulp, or a |y| in fp32)
+      running_mean: 3 a (|(1-m) rm| + |m mu|) + m e_mu;  running_var: 4 a (|(1-m) rv| + |m var_unbiased|) + m var_u e_Q / Q."""
+    a = A32
+    x, d, r = ref["x"], ref["d"], ref["rstd"]
+    R = x.shape[0]
+    n = bn_rows_depth(R)
+    e_mu = (n + 2) * a * x.abs().mean(0)
+    Q = d.pow(2).sum(0)
+    eQ = (n + 3) * a * Q + R * e_mu ** 2
+    e_r = (eQ / (2 * (Q + R * eps)) + 2.0 ** -22 + 2 * a) * 1.01
+    w, b = weight.double().abs(), bias.double().abs()
+    xhat = d * r
+    e32 = (w * (r * e_mu + xhat.abs() * e_r) + 4 * a * (x.abs() + ref["mu"].abs()) * r * w + 4 * a * b) * 1.01
+    yb = e32 + (0.5 * ulp(ref["y"].abs() + e32, torch.bfloat16) if out_dtype == torch.bfloat16 else a * (ref["y"].abs() + e32))
+    m = momentum
+    rm_b = 3 * a * ((1 - m) * rm.double().abs() + m * ref["mu"].abs()) + m * e_mu
+    vu = ref["var"] * R / (R - 1)
+    rv_b = 4 * a * ((1 - m) * rv.double().abs() + m * vu) + m * vu * eQ / Q.clamp_min(1e-300)
+    return yb, r * e_r, e_mu * 1.01, rm_b * 1.01, rv_b * 1.01
+
+
+def batchnorm_bwd_reference(x, dy, weight, save_mean, save_rstd):
+    """fp64 backward at the forward's saved fp32 statistics: xhat = (x - mean) rstd, dx = w rstd (dy - mean dy -
+    xhat mean(dy xhat)), dweight = sum dy xhat, dbias = sum dy."""
+    xhat = (x.double() - save_mean.double()) * save_rstd.double()
+    g = dy.double()
+    m1, m2 = g.mean(0), (g * xhat).mean(0)
+    dx = weight.double() * save_rstd.double() * (g - m1 - xhat * m2)
+    return dict(xhat=xhat, g=g, m1=m1, m2=m2, dx=dx, dw=(g * xhat).sum(0), db=g.sum(0))
+
+
+def batchnorm_bwd_bound(ref, weight, save_rstd, dw_init, db_init, out_dtype):
+    """Bounds of vdk_batchnorm_train_bwd; a = 2^-24, n = bn_rows_depth(R).  xh = (x - mean) rstd in fp32: 2a |xhat|
+    (the subtraction of a mean far from 0 included: it is relative to |x - mean|).
+      dbias += sum dy: n a (sum |dy| + |init|);  dweight += sum dy xh: n a (sum |dy xhat| + |init|) + 3 a sum |dy xhat|
+      m1 = s1 / R, m2 = s2 / R: (n + 2) a mean|dy|, (n + 2) a mean|dy xhat| + 3 a mean|dy xhat|
+      dx = w rstd (dy - m1 - xh m2): |w rstd| (dm1 + |xhat| dm2 + 2 a |xhat m2| + 3 a (|dy| + |m1| + |xhat m2|))
+           + 3 a |dx|, then the output rounding."""
+    a = A32
+    xhat, g = ref["xhat"], ref["g"]
+    R = g.shape[0]
+    n = bn_rows_depth(R)
+    t = (g * xhat).abs()
+    db_b = n * a * (g.abs().sum(0) + db_init.double().abs()) * 1.01
+    dw_b = (n * a * (t.sum(0) + dw_init.double().abs()) + 3 * a * t.sum(0)) * 1.01
+    dm1 = (n + 2) * a * g.abs().mean(0)
+    dm2 = (n + 5) * a * t.mean(0)
+    wr = (weight.double() * save_rstd.double()).abs()
+    inner = dm1 + xhat.abs() * dm2 + 2 * a * (xhat * ref["m2"]).abs() + 3 * a * (g.abs() + ref["m1"].abs() + (xhat * ref["m2"]).abs())
+    e32 = (wr * inner + 3 * a * ref["dx"].abs()) * 1.01
+    dxb = e32 + (0.5 * ulp(ref["dx"].abs() + e32, torch.bfloat16) if out_dtype == torch.bfloat16 else a * (ref["dx"].abs() + e32))
+    return dxb, dw_b, db_b

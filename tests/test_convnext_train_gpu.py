@@ -13,7 +13,7 @@ import torch.nn.functional as F
 
 from oracle.convnext import TimmWrapperOracle, randomize_
 from visiondk_b200 import _lib
-from visiondk_b200.backbone import TimmWrapper
+from visiondk_b200.backbone import CONVNEXT_ARCHS, TimmWrapper
 
 pytestmark = pytest.mark.gpu
 bf = lambda t: t.to(torch.bfloat16)
@@ -182,6 +182,45 @@ def test_train_forward_backward_matches_oracle_autograd(lib):
         assert rel(ours.output_layer[i].running_mean.cpu(), oracle.output_layer[i].running_mean) <= 2e-2
         assert rel(ours.output_layer[i].running_var.cpu(), oracle.output_layer[i].running_var) <= 2e-2
         assert int(ours.output_layer[i].num_batches_tracked) == 1
+
+
+@pytest.mark.parametrize("arch", sorted(CONVNEXT_ARCHS))
+def test_every_convnext_width_trains(lib, arch):
+    """Every CONVNEXT_ARCHS entry at depth (1, 1, 1, 1), 64^2, batch 4: stage widths 40 ... 1536 take the masked last
+    64-channel chunk of the depthwise weight gradient and the 1536-channel LayerNorm backward.  The per-parameter criteria
+    of test_train_forward_backward_matches_oracle_autograd (rel <= 6e-2, cos >= 0.995), except for one tensor: the last
+    block's fc2 bias gradient is the sum of only 16 bf16 rows of the residual-stream gradient, which nearly cancel behind
+    the batch-statistics BatchNorm (|ref| ~0.1); it measures rel 0.06-0.09 at cos >= 0.996 on the wider networks and is
+    held to rel <= 0.1, cos >= 0.995."""
+    dims = CONVNEXT_ARCHS[arch][1]
+    oracle, ours = build_pair(seed=13, depths=(1, 1, 1, 1), dims=dims)
+    torch.manual_seed(4)
+    x = torch.randn(4, 3, 64, 64)
+    wout = torch.randn(4, 64)
+    out_ref = oracle(x)
+    (out_ref * wout).sum().backward()
+    out = ours(x.cuda())
+    (out * wout.cuda()).sum().backward()
+    assert rel(out.detach().cpu(), out_ref.detach()) <= 3e-2
+    ref_grads = dict(oracle.named_parameters())
+    invariant = {"model.head.norm.weight", "model.head.norm.bias"}
+    bn_scale = ref_grads["output_layer.0.weight"].grad.abs().max().item()
+    bad, worst = [], []
+    for n, p in ours.named_parameters():
+        gr, g = ref_grads[n].grad, p.grad.detach().cpu()
+        assert torch.isfinite(g).all(), n
+        if n in invariant or gr.norm() < 1e-6 * (1 + gr.numel() ** 0.5):
+            if (g - gr).abs().max().item() > 5e-2 * bn_scale + 1e-3:
+                bad.append(f"{n}: |err| {(g - gr).abs().max().item():.3e} (exact gradient ~0)")
+            continue
+        r = rel(g, gr)
+        c = F.cosine_similarity(g.flatten(), gr.flatten(), dim=0).item()
+        worst.append((r, c, n))
+        if not (r <= (0.1 if n == "model.stages.3.blocks.0.mlp.fc2.bias" else 6e-2) and c >= 0.995):
+            bad.append(f"{n}: rel {r:.4f} cos {c:.5f} |ref| {gr.norm():.3e}")
+    for r, c, n in sorted(worst, reverse=True)[:4]:
+        print(f"  {arch} rel {r:.4f} cos {c:.5f} {n}")
+    assert not bad, "\n".join(bad)
 
 
 def test_convnext_base_224_training_gradients_match_oracle(lib):

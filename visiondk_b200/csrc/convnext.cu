@@ -75,7 +75,8 @@ dwconv7_ln_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W
   uint8_t* smem = dw_smem_raw + ((128u - (smem_u32(dw_smem_raw) & 127u)) & 127u);
   const int box_h = TH + 6, box_w = TW + 6;
   const int n_chunks = C / box_c;
-  const int chunk_bytes = box_h * box_w * box_c * 2;
+  const int box_bytes = box_h * box_w * box_c * 2;
+  const int chunk_bytes = (box_bytes + 127) & ~127;  // chunk stride: every TMA destination 128-byte aligned
   float* red = reinterpret_cast<float*>(smem + n_chunks * chunk_bytes);  // [group][TW][warps per group <= 16]
   uint64_t* bar = reinterpret_cast<uint64_t*>(red + 16 * TW * 16);
 
@@ -99,7 +100,7 @@ dwconv7_ln_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    mbar_arrive_expect_tx(bar, n_chunks * chunk_bytes);
+    mbar_arrive_expect_tx(bar, n_chunks * box_bytes);
     for (int ch = 0; ch < n_chunks; ++ch)
       tma_load_4d(smem + ch * chunk_bytes, &map_x, bar, ch * box_c, ox0 - 3, oy0 - 3, b);
   }
@@ -867,7 +868,7 @@ static int launch_dwconv_tw(const CUtensorMap& mx, int batch, int H, int W, int 
   const int tpg = ((C / 4) + 31) / 32 * 32;
   const int groups = std::max(1, std::min(512 / tpg, TH));
   const int n_chunks = C / box_c;
-  const int smem = n_chunks * (TH + 6) * (TW + 6) * box_c * 2 + 16 * TW * 16 * 4 + 16 + 128;
+  const int smem = n_chunks * (((TH + 6) * (TW + 6) * box_c * 2 + 127) & ~127) + 16 * TW * 16 * 4 + 16 + 128;
   auto kern = dwconv7_ln_kernel<TW, MODE>;
   VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   const unsigned grid = static_cast<unsigned>(batch) * ((H + TH - 1) / TH) * ((W + TW - 1) / TW);

@@ -80,11 +80,20 @@ int launch_col_sum(const __nv_bfloat16* x, int64_t M, int C, int ld, float* out,
 //   dgamma += sum_pixels dy * xh;  dbeta += sum_pixels dy
 // A pixel is shared by LPP lanes (IT 16-byte vectors each); a warp handles U x (32 / LPP) pixels per trip with all
 // of their loads issued before the first use (U * IT = 4 vectors of dy and of y in flight per lane), and the bf16
-// inputs stay packed in registers between the statistics pass and the output pass, so the kernel stays below 128
-// registers and HBM-bound. gamma / beta / 1/gamma live in shared memory; dgamma / dbeta are combined per warp by
-// shuffles, per block in shared memory, and leave as one global atomic per channel per block.
+// inputs stay packed in registers between the statistics pass and the output pass, so the narrow instantiations stay
+// within 128 registers and the kernel HBM-bound. gamma / beta / 1/gamma live in shared memory; dgamma / dbeta are
+// combined per warp by shuffles, per block in shared memory, and leave as one global atomic per channel per block.
+//
+// Accuracy: xh comes from the saved bf16 y, so it carries y's rounding amplified by 1/|gamma|: an error of up to
+// ulp_bf16(y) / (2 |gamma|) per element, which exceeds bf16 precision of xh itself once |beta / gamma| >> |xh|.  A
+// channel with gamma == 0 has no xh in y at all: it is taken as 0, so that channel's dx lacks its -xh * mean(g * xh)
+// term and its dgamma receives nothing (both finite).
+//
+// IT = 6 (C up to 1536, ConvNeXt-L stage 3) carries 96 dgamma / dbeta accumulators and runs at the 255-register cap
+// with a 36-byte spill (ptxas, sm_90a); IT = 3 and IT = 2 spill 200-400 bytes under their 128-register bound.
+
 template <int LPP, int IT, int U>
-__global__ void __launch_bounds__(256, IT == 4 ? 1 : 2)
+__global__ void __launch_bounds__(256, IT >= 4 ? 1 : 2)
 ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ y, const float* __restrict__ rstd,
               int B, int H, int W, int C, const float* __restrict__ ln_w, const float* __restrict__ ln_b, int patch,
               __nv_bfloat16* __restrict__ dx, const __nv_bfloat16* __restrict__ addend, float* __restrict__ dgamma,
@@ -99,9 +108,13 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restr
   float* s_db = s_dg + Cp;      // block partial of dbeta
   for (int c = threadIdx.x; c < Cp; c += 256) {
     float w = c < C ? ln_w[c] : 1.f;
-    if (fabsf(w) < 1e-12f) w = w < 0.f ? -1e-12f : 1e-12f;
+    float iw = 0.f;  // gamma == 0: y holds no trace of xh, which is taken as 0 (that channel's dgamma stays unknown)
+    if (w != 0.f) {
+      if (fabsf(w) < 1e-12f) w = w < 0.f ? -1e-12f : 1e-12f;
+      iw = 1.0f / w;
+    }
     s_w[c] = w;
-    s_iw[c] = 1.0f / w;
+    s_iw[c] = iw;
     s_b[c] = c < C ? ln_b[c] : 0.f;
     s_dg[c] = 0.f;
     s_db[c] = 0.f;
@@ -154,11 +167,11 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restr
       const int c = (sub + i * LPP) * 8;
       float w[8], iw[8], bb[8];
       *reinterpret_cast<float4*>(&w[0]) = *reinterpret_cast<const float4*>(s_w + c);
-      *reinterpret_cast<float4*>(&w[4]) = *reinterpret_cast<const float4*>(s_w + c + 4);
+            *reinterpret_cast<float4*>(&w[4]) = *reinterpret_cast<const float4*>(s_w + c + 4);
       *reinterpret_cast<float4*>(&iw[0]) = *reinterpret_cast<const float4*>(s_iw + c);
-      *reinterpret_cast<float4*>(&iw[4]) = *reinterpret_cast<const float4*>(s_iw + c + 4);
+            *reinterpret_cast<float4*>(&iw[4]) = *reinterpret_cast<const float4*>(s_iw + c + 4);
       *reinterpret_cast<float4*>(&bb[0]) = *reinterpret_cast<const float4*>(s_b + c);
-      *reinterpret_cast<float4*>(&bb[4]) = *reinterpret_cast<const float4*>(s_b + c + 4);
+            *reinterpret_cast<float4*>(&bb[4]) = *reinterpret_cast<const float4*>(s_b + c + 4);
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const bool okc = pix[u] < npix && c < C;
@@ -201,6 +214,10 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restr
             *reinterpret_cast<float4*>(&bb[0]) = *reinterpret_cast<const float4*>(s_b + c);
             *reinterpret_cast<float4*>(&bb[4]) = *reinterpret_cast<const float4*>(s_b + c + 4);
             float vdy[8], vy[8], o[8];
+            if constexpr (IT > 4) {  // recompute g and xh from the packed inputs rather than keep 16 IT floats live
+              asm volatile("" : "+r"(rdy[u][i].x), "+r"(rdy[u][i].y), "+r"(rdy[u][i].z), "+r"(rdy[u][i].w));
+              asm volatile("" : "+r"(ry[u][i].x), "+r"(ry[u][i].y), "+r"(ry[u][i].z), "+r"(ry[u][i].w));
+            }
             unpack8(rdy[u][i], vdy);
             unpack8(ry[u][i], vy);
 #pragma unroll
@@ -252,7 +269,7 @@ static void ln_bwd_launch(const __nv_bfloat16* dy, const __nv_bfloat16* y, const
   const int64_t npix = static_cast<int64_t>(B) * H * W;
   const int64_t pix_per_block_trip = 8 * (32 / LPP) * U;
   const int blocks = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>((npix + pix_per_block_trip - 1) / pix_per_block_trip,
-                                                                              sm_count() * (IT == 4 ? 1 : 2))));
+                                                                              sm_count() * (IT >= 4 ? 1 : 2))));
   const size_t smem = static_cast<size_t>(LPP) * IT * 8 * 5 * sizeof(float);
   ln_bwd_kernel<LPP, IT, U><<<blocks, 256, smem, s>>>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta);
 }
@@ -260,14 +277,15 @@ static void ln_bwd_launch(const __nv_bfloat16* dy, const __nv_bfloat16* y, const
 int launch_ln_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, const float* rstd, int B, int H, int W, int C,
                   const float* ln_w, const float* ln_b, int patch, __nv_bfloat16* dx, const __nv_bfloat16* addend,
                   float* dgamma, float* dbeta, cudaStream_t s) {
-  VDK_REQUIRE(C % 8 == 0 && C <= 1024, "ln_bwd: C must be a multiple of 8, <= 1024 (got %d)", C);
+  VDK_REQUIRE(C % 8 == 0 && C <= 1536, "ln_bwd: C must be a multiple of 8, <= 1536 (got %d)", C);
   const int vecs = C / 8;
   if (vecs <= 8) ln_bwd_launch<8, 1, 4>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);
   else if (vecs <= 16) ln_bwd_launch<16, 1, 4>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);
   else if (vecs <= 32) ln_bwd_launch<32, 1, 4>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);
   else if (vecs <= 64) ln_bwd_launch<32, 2, 2>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);
   else if (vecs <= 96) ln_bwd_launch<32, 3, 1>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);  // ViT-B: C = 768
-  else ln_bwd_launch<32, 4, 1>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);
+  else if (vecs <= 128) ln_bwd_launch<32, 4, 1>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);
+  else ln_bwd_launch<32, 6, 1>(dy, y, rstd, B, H, W, C, ln_w, ln_b, patch, dx, addend, dgamma, dbeta, s);  // ConvNeXt-L: C = 1536
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }
@@ -279,7 +297,9 @@ int launch_ln_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, const float* 
 // (zero-filled out of bounds, so no masks).  A thread owns 4 channels, ONE filter row dy and one 7-pixel half of
 // every tile row: per strip it reads 7 gradient and 13 input vectors for 7 x 7 x 4 FMAs (the 7 taps of its filter row
 // stay in 28 registers over all strips and all images of the group), so the loop is FMA-issue bound, not LDS bound.
-// The two halves meet in shared memory and each CTA issues one atomic per (tap, channel).
+// The two halves meet in shared memory and each CTA issues one atomic per (tap, channel).  C need only be a multiple of
+// 8 (ConvNeXt atto / femto / nano / tiny have 40 / 48 / 80 / 96 channels in stage 0): the last chunk reads channels past
+// C as TMA zero fill and stores nothing for them.
 constexpr int kWgT = 14;
 constexpr int kWgC = 64;
 constexpr int kWgR = 7;  // strip length (pixels) = taps per filter row
@@ -304,7 +324,7 @@ dwconv7_wgrad_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
   uint64_t* bar = reinterpret_cast<uint64_t*>(sg + ((g_bytes + 127) & ~127));
 
   const int tiles_w = (W + T - 1) / T, tiles_h = (H + T - 1) / T;
-  const int n_cc = C / kWgC;
+  const int n_cc = (C + kWgC - 1) / kWgC;
   int bid = blockIdx.x;
   const int cc = bid % n_cc; bid /= n_cc;
   const int tw = bid % tiles_w; bid /= tiles_w;
@@ -393,6 +413,7 @@ dwconv7_wgrad_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
   __syncthreads();
   for (int o = threadIdx.x; o < 50 * kWgC; o += blockDim.x) {
     const int slot = o / kWgC, ch = o - slot * kWgC;  // slot = dy * 7 + dx, or 49 for the bias
+    if (cc * kWgC + ch >= C) continue;                // zero-filled channels of a ragged last chunk
     float s = 0.f;
     if (slot < 49) {
       const int sdy = slot / 7, sdx = slot - sdy * 7;
@@ -410,7 +431,7 @@ int launch_dwconv7_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dconv, int
   const double wg_elems = static_cast<double>(B) * H * W * C;
   ProfScope prof(kProfDepthwise, 2.0 * 49.0 * wg_elems, 2.0 * 2.0 * wg_elems, s);  // read x and the output gradient
 
-  VDK_REQUIRE(C % kWgC == 0, "dwconv7_wgrad: C must be a multiple of %d (got %d)", kWgC, C);
+  VDK_REQUIRE(C % 8 == 0, "dwconv7_wgrad: C must be a multiple of 8 (got %d)", C);
   const int T = std::min(kWgT, std::max(H, W));
   CUtensorMap mx, mg;
   int rc = make_tma_nhwc_16bit(&mx, x, B, H, W, C, T + 6, T + 6, kWgC);
@@ -424,7 +445,7 @@ int launch_dwconv7_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dconv, int
   VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_wgrad_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_wgrad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   // images per CTA: keep >= ~4 CTAs per SM, and amortise the final atomics over as many images as that allows
-  const int64_t per_image = static_cast<int64_t>((H + T - 1) / T) * ((W + T - 1) / T) * (C / kWgC);
+  const int64_t per_image = static_cast<int64_t>((H + T - 1) / T) * ((W + T - 1) / T) * ((C + kWgC - 1) / kWgC);
   const int ipc = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(16, (per_image * B) / (sm_count() * 4))));
   const unsigned grid = static_cast<unsigned>(((B + ipc - 1) / ipc) * per_image);
   const int threads = ((16 * planes + 31) / 32) * 32;
