@@ -7,9 +7,12 @@
 //   warpgroup 0    : TMA producer (one thread; A tile 128x64, B tile BNx64 per stage, 128-byte swizzle), registers
 //                    handed to the consumers with setmaxnreg
 //   warpgroups 1-2 : consumers, 64 rows each: wgmma m64 x BN x 16 into registers (fp32), then the epilogue.  The
-//                    accumulator leaves the registers 64 columns at a time through shared memory so that each thread
-//                    finishes 32 consecutive columns of one row (bias / GELU / layer-scale+residual / LayerNorm /
-//                    GELU' -> 16-byte global stores) while the producer already fills the stages of the next tile.
+//                    epilogue math (bias / GELU / layer-scale+residual / LayerNorm / GELU') runs on the accumulator
+//                    fragments; each 64-row x 128-byte box of results is written to a swizzled shared-memory ring
+//                    (stmatrix for 16-bit outputs) and drained by a TMA store (a TMA reduce-add for atomic split-K), so
+//                    the stores run under the next tile's MMAs.  Each warpgroup syncs only its own 128 threads.  A
+//                    residual / saved pre-activation is TMA-loaded into the same ring while the tile's MMAs run and read
+//                    back in fragment layout (ldmatrix).
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
 
@@ -20,7 +23,7 @@ namespace vdk {
 constexpr int kBM = 128;
 constexpr int kBK = 64;  // 64 x 16-bit = one 128-byte swizzle row
 constexpr int kGemmThreads = 384;  // producer warpgroup, two consumer warpgroups
-constexpr int kAccLd = 64 + 4;     // fp32 row pitch of the staged 128 x 64 accumulator chunk (conflict-free row reads)
+constexpr int kBoxBytes = 64 * 128;  // epilogue box: one warpgroup's 64 rows x 128 bytes (64 16-bit or 32 fp32 columns)
 
 struct GemmParams {
   int M, N, K;
@@ -46,9 +49,15 @@ struct GemmCfg {
   static constexpr int kStageB = BN * kBK * 2;
   static constexpr int kStageBytes = kStageA + kStageB;
   static constexpr int kStages = (BN == 256) ? 3 : 5;
-  static constexpr int kAccBytes = kBM * kAccLd * 4;
-  // stages + staged accumulator chunk + bias [BN] + LayerNorm mean / rstd [2][128] + barriers + 1 KB align slack
-  static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + BN * 4 + 2 * kBM * 4 + 2 * kStages * 8 + 1024;
+  // epilogue ring of each consumer warpgroup, in boxes; it holds a whole 16-bit residual half tile (BN / 64 boxes)
+  static constexpr int kRing = (BN == 256) ? 4 : 3;
+  static_assert(BN / 64 <= kRing, "a 16-bit residual half tile must fit in the ring");
+  static constexpr int kRingBytes = 2 * kRing * kBoxBytes;
+  static constexpr int kParFloats = 3 * BN;  // per consumer warpgroup: bias, gamma, beta of the tile's columns
+  // stages + two rings + two parameter copies + full / empty / residual barriers + 1 KB align slack.  Within 227 KB:
+  //   BN = 256: 3 x 48 KB + 2 x 4 x 8 KB + 6 KB + 64 B + 1 KB = 215.1 KB (a fourth 48 KB stage does not fit)
+  //   BN = 128: 5 x 32 KB + 2 x 3 x 8 KB + 3 KB + 96 B + 1 KB = 212.1 KB (a fourth ring box per warpgroup does not fit)
+  static constexpr int kSmemBytes = kStages * kStageBytes + kRingBytes + 2 * kParFloats * 4 + (2 * kStages + 2) * 8 + 1024;
   static_assert(kSmemBytes <= 227 * 1024, "GEMM shared memory budget");
 };
 
@@ -122,113 +131,91 @@ __device__ __forceinline__ float2 unpack2(uint32_t u, int dtype) {
   }
 }
 
-// Per-chunk epilogue arithmetic on this thread's 32 consecutive columns [col0, col0 + ncols) of row `row`.
-// `bsm`: this tile's bias values for columns [col0, col0 + 32) in shared memory (zero beyond N): staged once per tile so
-// that the epilogue's critical path holds no global loads.
-__device__ __forceinline__ void add_bias32(float (&v)[32], const float* bsm) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 b = *reinterpret_cast<const float4*>(bsm + j);
-    v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
+// Epilogue arithmetic of one fragment pair: columns c, c + 1 of the tile (c even) in one row.  `par`: this warpgroup's
+// copy of the tile's bias / gamma / beta ([3][BN], zero beyond N), staged once per tile so that the epilogue's critical
+// path holds no global loads.  `r`: the residual / saved pre-activation pair.  The operations and their order are those
+// of the row-wise form: + bias, then the epilogue (fp32 throughout, GELU and GELU' in fp16x2 pairs).
+template <int BN>
+__device__ __forceinline__ void epi_pair(const GemmParams& p, float& x0, float& x1, const float* par, int c, float ln_mean,
+                                         float ln_rstd, float2 r) {
+  if (p.bias != nullptr && p.epilogue != VDK_EPI_LAYERNORM) {  // LayerNorm: added to the accumulator before the statistics
+    const float2 b = *reinterpret_cast<const float2*>(par + c);
+    x0 += b.x;
+    x1 += b.y;
   }
-}
-__device__ __forceinline__ void epi_math(const GemmParams& p, float (&v)[32], int row, int col0, int ncols, float ln_mean,
-                                         float ln_rstd, const float* bsm) {
-  if (p.bias != nullptr) add_bias32(v, bsm);
   if (p.epilogue == VDK_EPI_MUL_GELU_GRAD) {
-    if (row < p.M) {
-      const uint16_t* pre = reinterpret_cast<const uint16_t*>(p.residual) + static_cast<size_t>(row) * p.ldr + col0;
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        if (j < ncols) {
-          const uint4 t = *reinterpret_cast<const uint4*>(pre + j);
-          const float2 a0 = unpack2(t.x, p.out_dtype), a1 = unpack2(t.y, p.out_dtype);
-          const float2 a2 = unpack2(t.z, p.out_dtype), a3 = unpack2(t.w, p.out_dtype);
-          const float2 g0 = gelu_grad_pair(a0.x, a0.y), g1 = gelu_grad_pair(a1.x, a1.y);
-          const float2 g2 = gelu_grad_pair(a2.x, a2.y), g3 = gelu_grad_pair(a3.x, a3.y);
-          v[j] *= g0.x; v[j + 1] *= g0.y; v[j + 2] *= g1.x; v[j + 3] *= g1.y;
-          v[j + 4] *= g2.x; v[j + 5] *= g2.y; v[j + 6] *= g3.x; v[j + 7] *= g3.y;
-        }
-      }
-    }
+    const float2 g = gelu_grad_pair(r.x, r.y);
+    x0 *= g.x;
+    x1 *= g.y;
   } else if (p.epilogue == VDK_EPI_GELU) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 2) gelu_pair(v[j], v[j + 1]);
+    gelu_pair(x0, x1);
   } else if (p.epilogue == VDK_EPI_LAYERNORM) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      if (j < ncols) {
-        const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + col0 + j));
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.beta + col0 + j));
-        v[j] = (v[j] - ln_mean) * ln_rstd * g.x + b.x;
-        v[j + 1] = (v[j + 1] - ln_mean) * ln_rstd * g.y + b.y;
-        v[j + 2] = (v[j + 2] - ln_mean) * ln_rstd * g.z + b.z;
-        v[j + 3] = (v[j + 3] - ln_mean) * ln_rstd * g.w + b.w;
-      }
-    }
+    const float2 g = *reinterpret_cast<const float2*>(par + BN + c);
+    const float2 b = *reinterpret_cast<const float2*>(par + 2 * BN + c);
+    x0 = (x0 - ln_mean) * ln_rstd * g.x + b.x;
+    x1 = (x1 - ln_mean) * ln_rstd * g.y + b.y;
   } else if (p.epilogue == VDK_EPI_SCALE_RESIDUAL) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      if (j < ncols) {
-        const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + col0 + j));
-        v[j] *= g.x; v[j + 1] *= g.y; v[j + 2] *= g.z; v[j + 3] *= g.w;
-      }
-    }
-    if (row < p.M) {
-      if (p.out_dtype == VDK_DTYPE_FP32) {
-        const float* res = reinterpret_cast<const float*>(p.residual) + static_cast<size_t>(row) * p.ldr + col0;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          if (j < ncols) {
-            const float4 t = *reinterpret_cast<const float4*>(res + j);
-            v[j] += t.x; v[j + 1] += t.y; v[j + 2] += t.z; v[j + 3] += t.w;
-          }
-        }
-      } else {
-        const uint16_t* res = reinterpret_cast<const uint16_t*>(p.residual) + static_cast<size_t>(row) * p.ldr + col0;
-#pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          if (j < ncols) {
-            const uint4 t = *reinterpret_cast<const uint4*>(res + j);
-            const float2 a0 = unpack2(t.x, p.out_dtype), a1 = unpack2(t.y, p.out_dtype);
-            const float2 a2 = unpack2(t.z, p.out_dtype), a3 = unpack2(t.w, p.out_dtype);
-            v[j] += a0.x; v[j + 1] += a0.y; v[j + 2] += a1.x; v[j + 3] += a1.y;
-            v[j + 4] += a2.x; v[j + 5] += a2.y; v[j + 6] += a3.x; v[j + 7] += a3.y;
-          }
-        }
-      }
-    }
+    // gamma x is rounded before the residual is added: __fmul_rn keeps the compiler from contracting the two into an FMA
+    const float2 g = *reinterpret_cast<const float2*>(par + BN + c);
+    x0 = __fmul_rn(x0, g.x);
+    x1 = __fmul_rn(x1, g.y);
+    x0 += r.x;
+    x1 += r.y;
   }
 }
+
+// A warpgroup's box in ring slot `slot` is written: make it visible to the async proxy, let the leader hand it to TMA
+// (store, or reduce-add into fp32) and move to the next slot.  Before the barrier the leader waits until the store that
+// last read the NEXT slot is done reading, so after the barrier every thread may write that slot.
+template <int kRing>
+__device__ __forceinline__ void epi_publish(const CUtensorMap* map, const uint8_t* box, int& slot, bool leader, uint32_t bar_id,
+                                            int c0, int c1, int c2, bool reduce) {
+  fence_proxy_async_smem();
+  if (leader) tma_store_wait_read<kRing - 2>();
+  named_bar_sync(bar_id, 128);
+  if (leader) {
+    if (reduce) tma_reduce_add_3d(map, box, c0, c1, c2);
+    else tma_store_3d(map, box, c0, c1, c2);
+    tma_store_commit();
+  }
+  slot = (slot + 1 == kRing) ? 0 : slot + 1;
+}
+
+// byte offset of the 16-byte chunk `chunk` of row `row` in a 128-byte-swizzled box (the TMA SWIZZLE_128B pattern)
+__device__ __forceinline__ uint32_t box_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
+
 // kTA / kTB: operand stored with the contraction index as the slow dimension ([K,M] / [K,N] row-major: MN-major)
 template <int BN, bool kBf16, int kTA, int kTB>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const GemmParams p) {
+gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+               const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_aux,
+               const __grid_constant__ CUtensorMap map_r, const GemmParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kRing = Cfg::kRing;
   extern __shared__ uint8_t smem_raw[];
   // align inside the dynamic smem window without a pointer->integer->pointer round trip (which would demote every
   // later access to generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* acc_sm = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);  // [128][kAccLd]
-  float* bias_sm = acc_sm + kBM * kAccLd;                                      // [BN] bias of the tile being finished
-  float* ln_sm = bias_sm + BN;                                                 // [2][128] LayerNorm mean, rstd per row
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ln_sm + 2 * kBM);
+  uint8_t* ring_all = smem + kStages * Cfg::kStageBytes;                   // [2][kRing] boxes, 1024-byte aligned
+  float* par_all = reinterpret_cast<float*>(ring_all + Cfg::kRingBytes);  // [2][3][BN] bias, gamma, beta
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(par_all + 2 * Cfg::kParFloats);
   uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* res_bar = empty_bar + kStages;  // [2]: a consumer warpgroup's residual boxes have landed
 
-  const int num_m = (p.M + kBM - 1) / kBM;
-  const int num_n = (p.N + BN - 1) / BN;
-  const int num_kb_total = (p.K + kBK - 1) / kBK;
-  const int kb_per_split = (num_kb_total + p.split_k - 1) / p.split_k;
-  const int num_tiles = num_m * num_n * p.split_k;  // work items; split index is the slowest dimension
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&map_a);
     prefetch_tensormap(&map_b);
+    prefetch_tensormap(&map_d);
+    if (p.aux != nullptr) prefetch_tensormap(&map_aux);
+    if (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD) prefetch_tensormap(&map_r);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
+    mbar_init(&res_bar[0], 1);
+    mbar_init(&res_bar[1], 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -236,6 +223,12 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (threadIdx.x < 128) {
     // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    // the tile grid, computed in each role after its register hand-over (kept live across the hand-over, it spills)
+    const int num_m = (p.M + kBM - 1) / kBM;
+    const int num_n = (p.N + BN - 1) / BN;
+    const int num_kb_total = (p.K + kBK - 1) / kBK;
+    const int kb_per_split = (num_kb_total + p.split_k - 1) / p.split_k;
+    const int num_tiles = num_m * num_n * p.split_k;  // work items; split index is the slowest dimension
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -272,12 +265,30 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   } else {
     // ===================== consumers: mainloop + epilogue =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int num_m = (p.M + kBM - 1) / kBM;
+    const int num_n = (p.N + BN - 1) / BN;
+    const int num_kb_total = (p.K + kBK - 1) / kBK;
+    const int kb_per_split = (num_kb_total + p.split_k - 1) / p.split_k;
+    const int num_tiles = num_m * num_n * p.split_k;  // work items; split index is the slowest dimension
     const int ct = threadIdx.x - 128;  // 0..255
     const int cg = ct >> 7;            // consumer warpgroup: accumulator rows cg*64 .. cg*64+63 of the tile
     const int wl = (ct >> 5) & 3, lane = ct & 31;
-    const int frow = cg * 64 + wl * 16 + (lane >> 2);  // first of this thread's two fragment rows (the other is + 8)
     const int fcol = (lane & 3) * 2;
-    const int erow = ct & 127, half = ct >> 7;         // epilogue: row and 32-column half of a staged chunk
+    // epilogue: this thread's first fragment row in the warpgroup's box (the other is + 8), and the row / chunk parity
+    // whose address this lane gives to stmatrix / ldmatrix
+    const int frow = wl * 16 + (lane >> 2);
+    const int mrow = wl * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+    const int mcb = lane >> 4;
+    const bool leader = (ct & 127) == 0;  // issues, and waits for, every TMA transfer of this warpgroup's epilogue
+    const uint32_t bar_id = 2 + cg;       // named barrier of this warpgroup's 128 threads
+    uint8_t* ring = ring_all + cg * kRing * kBoxBytes;
+    float* par = par_all + cg * Cfg::kParFloats;
+    const bool f32 = p.out_dtype == VDK_DTYPE_FP32;
+    const int box_cols = f32 ? 32 : 64;
+    const bool has_res = p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD;
+    const bool reduce = p.partial_out && p.split_stride == 0;  // atomic split-K: TMA reduce-add into D
+    int slot = 0;  // ring slot of the next box
+    uint32_t res_phase = 0;
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
@@ -287,6 +298,21 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       const int n0 = (mn % num_n) * BN;
       const int kb0 = split * kb_per_split;
       const int kb1 = min(kb0 + kb_per_split, num_kb_total);
+      const int wrow0 = m0 + cg * 64;
+      const bool live = wrow0 < p.M;  // warpgroup-uniform: the half tile below a ragged M has nothing to write
+      const int nbox = (min(BN, p.N - n0) + box_cols - 1) / box_cols;
+      const int npre = has_res ? min(nbox, kRing) : 0;  // residual boxes loaded while the MMAs run
+      // the tile's per-column parameters (bias, gamma, beta) go to this warpgroup's copy in shared memory by cp.async, which
+      // holds no registers while the MMAs run; the previous tile's epilogue has read that copy (its last barrier is behind
+      // every thread of the warpgroup)
+      if (live && (ct & 127) < BN / 4) {
+        const int c = (ct & 127) * 4;  // this thread's 4 columns of each array
+        const bool in = n0 + c < p.N;  // N % 8 == 0: the 4 columns are all in or all out
+        if (p.bias != nullptr) cp_async_16_zfill(par + c, p.bias + (in ? n0 + c : 0), in);
+        if (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_LAYERNORM)
+          cp_async_16_zfill(par + BN + c, p.gamma + (in ? n0 + c : 0), in);
+        if (p.epilogue == VDK_EPI_LAYERNORM) cp_async_16_zfill(par + 2 * BN + c, p.beta + (in ? n0 + c : 0), in);
+      }
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait<true>(&full_bar[stage], phase);
@@ -303,6 +329,14 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
           else wgmma_m64n128k16_ss<kBf16, kTA, kTB>(acc, da + step_a * k, db + step_b * k, (kb > kb0 || k > 0) ? 1u : 0u);
         }
         wgmma_commit();
+        if (kb == kb0 && leader && live && npre > 0) {
+          // under the tile's first MMAs: once the previous tile's stores have read the ring, TMA-load the residual boxes
+          // into the slots this tile's boxes will use
+          tma_store_wait_read<0>();
+          mbar_arrive_expect_tx(&res_bar[cg], npre * kBoxBytes);
+          for (int i = 0; i < npre; ++i)
+            tma_load_3d(ring + ((slot + i) % kRing) * kBoxBytes, &map_r, &res_bar[cg], n0 + i * box_cols, wrow0, 0);
+        }
         // the previous stage's MMAs have retired once at most this one is pending: its slot may be refilled
         wgmma_wait<1>();
         if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
@@ -315,138 +349,160 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (!live) continue;
 
+      cp_async_wait_all();
+      named_bar_sync(bar_id, 128);  // the warpgroup's staged parameters are visible
+      float ln_mean[2] = {0.f, 0.f}, ln_rstd[2] = {1.f, 1.f};
       if (p.epilogue == VDK_EPI_LAYERNORM) {
-        // the tile spans the whole row (N <= BN): the four threads of a fragment quad hold every column of its two rows
+        // the tile spans the whole row (N <= BN): the four threads of a fragment quad hold every column of its two rows,
+        // and the butterfly leaves the same sums in all four.  The bias is added in place first (epi_pair skips it here),
+        // so that the statistics and the normalisation see the same acc + bias without holding the bias in registers.
+        if (p.bias != nullptr) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const float2 b = *reinterpret_cast<const float2*>(par + j * 8 + fcol);
+            acc[4 * j] += b.x;
+            acc[4 * j + 1] += b.y;
+            acc[4 * j + 2] += b.x;
+            acc[4 * j + 3] += b.y;
+          }
+        }
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           float sum = 0.f;
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int col = n0 + j * 8 + fcol + e;
-              if (col < p.N) sum += acc[4 * j + 2 * r + e] + (p.bias ? __ldg(p.bias + col) : 0.f);
-            }
+          for (int j = 0; j < BN / 8; ++j) {
+            if (j * 8 >= p.N) break;  // N % 8 == 0: the columns below N are a prefix of whole 8-column blocks
+            sum += acc[4 * j + 2 * r];
+            sum += acc[4 * j + 2 * r + 1];
+          }
           sum += __shfl_xor_sync(0xffffffffu, sum, 1);
           sum += __shfl_xor_sync(0xffffffffu, sum, 2);
           const float mean = sum / static_cast<float>(p.N);
           float sq = 0.f;
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int col = n0 + j * 8 + fcol + e;
-              if (col < p.N) {
-                const float d = acc[4 * j + 2 * r + e] + (p.bias ? __ldg(p.bias + col) : 0.f) - mean;
-                sq = fmaf(d, d, sq);
-              }
-            }
+          for (int j = 0; j < BN / 8; ++j) {
+            if (j * 8 >= p.N) break;
+            const float d0 = acc[4 * j + 2 * r] - mean;
+            sq = fmaf(d0, d0, sq);
+            const float d1 = acc[4 * j + 2 * r + 1] - mean;
+            sq = fmaf(d1, d1, sq);
+          }
           sq += __shfl_xor_sync(0xffffffffu, sq, 1);
           sq += __shfl_xor_sync(0xffffffffu, sq, 2);
-          if ((lane & 3) == 0) {
-            ln_sm[frow + 8 * r] = mean;
-            ln_sm[kBM + frow + 8 * r] = rsqrtf(sq / static_cast<float>(p.N) + p.ln_eps);
-          }
+          ln_mean[r] = mean;
+          ln_rstd[r] = rsqrtf(sq / static_cast<float>(p.N) + p.ln_eps);
         }
       }
-      if (p.bias != nullptr && ct < BN) bias_sm[ct] = (n0 + ct < p.N) ? __ldg(p.bias + n0 + ct) : 0.f;
-      const int row = m0 + erow;
+      if (npre > 0) {
+        mbar_wait<true>(&res_bar[cg], res_phase);
+        res_phase ^= 1;
+      }
+      const int dz = (p.partial_out && p.split_stride > 0) ? split : 0;  // slab of a deterministic split-K partial
+      int box_i = 0;                                                     // boxes of this tile so far
 #pragma unroll
       for (int sc = 0; sc < BN / 64; ++sc) {
-        if (n0 + sc * 64 < p.N) {  // block-uniform
+        if (n0 + sc * 64 >= p.N) continue;  // block-uniform
+        if (f32) {
+          // two boxes of 32 columns; a thread writes its float2 pairs (two wavefronts per warp store, the minimum)
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int j = sc * 8 + jj;
-            *reinterpret_cast<float2*>(acc_sm + frow * kAccLd + jj * 8 + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-            *reinterpret_cast<float2*>(acc_sm + (frow + 8) * kAccLd + jj * 8 + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-          }
-          named_bar_sync(1, 256);  // the chunk (and, before the first one, the bias and LayerNorm statistics) is in smem
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 t = *reinterpret_cast<const float4*>(acc_sm + erow * kAccLd + half * 32 + j);
-            v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
-          }
-          named_bar_sync(1, 256);  // every thread holds its piece: the buffer may take the next chunk
-          const float ln_mean = p.epilogue == VDK_EPI_LAYERNORM ? ln_sm[erow] : 0.f;
-          const float ln_rstd = p.epilogue == VDK_EPI_LAYERNORM ? ln_sm[kBM + erow] : 1.f;
-          const int col0 = n0 + sc * 64 + half * 32;
-          const int ncols = min(32, p.N - col0);  // multiple of 8 (N % 8 == 0 is required)
-          if (row < p.M && ncols > 0) {
-            if (p.partial_out) {
-              // split-K: raw fp32 partial sums.  With a slab stride every split owns its own copy of D (plain stores,
-              // the consumer adds the slabs in a fixed order: deterministic); otherwise they are atomically added
-              // into a D the caller zeroed.
-              if (p.split_stride > 0) {
-                float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(split) * p.split_stride +
-                             static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                  if (j < ncols) *reinterpret_cast<float4*>(out + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-              } else {
-                float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (j < ncols) atomicAdd(out + j, v[j]);
+          for (int hb = 0; hb < 2; ++hb) {
+            const int bcol = n0 + sc * 64 + hb * 32;
+            if (bcol >= p.N) continue;
+            uint8_t* box = ring + slot * kBoxBytes;
+            if (has_res && box_i >= npre) {  // an fp32 residual wider than the ring: load this box now
+              if (leader) {
+                mbar_arrive_expect_tx(&res_bar[cg], kBoxBytes);
+                tma_load_3d(box, &map_r, &res_bar[cg], bcol, wrow0, 0);
               }
-            } else {
-              if (p.aux != nullptr) {
-                // GELU with a saved pre-activation: store acc + bias, then apply the activation to the ROUNDED
-                // pre-activation (what the backward will see, and what autocast's 16-bit Linear output hands to nn.GELU)
-                if (p.bias != nullptr) add_bias32(v, bias_sm + (col0 - n0));
-                uint16_t* aux = reinterpret_cast<uint16_t*>(p.aux) + static_cast<size_t>(row) * p.ldd + col0;
+              mbar_wait<true>(&res_bar[cg], res_phase);
+              res_phase ^= 1;
+            }
 #pragma unroll
-                for (int j = 0; j < 32; j += 8) {
-                  if (j < ncols) {
-                    uint4 t;
-                    t.x = pack2(v[j], v[j + 1], p.out_dtype);
-                    t.y = pack2(v[j + 2], v[j + 3], p.out_dtype);
-                    t.z = pack2(v[j + 4], v[j + 5], p.out_dtype);
-                    t.w = pack2(v[j + 6], v[j + 7], p.out_dtype);
-                    *reinterpret_cast<uint4*>(aux + j) = t;
-                  }
-                }
+            for (int q = 0; q < 4; ++q) {
+              const int j = sc * 8 + hb * 4 + q;
 #pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                  float2 a = unpack2(pack2(v[j], v[j + 1], p.out_dtype), p.out_dtype);
-                  gelu_pair(a.x, a.y);
-                  v[j] = a.x;
-                  v[j + 1] = a.y;
-                }
-              } else {
-                epi_math(p, v, row, col0, ncols, ln_mean, ln_rstd, bias_sm + (col0 - n0));
-              }
-              if (p.out_dtype == VDK_DTYPE_FP32) {
-                float* out = reinterpret_cast<float*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                  if (j < ncols) *reinterpret_cast<float4*>(out + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-              } else {
-                uint16_t* out = reinterpret_cast<uint16_t*>(p.D) + static_cast<size_t>(row) * p.ldd + col0;
-#pragma unroll
-                for (int j = 0; j < 32; j += 8) {
-                  if (j < ncols) {
-                    uint4 t;
-                    t.x = pack2(v[j], v[j + 1], p.out_dtype);
-                    t.y = pack2(v[j + 2], v[j + 3], p.out_dtype);
-                    t.z = pack2(v[j + 4], v[j + 5], p.out_dtype);
-                    t.w = pack2(v[j + 6], v[j + 7], p.out_dtype);
-                    *reinterpret_cast<uint4*>(out + j) = t;
-                  }
-                }
+              for (int h = 0; h < 2; ++h) {
+                const int r = frow + 8 * h;
+                float2* dst = reinterpret_cast<float2*>(box + box_off(r, 2 * q + (fcol >> 2)) + (fcol & 2) * 4);
+                float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+                if (!p.partial_out) epi_pair<BN>(p, x0, x1, par, j * 8 + fcol, ln_mean[h], ln_rstd[h], has_res ? *dst : make_float2(0.f, 0.f));
+                *dst = make_float2(x0, x1);
               }
             }
+            epi_publish<kRing>(&map_d, box, slot, leader, bar_id, bcol, wrow0, dz, reduce);
+            ++box_i;
           }
+        } else {
+          const int bcol = n0 + sc * 64;
+          uint8_t* box = ring + slot * kBoxBytes;
+          if (p.aux != nullptr) {
+            // GELU with a saved pre-activation: store acc + bias, then apply the activation to the ROUNDED
+            // pre-activation (what the backward will see, and what autocast's 16-bit Linear output hands to nn.GELU)
+            // (the rounded pre-activation stays in the accumulator registers between the two boxes)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              uint32_t rq[4];
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const int j = sc * 8 + 2 * q + (i >> 1), h = i & 1;
+                float& x0 = acc[4 * j + 2 * h];
+                float& x1 = acc[4 * j + 2 * h + 1];
+                if (p.bias != nullptr) {
+                  const float2 b = *reinterpret_cast<const float2*>(par + j * 8 + fcol);
+                  x0 += b.x;
+                  x1 += b.y;
+                }
+                rq[i] = pack2(x0, x1, p.out_dtype);
+                const float2 a = unpack2(rq[i], p.out_dtype);
+                x0 = a.x;
+                x1 = a.y;
+              }
+              stmatrix_x4(smem_u32(box) + box_off(mrow, 2 * q + mcb), rq);
+            }
+            epi_publish<kRing>(&map_aux, box, slot, leader, bar_id, bcol, wrow0, 0, false);
+            box = ring + slot * kBoxBytes;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              uint32_t rq[4];
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const int j = sc * 8 + 2 * q + (i >> 1), h = i & 1;
+                float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+                gelu_pair(x0, x1);
+                rq[i] = pack2(x0, x1, p.out_dtype);
+              }
+              stmatrix_x4(smem_u32(box) + box_off(mrow, 2 * q + mcb), rq);
+            }
+          } else {
+            // the residual box (if any) was loaded into this slot; each warp reads and overwrites only its own rows
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const uint32_t addr = smem_u32(box) + box_off(mrow, 2 * q + mcb);
+              uint32_t rin[4] = {0u, 0u, 0u, 0u}, rq[4];
+              if (has_res) ldmatrix_x4(rin, addr);
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const int j = sc * 8 + 2 * q + (i >> 1), h = i & 1;
+                float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+                epi_pair<BN>(p, x0, x1, par, j * 8 + fcol, ln_mean[h], ln_rstd[h], unpack2(rin[i], p.out_dtype));
+                rq[i] = pack2(x0, x1, p.out_dtype);
+              }
+              stmatrix_x4(addr, rq);
+            }
+          }
+          epi_publish<kRing>(&map_d, box, slot, leader, bar_id, bcol, wrow0, 0, false);
+          ++box_i;
         }
       }
-      named_bar_sync(1, 256);  // bias and LayerNorm statistics of this tile are consumed
     }
+    if (leader) tma_store_wait<0>();  // the ring stays valid until the last stores have read it
   }
 }
 
 template <int BN, bool kBf16, int kTA, int kTB>
-static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap* maps, const GemmParams& p, cudaStream_t stream) {
   constexpr int kSmem = GemmCfg<BN>::kSmemBytes;
   auto kern = gemm_tn_kernel<BN, kBf16, kTA, kTB>;
   static bool attr_set = false;  // per instantiation
@@ -456,16 +512,15 @@ static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const GemmP
   }
   const int num_tiles = ((p.M + kBM - 1) / kBM) * ((p.N + BN - 1) / BN) * p.split_k;
   const int grid = num_tiles < sm_count() ? num_tiles : sm_count();
-  kern<<<grid, kGemmThreads, kSmem, stream>>>(ma, mb, p);
+  kern<<<grid, kGemmThreads, kSmem, stream>>>(maps[0], maps[1], maps[2], maps[3], maps[4], p);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }
 
 template <int BN, bool kBf16>
-static int launch_gemm_major(const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p, bool ta, bool tb,
-                             cudaStream_t s) {
-  if (ta) return tb ? launch_gemm<BN, kBf16, 1, 1>(ma, mb, p, s) : launch_gemm<BN, kBf16, 1, 0>(ma, mb, p, s);
-  return tb ? launch_gemm<BN, kBf16, 0, 1>(ma, mb, p, s) : launch_gemm<BN, kBf16, 0, 0>(ma, mb, p, s);
+static int launch_gemm_major(const CUtensorMap* maps, const GemmParams& p, bool ta, bool tb, cudaStream_t s) {
+  if (ta) return tb ? launch_gemm<BN, kBf16, 1, 1>(maps, p, s) : launch_gemm<BN, kBf16, 1, 0>(maps, p, s);
+  return tb ? launch_gemm<BN, kBf16, 0, 1>(maps, p, s) : launch_gemm<BN, kBf16, 0, 0>(maps, p, s);
 }
 
 }  // namespace vdk
@@ -524,7 +579,8 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   bool wide = (g.N % 256 == 0) || g.N > 512;
   if (g.epilogue == VDK_EPI_LAYERNORM) wide = g.N > 128;
   const int BN = wide ? 256 : 128;
-  CUtensorMap ma, mb;
+  CUtensorMap maps[5];  // A, B, D, aux_out, residual
+  CUtensorMap &ma = maps[0], &mb = maps[1], &md = maps[2], &maux = maps[3], &mr = maps[4];
   // K-major operand: rows = M (or N), box = tile rows x 64 contraction elements; MN-major: rows = contraction index,
   // box = 64 contraction rows x 64 M (or N) elements
   int rc = g.trans_a ? make_tma_2d_16bit(&ma, g.A, (uint64_t)g.K, (uint64_t)g.M, (uint64_t)g.lda, kBK, 64)
@@ -538,6 +594,23 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
                 "vdk_gemm: aux_out needs the GELU epilogue and a 16-bit output");
     VDK_REQUIRE((reinterpret_cast<uintptr_t>(g.aux_out) & 15) == 0, "vdk_gemm: aux_out must be 16-byte aligned");
   }
+  // the epilogue's TMA views: D (a 3-D [split][M][ldd] view for split-K slabs), aux_out and the residual, which has D's
+  // element type; the maps clip ragged M and N.  Unused views repeat D's map.
+  const int osize = g.out_dtype == VDK_DTYPE_FP32 ? 4 : 2;
+  const bool slabs = g.split_k > 1 && g.split_stride != 0;
+  rc = make_tma_epilogue_map(&md, g.D, osize, (uint64_t)g.M, (uint64_t)g.N, (uint64_t)g.ldd, slabs ? (uint64_t)split : 1,
+                             slabs ? (uint64_t)g.split_stride : 0);
+  if (rc != VDK_OK) return rc;
+  maux = md;
+  mr = md;
+  if (g.aux_out != nullptr) {
+    rc = make_tma_epilogue_map(&maux, g.aux_out, 2, (uint64_t)g.M, (uint64_t)g.N, (uint64_t)g.ldd, 1, 0);
+    if (rc != VDK_OK) return rc;
+  }
+  if (g.epilogue == VDK_EPI_SCALE_RESIDUAL || g.epilogue == VDK_EPI_MUL_GELU_GRAD) {
+    rc = make_tma_epilogue_map(&mr, g.residual, osize, (uint64_t)g.M, (uint64_t)g.N, (uint64_t)g.ldr, 1, 0);
+    if (rc != VDK_OK) return rc;
+  }
   GemmParams p{g.M, g.N, g.K, g.D, g.ldd, g.bias, g.gamma, g.beta, g.residual, g.ldr, g.out_dtype, g.epilogue,
                g.ln_eps, split, g.split_k > 1 ? (long long)g.split_stride : 0ll, g.aux_out, (g.split_k > 1) ? 1 : 0};
   const bool bf = g.in_dtype == VDK_DTYPE_BF16;
@@ -548,8 +621,8 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
                      (g.aux_out ? 2.0 * g.M * g.N : 0.0) + (g.residual ? osz * g.M * g.N : 0.0),
                  s);
   const bool ta = g.trans_a != 0, tb = g.trans_b != 0;
-  if (wide) return bf ? launch_gemm_major<256, true>(ma, mb, p, ta, tb, s) : launch_gemm_major<256, false>(ma, mb, p, ta, tb, s);
-  return bf ? launch_gemm_major<128, true>(ma, mb, p, ta, tb, s) : launch_gemm_major<128, false>(ma, mb, p, ta, tb, s);
+  if (wide) return bf ? launch_gemm_major<256, true>(maps, p, ta, tb, s) : launch_gemm_major<256, false>(maps, p, ta, tb, s);
+  return bf ? launch_gemm_major<128, true>(maps, p, ta, tb, s) : launch_gemm_major<128, false>(maps, p, ta, tb, s);
 }
 
 }  // namespace vdk

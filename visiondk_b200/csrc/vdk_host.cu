@@ -99,6 +99,28 @@ int make_tma_3d_16bit(CUtensorMap* map, const void* base, uint64_t d0, uint64_t 
   return VDK_OK;
 }
 
+int make_tma_epilogue_map(CUtensorMap* map, const void* base, int elem_bytes, uint64_t rows, uint64_t cols, uint64_t ld,
+                          uint64_t depth, uint64_t depth_stride) {
+  EncodeTiledFn fn = encode_tiled_fn();
+  if (!fn) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  const uint64_t eb = static_cast<uint64_t>(elem_bytes);
+  // one matrix: the pitch of a single-matrix map only has to be a legal stride, so take the matrix's own size
+  if (depth <= 1) depth_stride = (rows * ld * eb + 15) / 16 * 16 / eb;
+  if ((elem_bytes != 2 && elem_bytes != 4) || (reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * eb) % 16 != 0 ||
+      (depth_stride * eb) % 16 != 0)
+    return fail(VDK_ERR_INVALID, "epilogue TMA operand must be 16-byte aligned with 16-byte-multiple pitches (ld=%llu)",
+                (unsigned long long)ld);
+  cuuint64_t gdim[3] = {cols, rows, depth < 1 ? 1 : depth};
+  cuuint64_t gstride[2] = {ld * eb, depth_stride * eb};
+  cuuint32_t box[3] = {static_cast<cuuint32_t>(128 / elem_bytes), 64, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(map, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(base),
+                  gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeTiled (epilogue) failed with CUresult %d", (int)r);
+  return VDK_OK;
+}
+
 // ---- live profile (see vdk_host.h) ----
 struct ProfRecord {
   int category;

@@ -43,6 +43,13 @@ int make_tma_nhwc_16bit(CUtensorMap* map, const void* base, int B, int H, int W,
 int make_tma_3d_16bit(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t pitch1, uint64_t pitch2,
                       uint32_t box_rows);
 
+// 3-D map over `depth` row-major [rows][cols] matrices of 16-bit (elem_bytes 2) or fp32 (elem_bytes 4) elements: row pitch
+// `ld` elements, matrix pitch `depth_stride` elements (ignored when depth == 1).  Box = 64 rows x 128 bytes, 128-byte
+// swizzle; an fp32 map has the FLOAT32 element type so that a TMA reduce-add adds floats.  The GEMM epilogue's view of
+// its output, its saved pre-activation and its residual input.
+int make_tma_epilogue_map(CUtensorMap* map, const void* base, int elem_bytes, uint64_t rows, uint64_t cols, uint64_t ld,
+                          uint64_t depth, uint64_t depth_stride);
+
 int sm_count();
 
 // Live kernel timing inside a real step (bench.py's roofline): while a profile is open (vdk_prof_begin), every launch wrapped
