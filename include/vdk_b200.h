@@ -245,18 +245,21 @@ int vdk_convnext_forward(const vdk_convnext_net* net, const float* images, int b
 #define VDK_VIT_MAX_BLOCKS 48
 typedef struct vdk_vit_block {
   const float* ln1_w; const float* ln1_b;
-  const void* qkv_w;  const float* qkv_b;   /* [3*dim, dim], [3*dim]: rows ordered (q | k | v) x head x 64 as in timm */
+  const void* qkv_w;  const float* qkv_b;   /* [3*dim, dim], [3*dim]: rows ordered (q | k | v) x head x head_dim as in timm */
   const void* proj_w; const float* proj_b;  /* [dim, dim] */
   const float* ln2_w; const float* ln2_b;
-  const void* fc1_w;  const float* fc1_b;   /* [4*dim, dim] */
-  const void* fc2_w;  const float* fc2_b;   /* [dim, 4*dim] */
+  const void* fc1_w;  const float* fc1_b;   /* [mlp_dim, dim] */
+  const void* fc2_w;  const float* fc2_b;   /* [dim, mlp_dim] */
+  /* timm's LayerScale (DINOv2: blocks.{i}.ls1.gamma, ls2.gamma), [dim] each: x + ls1 * attn(...), x + ls2 * mlp(...).
+   * NULL = no LayerScale.  Inference only. */
+  const float* ls1; const float* ls2;
 } vdk_vit_block;
 typedef struct vdk_vit_net {
-  int image_size, patch, dim, depth, heads, feat_dim;
+  int image_size, patch, dim, depth, heads, feat_dim;  /* head_dim = dim / heads: 64, 72 or 80 (training: 64) */
   const void* patch_w;      /* [dim, Kp] bf16, Kp = 3*patch*patch rounded up to 8, (c, kh, kw) order, zero padded */
   const float* patch_b;     /* [dim] */
-  const float* cls_token;   /* [dim] */
-  const float* pos_embed;   /* [1 + (image_size/patch)^2, dim] */
+  const float* cls_token;   /* [dim]; NULL = no class token (SigLIP, inference only): tokens = (image_size/patch)^2 */
+  const float* pos_embed;   /* [tokens, dim]: [1 + (image_size/patch)^2, dim] with a class token */
   const float* ones;        /* [dim] of 1.0f (layer-scale slot of the residual epilogue: timm's default ViT has none) */
   vdk_vit_block blocks[VDK_VIT_MAX_BLOCKS];
   const float* norm_w; const float* norm_b;        /* model.norm, eps 1e-6 */
@@ -268,13 +271,15 @@ typedef struct vdk_vit_net {
    * Inference only: vdk_vit_train_* refuse a net with norm_pre_w set. */
   const float* norm_pre_w; const float* norm_pre_b;
   float ln_eps;             /* eps of norm_pre, the block norms and model.norm; 0 selects 1e-6 */
+  int mlp_dim;              /* MLP hidden width (multiple of 8); 0 = 4 * dim.  Another width is inference only (SigLIP: 4304) */
 } vdk_vit_net;
 size_t vdk_vit_workspace_bytes(const vdk_vit_net* net, int batch);
 /* images: fp32 NCHW [batch,3,S,S]; embeddings: fp32 [batch, feat_dim], L2-normalised when l2_normalize != 0. */
 int vdk_vit_forward(const vdk_vit_net* net, const float* images, int batch, int l2_normalize, float* embeddings,
                     void* workspace, size_t workspace_bytes, void* stream);
-/* softmax(Q K^T / sqrt(d)) V on the qkv Linear's output as stored: qkv bf16 [batch, tokens, 3, heads, 64] ->
- * out bf16 [batch, tokens, heads*64]  (timm Attention.forward, scores never written to memory). */
+/* softmax(Q K^T / sqrt(d)) V on the qkv Linear's output as stored: qkv bf16 [batch, tokens, 3, heads, head_dim] ->
+ * out bf16 [batch, tokens, heads*head_dim]  (timm Attention.forward, scores never written to memory).  head_dim 64, 72 or 80
+ * (other values: VDK_ERR_INVALID); with VDK_ATT_TC=0 (the earlier mma.sync kernel) 64 only. */
 int vdk_attention_fwd(const void* qkv, int batch, int tokens, int heads, int head_dim, void* out, void* stream);
 
 /* ---- ViT training forward / backward (BASELINE config 3: ViT-B/16 + CircleLoss) ----------------------------------- */
@@ -310,8 +315,8 @@ int vdk_vit_train_backward_units(const vdk_vit_net* net);
 int vdk_vit_train_backward_range(const vdk_vit_net* net, const vdk_vit_tensors* params, const vdk_vit_tensors* grads,
                                  const float* d_feats, int batch, void* workspace, size_t workspace_bytes, void* stream, int unit_begin,
                                  int unit_end);
-/* unit-test surface of the attention pair: forward that also saves the log2-domain log-sum-exp [batch, heads, tokens], and
- * the backward dqkv = d(attention)/d(qkv) for d_out (both [batch, tokens, heads*64] bf16). */
+/* unit-test surface of the attention pair: forward that also saves the log2-domain log-sum-exp [batch, heads, tokens] (head_dim
+ * 64, 72 or 80), and the backward dqkv = d(attention)/d(qkv) for d_out (both [batch, tokens, heads*64] bf16; head_dim 64 only). */
 int vdk_attention_fwd_lse(const void* qkv, int batch, int tokens, int heads, int head_dim, void* out, float* lse2, void* stream);
 int vdk_attention_bwd(const void* qkv, const void* out, const void* d_out, const float* lse2, int batch, int tokens, int heads,
                       int head_dim, void* dqkv, void* stream);

@@ -81,21 +81,20 @@ int make_tma_nhwc_16bit(CUtensorMap* map, const void* base, int B, int H, int W,
   return VDK_OK;
 }
 
-int make_tma_3d_16bit(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t pitch1, uint64_t pitch2,
-                      uint32_t box_rows) {
+int make_tma_qkv_16bit(CUtensorMap* map, const void* base, int D, int H, int N, int B, uint32_t box_cols, uint32_t box_rows) {
   EncodeTiledFn fn = encode_tiled_fn();
   if (!fn) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (pitch1 * 2) % 16 != 0 || (pitch2 * 2) % 16 != 0)
-    return fail(VDK_ERR_INVALID, "3-D TMA operand must be 16-byte aligned with 16-byte-multiple pitches");
-  if (box_rows > 256) return fail(VDK_ERR_INVALID, "TMA box must be <= 256 rows");
-  cuuint64_t gdim[3] = {d0, d1, d2};
-  cuuint64_t gstride[2] = {pitch1 * 2, pitch2 * 2};
-  cuuint32_t box[3] = {64, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(base), gdim, gstride, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeTiled (3-D) failed with CUresult %d", (int)r);
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (D * 2) % 16 != 0)
+    return fail(VDK_ERR_INVALID, "qkv TMA operand must be 16-byte aligned with head_dim * 2 a multiple of 16 (head_dim=%d)", D);
+  if ((box_cols != 64 && box_cols != 16) || box_rows > 256) return fail(VDK_ERR_INVALID, "qkv TMA box must be 64 or 16 columns, <= 256 rows");
+  cuuint64_t gdim[4] = {(cuuint64_t)D, 3ull * H, (cuuint64_t)N, (cuuint64_t)B};
+  cuuint64_t gstride[3] = {(cuuint64_t)D * 2, 3ull * H * D * 2, 3ull * H * D * 2 * N};
+  cuuint32_t box[4] = {box_cols, 1, box_rows, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), gdim, gstride, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeTiled (qkv) failed with CUresult %d", (int)r);
   return VDK_OK;
 }
 

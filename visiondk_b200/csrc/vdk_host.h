@@ -38,10 +38,10 @@ int make_tma_2d_16bit(CUtensorMap* map, const void* base, uint64_t rows, uint64_
 // (which is exactly the zero padding of a convolution).
 int make_tma_nhwc_16bit(CUtensorMap* map, const void* base, int B, int H, int W, int C, int box_h, int box_w, int box_c);
 
-// 3-D map over a 16-bit tensor [d2][d1][d0] (d0 contiguous; pitches in elements): box = [1][box_rows][64 elements], 128-byte
-// swizzle, out-of-bounds rows read as zero.  The attention kernel's view of the qkv buffer: [batch][tokens][3*heads*64].
-int make_tma_3d_16bit(CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t pitch1, uint64_t pitch2,
-                      uint32_t box_rows);
+// 4-D map over the qkv Linear's output, 16-bit [B][N][3H][D] (D contiguous), seen as (D, 3H, N, B): box = [1][box_rows][1]
+// [box_cols], box_cols 64 with 128-byte swizzle or 16 with 32-byte swizzle; out-of-bounds rows (past N) and columns (past D)
+// read as zero.  The attention kernel's view of its input.
+int make_tma_qkv_16bit(CUtensorMap* map, const void* base, int D, int H, int N, int B, uint32_t box_cols, uint32_t box_rows);
 
 // 3-D map over `depth` row-major [rows][cols] matrices of 16-bit (elem_bytes 2) or fp32 (elem_bytes 4) elements: row pitch
 // `ld` elements, matrix pitch `depth_stride` elements (ignored when depth == 1).  Box = 64 rows x 128 bytes, 128-byte

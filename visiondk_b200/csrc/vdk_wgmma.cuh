@@ -30,6 +30,27 @@ __device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t smem_addr, uint
   return d;
 }
 
+// 32-byte swizzle (layout type 3): the 16-column remainder of a head dim above 64, rows of 32 B = 16 x 16-bit, 8-row atoms of
+// 256 B.  K-major: one k16 step spans the whole row; 8-row groups are 256 B apart.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw32(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(256 >> 4) << 32;
+  d |= static_cast<uint64_t>(3) << 62;
+  return d;
+}
+// MN-major with 32-byte swizzle: 16 MN-elements (one row) x contraction rows, groups of 8 contraction rows 256 B apart (one k16
+// step: advance the start address by 512 B); a single 16-element MN block, so the leading byte offset is not used.
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw32(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(256 >> 4) << 32;
+  d |= static_cast<uint64_t>(3) << 62;
+  return d;
+}
+
 // before the first wgmma that reads accumulator registers written by ordinary instructions
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -116,6 +137,17 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_bf16(float (&d)[32], const ui
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d), "n"(kTB));
+}
+
+// D[64 x 16] (+)= A[64 x 16] . B[16 x 16]^T, bf16, A from registers as above, B in shared memory; kTB: 1 = MN-major B
+template <int kTB>
+__device__ __forceinline__ void wgmma_m64n16k16_rs_bf16(float (&d)[8], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d), "n"(kTB));
 }
 

@@ -6,9 +6,9 @@
 // FeatureExtractor.extract_cbir (models/faceX/face_model.py:120-144) runs per batch.
 //
 //   patchify (NCHW fp32 -> [B*N, 3*P*P] bf16)  -> GEMM(+bias)          patch embedding (Conv2d(3,C,P,P) as a GEMM)
-//   assemble: x[b,0] = cls + pos[0]; x[b,1+i] = tok[b,i] + pos[1+i]
-//   per block:  y = LN1(x); qkv = GEMM(y)+b; a = attention(qkv); x = x + GEMM(a)+b        (residual in the GEMM epilogue)
-//               y = LN2(x); h = GELU(GEMM(y)+b); x = x + GEMM(h)+b
+//   assemble: x[b,0] = cls + pos[0]; x[b,1+i] = tok[b,i] + pos[1+i]      (no class token: x[b,i] = tok[b,i] + pos[i])
+//   per block:  y = LN1(x); qkv = GEMM(y)+b; a = attention(qkv); x = x + ls1 * (GEMM(a)+b)  (residual in the GEMM epilogue;
+//               y = LN2(x); h = GELU(GEMM(y)+b); x = x + ls2 * (GEMM(h)+b)                  ls = 1 without LayerScale)
 //   y = LN_neck(LN_final(x)); embeddings = split-K GEMM over (token, channel) with BatchNorm1d folded [+ L2 normalise]
 //
 // Attention: one CTA = 64 query rows of one (image, head), 4 warps x 16 rows, K/V streamed in 64-row tiles through
@@ -46,22 +46,24 @@ vit_patchify_kernel(const float* __restrict__ x, int B, int S, int P, int Kp, __
   }
 }
 
-// x[b, 0, :] = cls + pos[0];  x[b, 1 + i, :] = tok[b, i, :] + pos[1 + i]
+// x[b, 0, :] = cls + pos[0];  x[b, 1 + i, :] = tok[b, i, :] + pos[1 + i].  cls == null (no class token): x[b, i] = tok[b, i] + pos[i]
 __global__ void __launch_bounds__(256)
 vit_assemble_kernel(const __nv_bfloat16* __restrict__ tok, const float* __restrict__ cls, const float* __restrict__ pos, int B,
                     int N, int C, __nv_bfloat16* __restrict__ x) {
-  const int64_t total = static_cast<int64_t>(B) * (N + 1) * (C / 2);
+  const int prefix = cls != nullptr ? 1 : 0;
+  const int T = N + prefix;
+  const int64_t total = static_cast<int64_t>(B) * T * (C / 2);
   for (int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
        t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int c2 = static_cast<int>(t % (C / 2));
     const int64_t row = t / (C / 2);
-    const int tk = static_cast<int>(row % (N + 1));
-    const int b = static_cast<int>(row / (N + 1));
+    const int tk = static_cast<int>(row % T);
+    const int b = static_cast<int>(row / T);
     float2 v;
-    if (tk == 0) {
+    if (tk < prefix) {
       v = make_float2(cls[2 * c2], cls[2 * c2 + 1]);
     } else {
-      v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(tok + (static_cast<int64_t>(b) * N + tk - 1) * C + 2 * c2));
+      v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(tok + (static_cast<int64_t>(b) * N + tk - prefix) * C + 2 * c2));
     }
     const float2 p = *reinterpret_cast<const float2*>(pos + static_cast<int64_t>(tk) * C + 2 * c2);
     *reinterpret_cast<__nv_bfloat162*>(x + row * C + 2 * c2) = __floats2bfloat162_rn(v.x + p.x, v.y + p.y);
@@ -267,13 +269,14 @@ attention_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, int B, int N, int H,
   }
 }
 
-int launch_attention_tc(const __nv_bfloat16* qkv, int B, int N, int H, __nv_bfloat16* out, float* lse2, cudaStream_t s);  // attention_tc.cu
+int launch_attention_tc(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
+                        cudaStream_t s);  // attention_tc.cu
 
 static int launch_attention_mma_sync(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
                                      cudaStream_t s);
 
-// Forward attention: the wgmma kernel (attention_tc.cu) by default; VDK_ATT_TC=0 selects the earlier mma.sync kernel (kept as
-// the comparison baseline and for A/B parity tests).
+// Forward attention: the wgmma kernel (attention_tc.cu, head_dim 64, 72 or 80) by default; VDK_ATT_TC=0 selects the earlier
+// mma.sync kernel (head_dim 64 only; kept as the comparison baseline and for A/B parity tests).
 static int launch_attention(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
                             cudaStream_t s) {
   static const bool use_tc = [] {
@@ -281,9 +284,10 @@ static int launch_attention(const __nv_bfloat16* qkv, int B, int N, int H, int h
     return e ? atoi(e) != 0 : true;
   }();
   if (!use_tc) return launch_attention_mma_sync(qkv, B, N, H, head_dim, out, lse2, s);
-  VDK_REQUIRE(head_dim == kAttD, "attention: head_dim must be 64 (got %d)", head_dim);
-  ProfScope prof(kProfAttention, 4.0 * static_cast<double>(B) * H * N * N * 64.0, 2.0 * static_cast<double>(B) * N * H * 64.0 * 4.0, s);
-  return launch_attention_tc(qkv, B, N, H, out, lse2, s);
+  VDK_REQUIRE(head_dim == 64 || head_dim == 72 || head_dim == 80, "attention: head_dim must be 64, 72 or 80 (got %d)", head_dim);
+  const double D = head_dim;
+  ProfScope prof(kProfAttention, 4.0 * static_cast<double>(B) * H * N * N * D, 2.0 * static_cast<double>(B) * N * H * D * 4.0, s);
+  return launch_attention_tc(qkv, B, N, H, head_dim, out, lse2, s);
 }
 
 static int launch_attention_mma_sync(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
@@ -540,6 +544,7 @@ static size_t up256v(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 
 struct VitLayout {
   int N, T, C, Kp;  // patches, tokens, width, padded patch-row length
+  int hd, mlp;      // head dim, MLP hidden width
   size_t M;         // batch * tokens
   size_t x, y, big, total;
 };
@@ -547,14 +552,20 @@ struct VitLayout {
 static int vit_layout(const vdk_vit_net* n, int batch, VitLayout* L) {
   VDK_REQUIRE(n, "vdk_vit: null network");
   VDK_REQUIRE(n->patch > 0 && n->image_size > 0 && n->image_size % n->patch == 0, "vdk_vit: image_size must be a multiple of patch");
-  VDK_REQUIRE(n->dim > 0 && n->heads > 0 && n->dim == n->heads * kAttD, "vdk_vit: dim must be heads * 64");
+  VDK_REQUIRE(n->dim > 0 && n->heads > 0 && n->dim % n->heads == 0, "vdk_vit: dim must be a multiple of heads");
+  const int hd = n->dim / n->heads;
+  VDK_REQUIRE(hd == 64 || hd == 72 || hd == 80, "vdk_vit: head dim (dim / heads) must be 64, 72 or 80 (got %d)", hd);
+  const int mlp = n->mlp_dim > 0 ? n->mlp_dim : 4 * n->dim;
+  VDK_REQUIRE(n->mlp_dim >= 0 && mlp % 8 == 0, "vdk_vit: mlp_dim must be a multiple of 8 (got %d)", n->mlp_dim);
   VDK_REQUIRE(n->dim % 256 == 0 || n->dim % 8 == 0, "vdk_vit: dim must be a multiple of 8");
   VDK_REQUIRE(n->depth > 0 && n->depth <= VDK_VIT_MAX_BLOCKS, "vdk_vit: bad depth");
   VDK_REQUIRE(n->feat_dim > 0 && n->feat_dim % 8 == 0, "vdk_vit: feat_dim must be a multiple of 8");
   const int G = n->image_size / n->patch;
   L->N = G * G;
-  L->T = L->N + 1;
+  L->T = L->N + (n->cls_token != nullptr ? 1 : 0);
   L->C = n->dim;
+  L->hd = hd;
+  L->mlp = mlp;
   L->Kp = (3 * n->patch * n->patch + 7) & ~7;
   L->M = static_cast<size_t>(batch) * L->T;
   size_t off = 0;
@@ -562,7 +573,7 @@ static int vit_layout(const vdk_vit_net* n, int batch, VitLayout* L) {
   L->x = take(L->M * L->C * 2);
   L->y = take(L->M * L->C * 2);
   // qkv / MLP hidden / patch rows + patch tokens / neck split-K slabs share one buffer
-  size_t big = L->M * 4 * static_cast<size_t>(L->C) * 2;
+  size_t big = L->M * static_cast<size_t>(std::max(3 * L->C, mlp)) * 2;
   big = std::max(big, static_cast<size_t>(batch) * L->N * (static_cast<size_t>(L->Kp) + L->C) * 2 + 256);
   big = std::max(big, static_cast<size_t>(batch) * n->feat_dim * 4 * 64);
   L->big = take(big);
@@ -609,7 +620,7 @@ extern "C" int vdk_vit_forward(const vdk_vit_net* net, const float* images, int 
   VDK_REQUIRE(images && embeddings && batch > 0, "vdk_vit_forward: null image/embedding buffer");
   VDK_REQUIRE(workspace && workspace_bytes >= L.total && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
               "vdk_vit_forward: workspace too small or misaligned");
-  VDK_REQUIRE(net->patch_w && net->cls_token && net->pos_embed && net->ones && net->norm_w && net->norm_b &&
+  VDK_REQUIRE(net->patch_w && net->pos_embed && net->ones && net->norm_w && net->norm_b &&
                   net->neck_ln_w && net->neck_ln_b && net->neck_w && net->neck_b,
               "vdk_vit_forward: null parameter");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -617,7 +628,7 @@ extern "C" int vdk_vit_forward(const vdk_vit_net* net, const float* images, int 
   __nv_bfloat16* x = reinterpret_cast<__nv_bfloat16*>(ws + L.x);
   __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(ws + L.y);
   __nv_bfloat16* big = reinterpret_cast<__nv_bfloat16*>(ws + L.big);
-  const int C = L.C, T = L.T, N = L.N, M = static_cast<int>(L.M);
+  const int C = L.C, T = L.T, N = L.N, M = static_cast<int>(L.M), Hm = L.mlp;
   const float eps = net->ln_eps > 0.f ? net->ln_eps : 1e-6f;
   VDK_REQUIRE((net->norm_pre_w == nullptr) == (net->norm_pre_b == nullptr), "vdk_vit_forward: norm_pre needs weight and bias");
 
@@ -661,15 +672,16 @@ extern "C" int vdk_vit_forward(const vdk_vit_net* net, const float* images, int 
     if (rc != VDK_OK) return rc;
     rc = gemm(y, b->qkv_w, big, M, 3 * C, C, C, VDK_EPI_NONE, b->qkv_b, nullptr, nullptr);
     if (rc != VDK_OK) return rc;
-    rc = launch_attention(big, batch, T, net->heads, kAttD, y, nullptr, s);
+    rc = launch_attention(big, batch, T, net->heads, L.hd, y, nullptr, s);
     if (rc != VDK_OK) return rc;
-    rc = gemm(y, b->proj_w, x, M, C, C, C, VDK_EPI_SCALE_RESIDUAL, b->proj_b, net->ones, x);  // x += proj(a), in place per tile
+    // x += ls1 * proj(a), in place per tile (timm's x + ls1(attn(...)); ls1 = 1 without LayerScale)
+    rc = gemm(y, b->proj_w, x, M, C, C, C, VDK_EPI_SCALE_RESIDUAL, b->proj_b, b->ls1 ? b->ls1 : net->ones, x);
     if (rc != VDK_OK) return rc;
     rc = launch_ln_patchify(x, batch, T, 1, C, b->ln2_w, b->ln2_b, eps, 1, y, nullptr, s);
     if (rc != VDK_OK) return rc;
-    rc = gemm(y, b->fc1_w, big, M, 4 * C, C, C, VDK_EPI_GELU, b->fc1_b, nullptr, nullptr);
+    rc = gemm(y, b->fc1_w, big, M, Hm, C, C, VDK_EPI_GELU, b->fc1_b, nullptr, nullptr);
     if (rc != VDK_OK) return rc;
-    rc = gemm(big, b->fc2_w, x, M, C, 4 * C, 4 * C, VDK_EPI_SCALE_RESIDUAL, b->fc2_b, net->ones, x);
+    rc = gemm(big, b->fc2_w, x, M, C, Hm, Hm, VDK_EPI_SCALE_RESIDUAL, b->fc2_b, b->ls2 ? b->ls2 : net->ones, x);
     if (rc != VDK_OK) return rc;
   }
   // ---- final LayerNorm, neck LayerNorm, Linear over (token, channel) with BatchNorm1d folded ----
@@ -799,8 +811,24 @@ vit_assemble_bwd_kernel(const __nv_bfloat16* __restrict__ dx, int B, int N, int 
 
 }  // namespace vdk
 
+// The training path is built for the plain ViT (and head dim 64: the attention backward); the features only the inference
+// forward has are refused by name.
+static int refuse_inference_only_features(const vdk_vit_net* net) {
+  VDK_REQUIRE(net, "vdk_vit_train: null net");
+  VDK_REQUIRE(net->dim == net->heads * 64, "vdk_vit_train: head dim %d: training needs head dim 64 (the attention backward)",
+              net->heads > 0 ? net->dim / net->heads : 0);
+  VDK_REQUIRE(net->mlp_dim == 0 || net->mlp_dim == 4 * net->dim, "vdk_vit_train: an MLP width other than 4 * dim (mlp_dim %d) is built "
+              "for inference only", net->mlp_dim);
+  VDK_REQUIRE(net->cls_token != nullptr, "vdk_vit_train: a ViT without a class token is built for inference only");
+  for (int i = 0; i < net->depth && i < VDK_VIT_MAX_BLOCKS; ++i)
+    VDK_REQUIRE(net->blocks[i].ls1 == nullptr && net->blocks[i].ls2 == nullptr,
+                "vdk_vit_train: LayerScale (block %d) is built for inference only", i);
+  return VDK_OK;
+}
+
 extern "C" int vdk_vit_pack(const vdk_vit_tensors* p, vdk_vit_net* net, void* stream) {
   VDK_REQUIRE(p && net, "vdk_vit_pack: null argument");
+  RC(refuse_inference_only_features(net));
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   VitLayout L;
   RC(vit_layout(net, 2, &L));
@@ -822,7 +850,7 @@ extern "C" int vdk_vit_pack(const vdk_vit_tensors* p, vdk_vit_net* net, void* st
 
 extern "C" size_t vdk_vit_train_workspace_bytes(const vdk_vit_net* net, int batch) {
   VitTrainLayout L;
-  if (!net || batch <= 1 || vit_train_layout(net, batch, &L) != VDK_OK) return 0;
+  if (!net || batch <= 1 || refuse_inference_only_features(net) != VDK_OK || vit_train_layout(net, batch, &L) != VDK_OK) return 0;
   return L.total;
 }
 
@@ -836,6 +864,7 @@ extern "C" int vdk_vit_train_forward(const vdk_vit_net* net, const vdk_vit_tenso
                                      float bn_momentum, float* out_feats, void* workspace, size_t workspace_bytes, void* stream) {
   VDK_REQUIRE(net && p && images && out_feats, "vdk_vit_train_forward: null argument");
   RC(refuse_pre_norm(net));
+  RC(refuse_inference_only_features(net));
   VitTrainLayout L;
   RC(vit_train_layout(net, batch, &L));
   VDK_REQUIRE(workspace && workspace_bytes >= L.total && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
@@ -900,6 +929,7 @@ extern "C" int vdk_vit_train_backward_units(const vdk_vit_net* net) { return net
 static int vit_backward_range(const vdk_vit_net* net, const vdk_vit_tensors* p, const vdk_vit_tensors* g, const float* d_feats, int batch,
                               void* workspace, size_t workspace_bytes, void* stream, int u_begin, int u_end) {
   VDK_REQUIRE(net && p && g && d_feats, "vdk_vit_train_backward: null argument");
+  RC(refuse_inference_only_features(net));
   VDK_REQUIRE(u_begin >= 0 && u_begin < u_end && u_end <= net->depth + 2, "vdk_vit_train_backward: bad unit range [%d, %d)", u_begin, u_end);
   auto active = [&](int unit) { return unit >= u_begin && unit < u_end; };
   VitTrainLayout L;

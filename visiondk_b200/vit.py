@@ -7,6 +7,10 @@ attn.qkv, attn.proj, norm2, mlp.fc1, mlp.fc2}`, `model.norm`) and `output_layer.
 so reference checkpoints load with `strict=True`.  The eval forward runs in `vdk_vit_forward`, the train-mode forward and
 backward (BASELINE config 3) in `vdk_vit_train_forward` / `vdk_vit_train_backward` (csrc/vit.cu) as ONE autograd node;
 training needs 3*patch^2 % 8 == 0 and at most 208 tokens (ViT-*/16 at 224^2).
+
+The CBIR configs' self-supervised and contrastive towers (DINO ViT-B/8, DINOv2 ViT-L/14, SigLIP So400m/14, CLIP ViT-H/14) add
+head dims 72 and 80, a model without a class token (`model.cls_token` absent, pos_embed [N, dim]), LayerScale
+(`model.blocks.{i}.ls1.gamma`, `ls2.gamma`) and an MLP width other than 4 * dim.  Those are built for extraction only.
 """
 from __future__ import annotations
 
@@ -27,11 +31,21 @@ VIT_ARCHS = {
     "vit_base_patch16_clip_224": (16, 768, 12, 12),
     "vit_large_patch14_clip_224": (14, 1024, 24, 16),
     "vit_large_patch14_clip_336": (14, 1024, 24, 16),
+    "vit_base_patch8_224": (8, 768, 12, 12),                # DINO ViT-B/8 (.dino)
+    "vit_large_patch14_dinov2": (14, 1024, 24, 16),        # DINOv2 ViT-L/14 (.lvd142m), 518^2
+    "vit_so400m_patch14_siglip_224": (14, 1152, 27, 16),   # SigLIP So400m/14 (.webli): head dim 72
+    "vit_huge_patch14_clip_224": (14, 1280, 32, 16),       # CLIP ViT-H/14 (.laion2b_ft_in12k_in1k): head dim 80
 }
 # timm 0.9.16 `vit_*_clip_*` (the CLIP image towers; BASELINE config 5's ViT-L/14 at 336^2): VisionTransformer(pre_norm=True,
 # norm_layer=nn.LayerNorm): a `norm_pre` LayerNorm after cls / position, NO bias in patch_embed.proj, LayerNorm eps 1e-5,
 # standard GELU (the `*_clip_quickgelu_*` architectures are separate timm entries and are not built).
-VIT_PRE_NORM = {"vit_base_patch16_clip_224", "vit_large_patch14_clip_224", "vit_large_patch14_clip_336"}
+VIT_PRE_NORM = {"vit_base_patch16_clip_224", "vit_large_patch14_clip_224", "vit_large_patch14_clip_336", "vit_huge_patch14_clip_224"}
+# timm 0.9.16 side attributes of the entries above (absent: 4 * dim MLP, a class token, no LayerScale):
+VIT_MLP_DIM = {"vit_so400m_patch14_siglip_224": 4304}          # mlp_ratio 3.7362 -> int(1152 * 3.7362)
+VIT_NO_CLASS_TOKEN = {"vit_so400m_patch14_siglip_224"}         # class_token=False: no cls_token parameter at all
+VIT_LAYER_SCALE = {"vit_large_patch14_dinov2"}                 # init_values=1e-5: blocks.{i}.ls1.gamma, ls2.gamma
+VIT_IMAGE_SIZE = {"vit_large_patch14_dinov2": 518, "vit_large_patch14_clip_336": 336}  # pretrained resolution (else 224)
+VIT_HEAD_DIMS = (64, 72, 80)
 MAX_BLOCKS = 48
 
 
@@ -43,19 +57,29 @@ class _Attention(nn.Module):
 
 
 class _Mlp(nn.Module):
-    def __init__(self, dim):
+    def __init__(self, dim, hidden):
         super().__init__()
-        self.fc1 = nn.Linear(dim, 4 * dim)
-        self.fc2 = nn.Linear(4 * dim, dim)
+        self.fc1 = nn.Linear(dim, hidden)
+        self.fc2 = nn.Linear(hidden, dim)
+
+
+class _LayerScale(nn.Module):
+    def __init__(self, dim, init_values=1e-5):
+        super().__init__()
+        self.gamma = nn.Parameter(init_values * torch.ones(dim))
 
 
 class _Block(nn.Module):
-    def __init__(self, dim, eps=1e-6):
+    def __init__(self, dim, eps=1e-6, mlp_dim=None, layer_scale=False):
         super().__init__()
         self.norm1 = nn.LayerNorm(dim, eps=eps)
         self.attn = _Attention(dim)
+        if layer_scale:
+            self.ls1 = _LayerScale(dim)
         self.norm2 = nn.LayerNorm(dim, eps=eps)
-        self.mlp = _Mlp(dim)
+        self.mlp = _Mlp(dim, mlp_dim or 4 * dim)
+        if layer_scale:
+            self.ls2 = _LayerScale(dim)
 
 
 class _PatchEmbed(nn.Module):
@@ -67,29 +91,51 @@ class _PatchEmbed(nn.Module):
 class ViTParams(nn.Module):
     """timm 0.9.16 `VisionTransformer(num_classes=0, global_pool='')` parameter tree (timm/models/vision_transformer.py)."""
 
-    def __init__(self, image_size, patch, dim, depth, heads, pre_norm=False):
+    def __init__(self, image_size, patch, dim, depth, heads, pre_norm=False, mlp_dim=None, class_token=True, layer_scale=False):
         super().__init__()
         self.image_size, self.patch, self.dim, self.depth, self.heads = image_size, patch, dim, depth, heads
         self.pre_norm = bool(pre_norm)
+        self.mlp_dim = int(mlp_dim or 4 * dim)
+        self.class_token, self.layer_scale = bool(class_token), bool(layer_scale)
         self.ln_eps = 1e-5 if pre_norm else 1e-6
         n = (image_size // patch) ** 2
+        self.tokens = n + (1 if class_token else 0)
         self.patch_embed = _PatchEmbed(patch, dim, bias=not pre_norm)
-        self.cls_token = nn.Parameter(torch.zeros(1, 1, dim))
-        self.pos_embed = nn.Parameter(torch.randn(1, n + 1, dim) * 0.02)
+        if class_token:
+            self.cls_token = nn.Parameter(torch.zeros(1, 1, dim))
+        self.pos_embed = nn.Parameter(torch.randn(1, self.tokens, dim) * 0.02)
         if pre_norm:
             self.norm_pre = nn.LayerNorm(dim, eps=self.ln_eps)
-        self.blocks = nn.Sequential(*[_Block(dim, self.ln_eps) for _ in range(depth)])
+        self.blocks = nn.Sequential(*[_Block(dim, self.ln_eps, self.mlp_dim, layer_scale) for _ in range(depth)])
         self.norm = nn.LayerNorm(dim, eps=self.ln_eps)
         for m in self.modules():
             if isinstance(m, nn.Linear):
                 nn.init.trunc_normal_(m.weight, std=0.02)
                 nn.init.zeros_(m.bias)
-        nn.init.normal_(self.cls_token, std=1e-6)
+        if class_token:
+            nn.init.normal_(self.cls_token, std=1e-6)
+
+    def inference_only_features(self):
+        """Names of what this model has that the training kernels do not implement (empty: trainable)."""
+        f = []
+        if self.pre_norm:
+            f.append("pre_norm (CLIP towers)")
+        if self.dim != 64 * self.heads:
+            f.append(f"head dim {self.dim // self.heads}")
+        if not self.class_token:
+            f.append("no class token")
+        if self.layer_scale:
+            f.append("LayerScale")
+        if self.mlp_dim != 4 * self.dim:
+            f.append(f"MLP width {self.mlp_dim}")
+        if self.tokens > 208:  # the attention backward keeps one head's probability matrix in shared memory
+            f.append(f"{self.tokens} tokens (training takes at most 208)")
+        return f
 
 
 class _VitBlockC(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("ln1_w", "ln1_b", "qkv_w", "qkv_b", "proj_w", "proj_b", "ln2_w", "ln2_b", "fc1_w", "fc1_b",
-                                          "fc2_w", "fc2_b")]
+                                          "fc2_w", "fc2_b", "ls1", "ls2")]
 
 
 class _VitBlockTensorsC(C.Structure):
@@ -114,14 +160,14 @@ class VitNetC(C.Structure):
                 ("ones", C.c_void_p), ("blocks", _VitBlockC * MAX_BLOCKS),
                 ("norm_w", C.c_void_p), ("norm_b", C.c_void_p), ("neck_ln_w", C.c_void_p), ("neck_ln_b", C.c_void_p),
                 ("neck_w", C.c_void_p), ("neck_b", C.c_void_p),
-                ("norm_pre_w", C.c_void_p), ("norm_pre_b", C.c_void_p), ("ln_eps", C.c_float)]
+                ("norm_pre_w", C.c_void_p), ("norm_pre_b", C.c_void_p), ("ln_eps", C.c_float), ("mlp_dim", C.c_int)]
 
 
 class ViTWrapper(nn.Module):
     """Drop-in for the reference's TimmWrapper when the timm model is a VisionTransformer (eval / extract path)."""
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, patch=None, dim=None, depth=None,
-                 heads=None, pre_norm=None, **kwargs):
+                 heads=None, pre_norm=None, mlp_dim=None, class_token=None, layer_scale=None, **kwargs):
         super().__init__()
         if dim is None:
             if model_name not in VIT_ARCHS:
@@ -129,11 +175,20 @@ class ViTWrapper(nn.Module):
             patch, dim, depth, heads = VIT_ARCHS[model_name]
         if pre_norm is None:
             pre_norm = model_name in VIT_PRE_NORM
-        if image_size % patch != 0 or dim != heads * 64 or depth > MAX_BLOCKS:
-            raise ValueError("ViT on H100: image_size must be a multiple of patch, head_dim must be 64, depth <= 48")
+        if mlp_dim is None:
+            mlp_dim = VIT_MLP_DIM.get(model_name, 4 * dim)
+        if class_token is None:
+            class_token = model_name not in VIT_NO_CLASS_TOKEN
+        if layer_scale is None:
+            layer_scale = model_name in VIT_LAYER_SCALE
+        if (image_size % patch != 0 or dim % heads != 0 or dim // heads not in VIT_HEAD_DIMS or depth > MAX_BLOCKS or
+                mlp_dim % 8 != 0):
+            raise ValueError("ViT on H100: image_size must be a multiple of patch, head_dim 64, 72 or 80, depth <= 48, mlp_dim a "
+                             "multiple of 8")
         self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = ViTParams(image_size, patch, dim, depth, heads, pre_norm=pre_norm)
-        tokens = (image_size // patch) ** 2 + 1
+        self.model = ViTParams(image_size, patch, dim, depth, heads, pre_norm=pre_norm, mlp_dim=mlp_dim, class_token=class_token,
+                               layer_scale=layer_scale)
+        tokens = self.model.tokens
         self.output_layer = nn.Sequential(nn.LayerNorm(dim), nn.Flatten(1), nn.Linear(tokens * dim, feat_dim),
                                           nn.BatchNorm1d(feat_dim))
         self._packed: Optional[Dict] = None
@@ -145,8 +200,9 @@ class ViTWrapper(nn.Module):
                                "load a checkpoint with load_state_dict (keys are timm's)")
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.training and self.model.pre_norm:
-            raise NotImplementedError("pre_norm ViT variants (CLIP towers) are built for inference / extraction only")
+        if self.training and self.model.inference_only_features():
+            raise NotImplementedError(f"{self.model_name}: {', '.join(self.model.inference_only_features())}: built for inference / "
+                                      "extraction only")
         if self.training:
             return _ViTTrainFn.apply(self, x, *[p for _, p in self.named_parameters()])
         return self.embed(x, l2_normalize=False)
@@ -321,7 +377,9 @@ class ViTWrapper(nn.Module):
         if m.pre_norm:
             net.norm_pre_w, net.norm_pre_b = f32(m.norm_pre.weight), f32(m.norm_pre.bias)
         net.ln_eps = float(m.ln_eps)
-        net.cls_token, net.pos_embed = f32(m.cls_token.reshape(-1)), f32(m.pos_embed.reshape(-1, m.dim))
+        net.mlp_dim = m.mlp_dim
+        net.cls_token = f32(m.cls_token.reshape(-1)) if m.class_token else 0
+        net.pos_embed = f32(m.pos_embed.reshape(-1, m.dim))
         net.ones = f32(torch.ones(m.dim))
         for i, blk in enumerate(m.blocks):
             b = net.blocks[i]
@@ -331,6 +389,8 @@ class ViTWrapper(nn.Module):
             b.ln2_w, b.ln2_b = f32(blk.norm2.weight), f32(blk.norm2.bias)
             b.fc1_w, b.fc1_b = bf16(blk.mlp.fc1.weight), f32(blk.mlp.fc1.bias)
             b.fc2_w, b.fc2_b = bf16(blk.mlp.fc2.weight), f32(blk.mlp.fc2.bias)
+            if m.layer_scale:
+                b.ls1, b.ls2 = f32(blk.ls1.gamma), f32(blk.ls2.gamma)
         net.norm_w, net.norm_b = f32(m.norm.weight), f32(m.norm.bias)
         ln, lin, bn = self.output_layer[0], self.output_layer[2], self.output_layer[3]
         net.neck_ln_w, net.neck_ln_b = f32(ln.weight), f32(ln.bias)
