@@ -49,6 +49,9 @@ int vdk_device_check(void);
 #define VDK_EPI_LAYERNORM 3      /* D = LayerNorm_N(acc + bias) * gamma + beta; the tile must span the row (N <= 256) */
 #define VDK_EPI_MUL_GELU_GRAD 4  /* D = acc * gelu'(residual[m,n]): dgrad through the MLP's GELU (residual = saved pre-activation);
                                     the derivative of the same fp16x2 form, |gelu'~ - gelu'| <= 8e-3 before the output rounding */
+/* vdk_conv2d only (vdk_gemm rejects them): */
+#define VDK_EPI_RELU 5           /* D = max(acc + bias[n], 0)  (conv + folded BatchNorm + ReLU) */
+#define VDK_EPI_RESIDUAL_RELU 6  /* D = max(residual[m,n] + (acc + bias[n]), 0)  (last conv of a ResNet bottleneck) */
 
 typedef struct vdk_gemm_desc {
   const void* A; /* [M,K] 16-bit, pitch lda */
@@ -87,6 +90,61 @@ int vdk_gemm_tn(const void* A, const void* B, void* D, int M, int N, int K, int 
                 const float* gamma,    /* [N], VDK_EPI_SCALE_RESIDUAL only */
                 const void* residual,  /* [M,ldr] same dtype as D, VDK_EPI_SCALE_RESIDUAL only */
                 int ldr, void* stream);
+
+/* ---- dense 2-D convolution: implicit GEMM on the wgmma GEMM --------------------------------- */
+/* y = epilogue(conv2d(x, w) + bias): NHWC bf16 activations, square kernel, equal stride and zero padding on both axes —
+ * the Conv2d + eval BatchNorm (folded into w and bias) [+ residual] + ReLU of timm's ResNet Bottleneck
+ * (timm/models/resnet.py).  The GEMM row is the output pixel (b, ho, wo), M = B*Ho*Wo; K = kernel*kernel*Cin in
+ * (kh, kw, cin) order.  1x1 / stride-1 convolutions run as a plain GEMM over [B*H*W, Cin]; every other shape gathers its
+ * A tiles straight from x with TMA im2col loads (no im2col buffer).  Ho = (H + 2 pad - kernel) / stride + 1. */
+typedef struct vdk_conv_desc {
+  const void* x;        /* [B, H, W, Cin] bf16 */
+  const void* w;        /* [Cout, kernel, kernel, Cin] bf16 */
+  const float* bias;    /* [Cout] or NULL */
+  const void* residual; /* [B, Ho, Wo, Cout] bf16, VDK_EPI_RESIDUAL_RELU only; may be y itself (in place) */
+  void* y;              /* [B, Ho, Wo, Cout] bf16 */
+  int B, H, W, Cin, Cout;
+  int kernel, stride, pad;
+  int epilogue; /* VDK_EPI_NONE, VDK_EPI_RELU or VDK_EPI_RESIDUAL_RELU */
+} vdk_conv_desc;
+/* Cin a multiple of 64, Cout a multiple of 8, 1 <= kernel <= 16, 1 <= stride <= 8, 0 <= pad < kernel. */
+int vdk_conv2d(const vdk_conv_desc* desc, void* stream);
+
+/* ---- ResNet embedding forward (eval) --------------------------------------------------------- */
+/* Replaces TimmWrapper.forward for timm's Bottleneck ResNets (resnet50/101/152, their -D variants, wide_resnet50_2/101_2;
+ * models/faceX/backbone/timm_wrapper.py:16-21, 30-38, 51-54) followed by F.normalize (face_model.py:139): every eval
+ * BatchNorm folded into its conv (bf16 weight [Cout, kh, kw, Cin], fp32 bias), NHWC bf16 activations in `workspace`. */
+#define VDK_RESNET_MAX_BLOCKS 64
+typedef struct vdk_resnet_conv {
+  const void* w;  /* bf16 [Cout, kh, kw, Cin] (stem: [Cout, Kp] patch rows, see below) */
+  const float* b; /* [Cout] */
+} vdk_resnet_conv;
+typedef struct vdk_resnet_block {
+  vdk_resnet_conv conv1; /* 1x1, Cin -> width, + ReLU */
+  vdk_resnet_conv conv2; /* 3x3 / stride (1, or 2 in the first block of stages 2-4), + ReLU */
+  vdk_resnet_conv conv3; /* 1x1, width -> 4 * planes, + shortcut, + ReLU */
+  vdk_resnet_conv down;  /* shortcut conv, w == NULL: identity.  1x1 / stride; with avg_down and stride 2 the
+                            AvgPool2d(2, 2) is folded in: [Cout, 2, 2, Cin] with the 1x1 weight / 4 at every tap */
+} vdk_resnet_block;
+typedef struct vdk_resnet_net {
+  int image_size; /* square input side, multiple of 32 */
+  int feat_dim;   /* embedding width, multiple of 8 */
+  int depths[4];
+  int base_width; /* 64, or 128 for wide_resnet*_2: width of stage s's 3x3 conv = base_width * 2^s */
+  int deep_stem;  /* 0: conv 7x7/s2 (stem[0], Kp = 192); 1: ResNet-D deep stem 3x3/s2 3->32 (Kp 64), 3x3 32->32, 3x3 32->64
+                     (Kp 320 each) — all as GEMMs over zero-padded (kh, kw, c) patch rows */
+  int avg_down;   /* 1: the shortcut of stride-2 blocks is AvgPool2d(2, 2) + 1x1 conv (ResNet-D) */
+  vdk_resnet_conv stem[3]; /* the stem's BatchNorms folded in (bn1 into the last one) */
+  vdk_resnet_block blocks[VDK_RESNET_MAX_BLOCKS]; /* stage-major */
+  const void* neck_w;  /* [feat_dim, h*w*2048] bf16, K order (h, w, c), BN2d/BN1d eval statistics folded in */
+  const float* neck_b; /* [feat_dim] */
+} vdk_resnet_net;
+size_t vdk_resnet_workspace_bytes(const vdk_resnet_net* net, int batch);
+/* images: fp32 NCHW [batch,3,S,S]; embeddings: fp32 [batch, feat_dim], L2-normalised when l2_normalize != 0. */
+int vdk_resnet_forward(const vdk_resnet_net* net, const float* images, int batch, int l2_normalize, float* embeddings,
+                       void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_conv_desc and vdk_resnet_net, in that order (vdk_struct_sizes' contract for these two). */
+int vdk_resnet_struct_sizes(size_t* out, int n);
 
 /* ---- ConvNeXt embedding forward (eval) ------------------------------------------------------ */
 /* Replaces TimmWrapper.forward (models/faceX/backbone/timm_wrapper.py:51-54: timm ConvNeXt features with

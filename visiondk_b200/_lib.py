@@ -15,6 +15,7 @@ VDK_OK = 0
 VDK_ERR_INVALID, VDK_ERR_CUDA, VDK_ERR_WORKSPACE, VDK_ERR_OVERFLOW = -1, -2, -3, -4
 DTYPE_BF16, DTYPE_FP16, DTYPE_FP32 = 0, 1, 2
 EPI_NONE, EPI_GELU, EPI_SCALE_RESIDUAL, EPI_LAYERNORM, EPI_MUL_GELU_GRAD = 0, 1, 2, 3, 4
+EPI_RELU, EPI_RESIDUAL_RELU = 5, 6  # vdk_conv2d only
 
 
 class HeadDesc(C.Structure):
@@ -63,6 +64,14 @@ class GemmDesc(C.Structure):
     ]
 
 
+class ConvDesc(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("w", C.c_void_p), ("bias", C.c_void_p), ("residual", C.c_void_p), ("y", C.c_void_p),
+        ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("Cin", C.c_int), ("Cout", C.c_int),
+        ("kernel", C.c_int), ("stride", C.c_int), ("pad", C.c_int), ("epilogue", C.c_int),
+    ]
+
+
 # name -> (restype, argtypes); must list every symbol include/vdk_b200.h declares (tests check this).
 SIGNATURES = {
     "vdk_version": (_i, []),
@@ -76,6 +85,10 @@ SIGNATURES = {
     "vdk_prof_end": (_i, [C.POINTER(ProfTotal), _i]),
     "vdk_gemm": (_i, [_p, _p]),
     "vdk_gemm_effective_splits": (_i, [_i, _i]),
+    "vdk_conv2d": (_i, [_p, _p]),
+    "vdk_resnet_workspace_bytes": (_sz, [_p, _i]),
+    "vdk_resnet_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
+    "vdk_resnet_struct_sizes": (_i, [_p, _i]),
     "vdk_dwconv7_ln": (_i, [_p, _i, _i, _i, _i, _p, _p, _p, _p, C.c_float, _p, _p]),
     "vdk_layernorm_patchify": (_i, [_p, _i, _i, _i, _i, _p, _p, C.c_float, _i, _p, _p]),
     "vdk_dwconv7": (_i, [_i, _p, _i, _i, _i, _i, _p, _p, _p, _p, C.c_float, _p, _p, _p, _p]),

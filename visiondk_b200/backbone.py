@@ -92,6 +92,21 @@ class ConvNeXtParams(nn.Module):
                 nn.init.zeros_(m.bias)
 
 
+@torch.no_grad()
+def fold_cnn_neck(output_layer: nn.Sequential, c_last: int, hw: int, feat_dim: int, device):
+    """The CNN neck BatchNorm2d -> Flatten -> Linear -> BatchNorm1d (eval statistics) as one Linear over the final map in
+    (h, w, c) order: (weight [feat_dim, hw*hw*c_last], bias [feat_dim]) in fp64."""
+    bn2, lin, bn1 = output_layer[0], output_layer[2], output_layer[3]
+    s2 = (bn2.weight.double() / torch.sqrt(bn2.running_var.double() + bn2.eps)).to(device)
+    t2 = (bn2.bias.double().to(device) - bn2.running_mean.double().to(device) * s2)
+    s1 = (bn1.weight.double() / torch.sqrt(bn1.running_var.double() + bn1.eps)).to(device)
+    w = lin.weight.detach().double().to(device).reshape(feat_dim, c_last, hw, hw)
+    bias = lin.bias.detach().double().to(device) + (w * t2.view(1, -1, 1, 1)).sum(dim=(1, 2, 3))
+    bias = s1 * (bias - bn1.running_mean.double().to(device)) + bn1.bias.double().to(device)
+    w = w * s2.view(1, -1, 1, 1) * s1.view(-1, 1, 1, 1)
+    return w.permute(0, 2, 3, 1).reshape(feat_dim, hw * hw * c_last), bias
+
+
 class _BlockC(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("dw_w", "dw_b", "ln_w", "ln_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "gamma",
                                           "dw_w_flip", "fc2_wg")]
@@ -404,17 +419,7 @@ class TimmWrapper(nn.Module):
                 b.gamma = f32(blk.gamma)
                 bi += 1
         net.head_ln_w, net.head_ln_b = f32(m.head.norm.weight), f32(m.head.norm.bias)
-        bn2, lin, bn1 = self.output_layer[0], self.output_layer[2], self.output_layer[3]
-        c_last, hw = m.dims[-1], self.image_size // 32
-        with torch.no_grad():
-            s2 = (bn2.weight.double() / torch.sqrt(bn2.running_var.double() + bn2.eps)).to(device)
-            t2 = (bn2.bias.double().to(device) - bn2.running_mean.double().to(device) * s2)
-            s1 = (bn1.weight.double() / torch.sqrt(bn1.running_var.double() + bn1.eps)).to(device)
-            w = lin.weight.detach().double().to(device).reshape(self.feat_dim, c_last, hw, hw)
-            bias = lin.bias.detach().double().to(device) + (w * t2.view(1, -1, 1, 1)).sum(dim=(1, 2, 3))
-            bias = s1 * (bias - bn1.running_mean.double().to(device)) + bn1.bias.double().to(device)
-            w = w * s2.view(1, -1, 1, 1) * s1.view(-1, 1, 1, 1)
-            w = w.permute(0, 2, 3, 1).reshape(self.feat_dim, hw * hw * c_last)
+        w, bias = fold_cnn_neck(self.output_layer, m.dims[-1], self.image_size // 32, self.feat_dim, device)
         net.neck_w, net.neck_b = bf16(w), f32(bias)
         self._packed, self._packed_key = {"net": net, "keep": keep}, key
         return net
@@ -460,4 +465,7 @@ class BackboneFactory:
         if model_name.startswith("vit_"):  # Transformer backbones: eval / extract path (visiondk_b200/vit.py)
             from .vit import ViTWrapper
             return ViTWrapper(model_name=model_name, **self.backbone_param)
+        from .resnet import RESNET_ARCHS, ResNetWrapper
+        if model_name in RESNET_ARCHS:  # Bottleneck ResNets: eval / extract path (visiondk_b200/resnet.py)
+            return ResNetWrapper(model_name=model_name, **self.backbone_param)
         return TimmWrapper(model_name=model_name, **self.backbone_param)

@@ -842,6 +842,30 @@ int launch_neck_finalize(const float* slabs, int n_slabs, size_t slab_stride, in
 
 static size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 
+int launch_neck(const __nv_bfloat16* feats, int batch, int Kn, int F, const void* neck_w, const float* neck_b, int l2_normalize,
+                float* scratch, size_t scratch_bytes, float* embeddings, cudaStream_t s) {
+  const int tiles = ((batch + 127) / 128) * ((F + 255) / 256);
+  // split-K over ~2 waves of CTAs; every split writes its own fp32 slab into the scratch buffer and neck_finalize adds the
+  // slabs in order, so the embedding is bitwise reproducible
+  const size_t slab = static_cast<size_t>(batch) * F;
+  int split = std::max(1, (2 * sm_count()) / std::max(1, tiles));
+  split = static_cast<int>(std::min<size_t>(split, scratch_bytes / (slab * sizeof(float))));
+  split = vdk_gemm_effective_splits(Kn, std::max(1, split));
+  {
+    vdk_gemm_desc g{};
+    g.A = feats; g.B = neck_w; g.D = scratch;
+    g.M = batch; g.N = F; g.K = Kn; g.lda = Kn; g.ldb = Kn; g.ldd = F;
+    g.in_dtype = VDK_DTYPE_BF16; g.out_dtype = VDK_DTYPE_FP32; g.epilogue = VDK_EPI_NONE;
+    g.split_k = split;
+    g.split_stride = split > 1 ? static_cast<long long>(slab) : 0;
+    const int rc = gemm_run(g, s);
+    if (rc != VDK_OK) return rc;
+  }
+  neck_finalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, s>>>(scratch, split, slab, batch, F, neck_b, l2_normalize, embeddings);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
 static int check_net(const vdk_convnext_net* n) {
   VDK_REQUIRE(n, "vdk_convnext: null network");
   VDK_REQUIRE(n->image_size > 0 && n->image_size % 32 == 0, "vdk_convnext: image_size must be a multiple of 32");
@@ -1151,30 +1175,7 @@ extern "C" int vdk_convnext_forward(const vdk_convnext_net* net, const float* im
     if (rc != VDK_OK) return rc;
   }
   // ---- neck: BN2d -> Flatten -> Linear -> BN1d, all folded into one skinny GEMM (eval statistics) ----
-  {
-    const int Kn = H * W * C, F = net->feat_dim;
-    const int tiles = ((batch + 127) / 128) * ((F + 255) / 256);
-    // split-K over ~2 waves of CTAs; every split writes its own fp32 slab into the (now idle) hidden buffer and
-    // neck_finalize adds the slabs in order, so the embedding is bitwise reproducible
-    const size_t slab = static_cast<size_t>(batch) * F;
-    const size_t hbytes = up256(std::max(max_m4c, static_cast<size_t>(batch) * hw0 * 48) * 2);
-    int split = std::max(1, (2 * sm_count()) / std::max(1, tiles));
-    split = static_cast<int>(std::min<size_t>(split, hbytes / (slab * sizeof(float))));
-    split = vdk_gemm_effective_splits(Kn, std::max(1, split));
-    float* slabs = reinterpret_cast<float*>(hbuf);
-    {
-      vdk_gemm_desc g{};
-      g.A = ybuf; g.B = net->neck_w; g.D = slabs;
-      g.M = batch; g.N = F; g.K = Kn; g.lda = Kn; g.ldb = Kn; g.ldd = F;
-      g.in_dtype = VDK_DTYPE_BF16; g.out_dtype = VDK_DTYPE_FP32; g.epilogue = VDK_EPI_NONE;
-      g.split_k = split;
-      g.split_stride = split > 1 ? static_cast<long long>(slab) : 0;
-      rc = gemm_run(g, s);
-      if (rc != VDK_OK) return rc;
-    }
-    neck_finalize_kernel<<<(batch * 32 + 255) / 256, 256, 0, s>>>(slabs, split, slab, batch, F, net->neck_b, l2_normalize,
-                                                                 embeddings);
-    VDK_CUDA_OK(cudaGetLastError());
-  }
-  return VDK_OK;
+  return launch_neck(ybuf, batch, H * W * C, net->feat_dim, net->neck_w, net->neck_b, l2_normalize,
+                     reinterpret_cast<float*>(hbuf), up256(std::max(max_m4c, static_cast<size_t>(batch) * hw0 * 48) * 2),
+                     embeddings, s);
 }

@@ -17,6 +17,12 @@ int launch_ln_patchify(const __nv_bfloat16* x, int B, int H, int W, int C, const
                        int patch, __nv_bfloat16* out, float* rstd_out, cudaStream_t s);
 
 // embeddings[row] = bias + sum of split-K slabs (fixed order) [, canonically L2-normalised]
+// The CNN neck (BN2d -> Flatten -> Linear -> BN1d folded into neck_w / neck_b): feats [batch, Kn] bf16 (the final map in
+// (h, w, c) order) -> embeddings [batch, F] fp32 [, L2-normalised], as a deterministic split-K GEMM whose fp32 slabs go
+// to `scratch` (as many splits as fit in scratch_bytes, up to ~2 waves) + neck_finalize.
+int launch_neck(const __nv_bfloat16* feats, int batch, int Kn, int F, const void* neck_w, const float* neck_b, int l2_normalize,
+                float* scratch, size_t scratch_bytes, float* embeddings, cudaStream_t s);
+
 int launch_neck_finalize(const float* slabs, int n_slabs, size_t slab_stride, int B, int F, const float* bias, int l2norm,
                          float* out, cudaStream_t s);
 

@@ -24,21 +24,42 @@ constexpr int kBM = 128;
 constexpr int kBK = 64;  // 64 x 16-bit = one 128-byte swizzle row
 constexpr int kGemmThreads = 384;  // producer warpgroup, two consumer warpgroups
 constexpr int kBoxBytes = 64 * 128;  // epilogue box: one warpgroup's 64 rows x 128 bytes (64 16-bit or 32 fp32 columns)
+// A-operand / epilogue set of a gemm_tn_kernel instantiation.  kGemmPlain: vdk_gemm (dense A, epilogues NONE..MUL_GELU_GRAD);
+// the two convolution modes add the ReLU epilogues and are compiled only into vdk_conv2d's instantiations.
+constexpr int kGemmPlain = 0;
+constexpr int kConvDense = 1;   // 1x1 / stride-1 convolution: a plain GEMM over [B*H*W, Cin]
+constexpr int kConvIm2col = 2;  // k x k / stride-s convolution: A tiles gathered from NHWC by TMA im2col loads
 
+// The implicit-GEMM convolution modes (kConvIm2col) overlay their geometry on fields they do not use, so that the struct —
+// and with it the code of the plain GEMM instantiations — stays as it is.
 struct GemmParams {
   int M, N, K;
   void* D;
   int ldd;
   const float* bias;
-  const float* gamma;  // layer-scale (SCALE_RESIDUAL) or LayerNorm weight (LAYERNORM)
-  const float* beta;   // LayerNorm bias
+  union {
+    struct {
+      const float* gamma;  // layer-scale (SCALE_RESIDUAL) or LayerNorm weight (LAYERNORM)
+      const float* beta;   // LayerNorm bias
+    };
+    struct {  // convolution: row m = output pixel (b, ho, wo); K blocks = (filter tap (dy, dx) row-major, 64-channel block)
+      int cv_cpb;               // Cin / 64: K blocks per filter tap
+      int cv_kw;                // filter width
+      int cv_stride, cv_pad;
+    };
+  };
   const void* residual;  // SCALE_RESIDUAL: added; MUL_GELU_GRAD: the saved 16-bit pre-activation whose GELU' scales the output
   int ldr;
   int out_dtype;
   int epilogue;
   float ln_eps;
   int split_k;  // > 1: each tile's K range is split over split_k work items, fp32 partials are atomically added
-  long long split_stride;  // > 0: split s writes its partial tile to D + s*split_stride with plain stores (deterministic)
+  union {
+    long long split_stride;  // > 0: split s writes its partial tile to D + s*split_stride with plain stores (deterministic)
+    struct {
+      int cv_wo, cv_howo;  // convolution: output width, output pixels per image
+    };
+  };
   void* aux;  // GELU only: also store the pre-activation (acc + bias) here, pitch ldd (saved for the backward)
   int partial_out;  // the caller asked for split-K: raw fp32 partials are added / slab-stored even if one split remains
 };
@@ -135,7 +156,7 @@ __device__ __forceinline__ float2 unpack2(uint32_t u, int dtype) {
 // copy of the tile's bias / gamma / beta ([3][BN], zero beyond N), staged once per tile so that the epilogue's critical
 // path holds no global loads.  `r`: the residual / saved pre-activation pair.  The operations and their order are those
 // of the row-wise form: + bias, then the epilogue (fp32 throughout, GELU and GELU' in fp16x2 pairs).
-template <int BN>
+template <int BN, int kMode>
 __device__ __forceinline__ void epi_pair(const GemmParams& p, float& x0, float& x1, const float* par, int c, float ln_mean,
                                          float ln_rstd, float2 r) {
   if (p.bias != nullptr && p.epilogue != VDK_EPI_LAYERNORM) {  // LayerNorm: added to the accumulator before the statistics
@@ -162,6 +183,15 @@ __device__ __forceinline__ void epi_pair(const GemmParams& p, float& x0, float& 
     x0 += r.x;
     x1 += r.y;
   }
+  if constexpr (kMode != kGemmPlain) {
+    if (p.epilogue == VDK_EPI_RELU) {
+      x0 = fmaxf(x0, 0.f);
+      x1 = fmaxf(x1, 0.f);
+    } else if (p.epilogue == VDK_EPI_RESIDUAL_RELU) {
+      x0 = fmaxf(x0 + r.x, 0.f);
+      x1 = fmaxf(x1 + r.y, 0.f);
+    }
+  }
 }
 
 // A warpgroup's box in ring slot `slot` is written: make it visible to the async proxy, let the leader hand it to TMA
@@ -185,7 +215,8 @@ __device__ __forceinline__ void epi_publish(const CUtensorMap* map, const uint8_
 __device__ __forceinline__ uint32_t box_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
 
 // kTA / kTB: operand stored with the contraction index as the slow dimension ([K,M] / [K,N] row-major: MN-major)
-template <int BN, bool kBf16, int kTA, int kTB>
+// kMode: kGemmPlain, kConvDense or kConvIm2col (see above)
+template <int BN, bool kBf16, int kTA, int kTB, int kMode>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_aux,
@@ -209,7 +240,9 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     prefetch_tensormap(&map_b);
     prefetch_tensormap(&map_d);
     if (p.aux != nullptr) prefetch_tensormap(&map_aux);
-    if (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD) prefetch_tensormap(&map_r);
+    if (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
+        (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU))
+      prefetch_tensormap(&map_r);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
@@ -238,12 +271,25 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         const int n0 = (mn % num_n) * BN;
         const int kb0 = split * kb_per_split;
         const int kb1 = min(kb0 + kb_per_split, num_kb_total);
+        // im2col: the tile's first output pixel, as the input position of its filter window's top-left tap.  The TMA unit
+        // walks the next 127 pixels through the map's bounding box (across rows and images); rows past M read as zero.
+        int cw = 0, ch = 0, cn = 0;
+        if constexpr (kMode == kConvIm2col) {
+          cn = m0 / p.cv_howo;
+          const int r = m0 - cn * p.cv_howo, ho = r / p.cv_wo;
+          ch = ho * p.cv_stride - p.cv_pad;
+          cw = (r - ho * p.cv_wo) * p.cv_stride - p.cv_pad;
+        }
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait_relaxed<true>(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kStageA;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          if (kTA) {  // [K,M] storage: 64-wide M blocks x 64 contraction rows, 8 KB each
+          if constexpr (kMode == kConvIm2col) {  // K block kb = (filter tap, 64-channel block)
+            const int tap = kb / p.cv_cpb, c0 = (kb - tap * p.cv_cpb) * kBK, dy = tap / p.cv_kw;
+            tma_load_im2col_4d(sa, &map_a, &full_bar[stage], c0, cw, ch, cn, static_cast<uint16_t>(tap - dy * p.cv_kw),
+                               static_cast<uint16_t>(dy), kEvictNormal);
+          } else if (kTA) {  // [K,M] storage: 64-wide M blocks x 64 contraction rows, 8 KB each
 #pragma unroll
             for (int j = 0; j < kBM / 64; ++j) tma_load_2d(sa + j * 8192, &map_a, &full_bar[stage], m0 + j * 64, kb * kBK, kEvictNormal);
           } else {
@@ -285,7 +331,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     float* par = par_all + cg * Cfg::kParFloats;
     const bool f32 = p.out_dtype == VDK_DTYPE_FP32;
     const int box_cols = f32 ? 32 : 64;
-    const bool has_res = p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD;
+    const bool has_res = p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
+                         (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU);
     const bool reduce = p.partial_out && p.split_stride == 0;  // atomic split-K: TMA reduce-add into D
     int slot = 0;  // ring slot of the next box
     uint32_t res_phase = 0;
@@ -427,7 +474,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 const int r = frow + 8 * h;
                 float2* dst = reinterpret_cast<float2*>(box + box_off(r, 2 * q + (fcol >> 2)) + (fcol & 2) * 4);
                 float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-                if (!p.partial_out) epi_pair<BN>(p, x0, x1, par, j * 8 + fcol, ln_mean[h], ln_rstd[h], has_res ? *dst : make_float2(0.f, 0.f));
+                if (!p.partial_out) epi_pair<BN, kMode>(p, x0, x1, par, j * 8 + fcol, ln_mean[h], ln_rstd[h], has_res ? *dst : make_float2(0.f, 0.f));
                 *dst = make_float2(x0, x1);
               }
             }
@@ -486,7 +533,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
               for (int i = 0; i < 4; ++i) {
                 const int j = sc * 8 + 2 * q + (i >> 1), h = i & 1;
                 float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-                epi_pair<BN>(p, x0, x1, par, j * 8 + fcol, ln_mean[h], ln_rstd[h], unpack2(rin[i], p.out_dtype));
+                epi_pair<BN, kMode>(p, x0, x1, par, j * 8 + fcol, ln_mean[h], ln_rstd[h], unpack2(rin[i], p.out_dtype));
                 rq[i] = pack2(x0, x1, p.out_dtype);
               }
               stmatrix_x4(addr, rq);
@@ -501,10 +548,10 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   }
 }
 
-template <int BN, bool kBf16, int kTA, int kTB>
+template <int BN, bool kBf16, int kTA, int kTB, int kMode = kGemmPlain>
 static int launch_gemm(const CUtensorMap* maps, const GemmParams& p, cudaStream_t stream) {
   constexpr int kSmem = GemmCfg<BN>::kSmemBytes;
-  auto kern = gemm_tn_kernel<BN, kBf16, kTA, kTB>;
+  auto kern = gemm_tn_kernel<BN, kBf16, kTA, kTB, kMode>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
@@ -625,7 +672,65 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   return bf ? launch_gemm_major<128, true>(maps, p, ta, tb, s) : launch_gemm_major<128, false>(maps, p, ta, tb, s);
 }
 
+int conv_run(const vdk_conv_desc& c, cudaStream_t s) {
+  VDK_REQUIRE(c.x && c.w && c.y, "vdk_conv2d: null operand");
+  VDK_REQUIRE(c.B > 0 && c.H > 0 && c.W > 0, "vdk_conv2d: empty input B=%d H=%d W=%d", c.B, c.H, c.W);
+  VDK_REQUIRE(c.Cin > 0 && c.Cin % 64 == 0, "vdk_conv2d: Cin must be a positive multiple of 64 (Cin=%d)", c.Cin);
+  VDK_REQUIRE(c.Cout > 0 && c.Cout % 8 == 0, "vdk_conv2d: Cout must be a positive multiple of 8 (Cout=%d)", c.Cout);
+  // the im2col map holds the bounding-box corners in 8 signed bits and the tap offsets in 8 unsigned bits
+  VDK_REQUIRE(c.kernel >= 1 && c.kernel <= 16 && c.stride >= 1 && c.stride <= 8 && c.pad >= 0 && c.pad < c.kernel,
+              "vdk_conv2d: unsupported kernel=%d stride=%d pad=%d", c.kernel, c.stride, c.pad);
+  VDK_REQUIRE(c.H + 2 * c.pad >= c.kernel && c.W + 2 * c.pad >= c.kernel, "vdk_conv2d: kernel larger than the padded input");
+  VDK_REQUIRE(c.epilogue == VDK_EPI_NONE || c.epilogue == VDK_EPI_RELU || c.epilogue == VDK_EPI_RESIDUAL_RELU,
+              "vdk_conv2d: epilogue must be NONE, RELU or RESIDUAL_RELU (got %d)", c.epilogue);
+  VDK_REQUIRE((c.epilogue == VDK_EPI_RESIDUAL_RELU) == (c.residual != nullptr),
+              "vdk_conv2d: a residual is given exactly with the RESIDUAL_RELU epilogue");
+  VDK_REQUIRE((reinterpret_cast<uintptr_t>(c.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.w) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(c.y) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.residual) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(c.bias) & 15) == 0,
+              "vdk_conv2d: operands must be 16-byte aligned");
+  const int Ho = (c.H + 2 * c.pad - c.kernel) / c.stride + 1, Wo = (c.W + 2 * c.pad - c.kernel) / c.stride + 1;
+  const long long M = static_cast<long long>(c.B) * Ho * Wo;
+  const long long K = static_cast<long long>(c.kernel) * c.kernel * c.Cin;
+  VDK_REQUIRE(M < (1ll << 31) && K < (1ll << 31), "vdk_conv2d: problem too large (M=%lld K=%lld)", M, K);
+  const bool dense = c.kernel == 1 && c.stride == 1;  // pad < kernel: no padding either
+  const bool wide = (c.Cout % 256 == 0) || c.Cout > 512;
+  const int BN = wide ? 256 : 128;
+  CUtensorMap maps[5];  // A, B, D, aux_out (unused), residual
+  int rc = dense ? make_tma_2d_16bit(&maps[0], c.x, (uint64_t)M, (uint64_t)c.Cin, (uint64_t)c.Cin, kBM, kBK)
+                 : make_tma_im2col_16bit(&maps[0], c.x, c.B, c.H, c.W, c.Cin, c.kernel, c.stride, c.pad);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_2d_16bit(&maps[1], c.w, (uint64_t)c.Cout, (uint64_t)K, (uint64_t)K, BN, kBK);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_epilogue_map(&maps[2], c.y, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
+  if (rc != VDK_OK) return rc;
+  maps[3] = maps[2];
+  maps[4] = maps[2];
+  if (c.residual != nullptr) {
+    rc = make_tma_epilogue_map(&maps[4], c.residual, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
+    if (rc != VDK_OK) return rc;
+  }
+  GemmParams p{};
+  p.M = static_cast<int>(M); p.N = c.Cout; p.K = static_cast<int>(K);
+  p.D = c.y; p.ldd = c.Cout; p.bias = c.bias; p.residual = c.residual; p.ldr = c.Cout;
+  p.out_dtype = VDK_DTYPE_BF16; p.epilogue = c.epilogue; p.split_k = 1;
+  p.cv_cpb = c.Cin / kBK; p.cv_kw = c.kernel; p.cv_stride = c.stride; p.cv_pad = c.pad;
+  p.cv_wo = Wo; p.cv_howo = Ho * Wo;
+  // algorithmic bytes: the input once, the weights once, the output once, the residual once
+  ProfScope prof(kProfGemm, 2.0 * M * c.Cout * K,
+                 2.0 * (static_cast<double>(c.B) * c.H * c.W * c.Cin + static_cast<double>(c.Cout) * K + M * c.Cout) +
+                     (c.residual ? 2.0 * M * c.Cout : 0.0),
+                 s);
+  if (dense) return wide ? launch_gemm<256, true, 0, 0, kConvDense>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvDense>(maps, p, s);
+  return wide ? launch_gemm<256, true, 0, 0, kConvIm2col>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvIm2col>(maps, p, s);
+}
+
 }  // namespace vdk
+
+extern "C" int vdk_conv2d(const vdk_conv_desc* desc, void* stream) {
+  VDK_REQUIRE(desc, "vdk_conv2d: null descriptor");
+  return vdk::conv_run(*desc, reinterpret_cast<cudaStream_t>(stream));
+}
 
 extern "C" int vdk_gemm_effective_splits(int K, int split_k) {
   int split = split_k < 1 ? 1 : split_k;

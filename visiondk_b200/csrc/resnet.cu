@@ -1,0 +1,250 @@
+// resnet.cu — timm 0.9.16 Bottleneck ResNet (resnet50/101/152, -D variants, wide_resnet*_2) embedding forward for the
+// faceX / CBIR extract path, NHWC bf16, every eval BatchNorm folded into its convolution.
+//
+// Replaces TimmWrapper.forward for ResNet backbones (models/faceX/backbone/timm_wrapper.py:16-21, 30-38, 51-54: timm
+// ResNet with num_classes=0, global_pool='' -> BatchNorm2d -> Flatten -> Linear -> BatchNorm1d) and F.normalize
+// (face_model.py:139).
+//
+// Every convolution of the stages is vdk_conv2d (gemm.cu: 1x1 / stride 1 as a plain GEMM, 3x3 and stride-2 shortcuts as
+// implicit GEMMs with TMA im2col A tiles) with the bias + ReLU / residual + ReLU epilogues.  Written here:
+//   patch_rows   the stem's explicit im2col: fp32 NCHW image (or the deep stem's 32-channel bf16 maps) -> bf16 rows of
+//                (kh, kw, c) zero padded to a multiple of 64, then a GEMM with the ReLU epilogue (Cin = 3 or 32 is too
+//                narrow for the 64-channel im2col loads)
+//   maxpool3s2   MaxPool2d(3, 2, padding 1) over NHWC
+// and the neck is the ConvNeXt path's (launch_neck).
+#include "vdk_host.h"
+
+#include <algorithm>
+#include "convnext_internal.h"
+
+namespace vdk {
+
+// out[m][e] for output pixel m = (b, ho, wo) and e = (dy * k + dx) * C + c < K: x[b, c, ho*stride - pad + dy, ...] (zero
+// outside the image), 0 for K <= e < Kp.  One thread writes 8 consecutive entries (16 bytes) of a row.
+template <typename T, bool kNCHW>
+__global__ void __launch_bounds__(256) patch_rows_kernel(const T* __restrict__ x, int B, int H, int W, int C, int k,
+                                                         int stride, int pad, int Ho, int Wo, int K, int Kp,
+                                                         __nv_bfloat16* __restrict__ out) {
+  const int chunks = Kp / 8;
+  const int64_t total = static_cast<int64_t>(B) * Ho * Wo * chunks;
+  for (int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+       t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int ch = static_cast<int>(t % chunks);
+    const int64_t m = t / chunks;
+    const int wo = static_cast<int>(m % Wo);
+    const int ho = static_cast<int>((m / Wo) % Ho);
+    const int b = static_cast<int>(m / (static_cast<int64_t>(Wo) * Ho));
+    float v[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int e = ch * 8 + i;
+      v[i] = 0.f;
+      if (e < K) {
+        const int tap = e / C, c = e - tap * C;
+        const int dy = tap / k, dx = tap - dy * k;
+        const int ih = ho * stride - pad + dy, iw = wo * stride - pad + dx;
+        if (ih >= 0 && ih < H && iw >= 0 && iw < W) {
+          const int64_t idx = kNCHW ? ((static_cast<int64_t>(b) * C + c) * H + ih) * W + iw
+                                    : ((static_cast<int64_t>(b) * H + ih) * W + iw) * C + c;
+          v[i] = static_cast<float>(x[idx]);
+        }
+      }
+    }
+    uint4 o;
+    uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
+      ow[i] = *reinterpret_cast<uint32_t*>(&h);
+    }
+    *reinterpret_cast<uint4*>(out + m * Kp + ch * 8) = o;
+  }
+}
+
+// MaxPool2d(kernel 3, stride 2, padding 1) over NHWC bf16 (padding never wins: it is -inf); one thread = 8 channels of one
+// output pixel.  Exact (a max of bf16 values is one of them).
+__global__ void __launch_bounds__(256) maxpool3s2_kernel(const __nv_bfloat16* __restrict__ x, int B, int H, int W, int C,
+                                                         int Ho, int Wo, __nv_bfloat16* __restrict__ y) {
+  const int cc = C / 8;
+  const int64_t total = static_cast<int64_t>(B) * Ho * Wo * cc;
+  for (int64_t t = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+       t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int c8 = static_cast<int>(t % cc);
+    const int64_t m = t / cc;
+    const int wo = static_cast<int>(m % Wo);
+    const int ho = static_cast<int>((m / Wo) % Ho);
+    const int b = static_cast<int>(m / (static_cast<int64_t>(Wo) * Ho));
+    float mx[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) mx[i] = -INFINITY;
+    for (int dy = 0; dy < 3; ++dy) {
+      const int ih = ho * 2 - 1 + dy;
+      if (ih < 0 || ih >= H) continue;
+      for (int dx = 0; dx < 3; ++dx) {
+        const int iw = wo * 2 - 1 + dx;
+        if (iw < 0 || iw >= W) continue;
+        const uint4 u = *reinterpret_cast<const uint4*>(x + ((static_cast<int64_t>(b) * H + ih) * W + iw) * C + c8 * 8);
+        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 f = __bfloat1622float2(h[i]);
+          mx[2 * i] = fmaxf(mx[2 * i], f.x);
+          mx[2 * i + 1] = fmaxf(mx[2 * i + 1], f.y);
+        }
+      }
+    }
+    uint4 o;
+    uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      __nv_bfloat162 h = __floats2bfloat162_rn(mx[2 * i], mx[2 * i + 1]);
+      ow[i] = *reinterpret_cast<uint32_t*>(&h);
+    }
+    *reinterpret_cast<uint4*>(y + m * C + c8 * 8) = o;
+  }
+}
+
+static size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
+
+static int grid_for(int64_t threads) { return static_cast<int>(std::min<int64_t>((threads + 255) / 256, 132 * 16)); }
+
+static int check_net(const vdk_resnet_net* n) {
+  VDK_REQUIRE(n, "vdk_resnet: null network");
+  // every map a stride-2 layer reads then has an even side: AvgPool2d(2, 2, ceil_mode=True) never sees a partial window
+  VDK_REQUIRE(n->image_size > 0 && n->image_size % 32 == 0, "vdk_resnet: image_size must be a multiple of 32 (got %d)",
+              n->image_size);
+  VDK_REQUIRE(n->feat_dim > 0 && n->feat_dim % 8 == 0, "vdk_resnet: feat_dim must be a multiple of 8");
+  VDK_REQUIRE(n->base_width == 64 || n->base_width == 128, "vdk_resnet: base_width must be 64 or 128 (got %d)", n->base_width);
+  int nb = 0;
+  for (int s = 0; s < 4; ++s) {
+    VDK_REQUIRE(n->depths[s] >= 1, "vdk_resnet: every stage needs at least one block");
+    nb += n->depths[s];
+  }
+  VDK_REQUIRE(nb <= VDK_RESNET_MAX_BLOCKS, "vdk_resnet: too many blocks (%d)", nb);
+  for (int i = 0; i < (n->deep_stem ? 3 : 1); ++i) VDK_REQUIRE(n->stem[i].w && n->stem[i].b, "vdk_resnet: missing stem weights");
+  for (int i = 0; i < nb; ++i) {
+    const vdk_resnet_block& b = n->blocks[i];
+    VDK_REQUIRE(b.conv1.w && b.conv1.b && b.conv2.w && b.conv2.b && b.conv3.w && b.conv3.b, "vdk_resnet: block %d misses a conv", i);
+  }
+  int first = 0;
+  for (int s = 0; s < 4; ++s) {
+    VDK_REQUIRE(n->blocks[first].down.w && n->blocks[first].down.b, "vdk_resnet: the first block of stage %d needs its shortcut conv", s);
+    first += n->depths[s];
+  }
+  VDK_REQUIRE(n->neck_w && n->neck_b, "vdk_resnet: missing neck");
+  return VDK_OK;
+}
+
+struct ResnetSizes {
+  size_t act;   // elements of the largest activation map
+  size_t rows;  // elements of the stem's patch rows
+};
+
+static ResnetSizes resnet_sizes(const vdk_resnet_net* n, int batch) {
+  const size_t S = n->image_size, B = batch;
+  ResnetSizes z;
+  z.act = B * (S / 2) * (S / 2) * 64;  // stem output (the deep stem's 32-channel maps are smaller)
+  size_t hin = S / 4;
+  for (int s = 0; s < 4; ++s) {
+    const size_t width = static_cast<size_t>(n->base_width) << s, out = static_cast<size_t>(256) << s;
+    const size_t ho = s == 0 ? hin : hin / 2;
+    z.act = std::max(z.act, B * hin * hin * width);  // conv1 of the first block runs at the input resolution
+    z.act = std::max(z.act, B * ho * ho * out);
+    hin = ho;
+  }
+  z.rows = B * (S / 2) * (S / 2) * (n->deep_stem ? 320 : 192);
+  return z;
+}
+
+}  // namespace vdk
+
+using namespace vdk;
+
+extern "C" size_t vdk_resnet_workspace_bytes(const vdk_resnet_net* net, int batch) {
+  if (!net || batch <= 0 || net->image_size <= 0 || net->base_width <= 0) return 0;
+  const ResnetSizes z = resnet_sizes(net, batch);
+  // x (block input / output), shortcut, t1 (conv1 out, neck slabs), t2 (conv2 out), stem patch rows
+  return 4 * up256(z.act * 2) + up256(z.rows * 2) + 1024;
+}
+
+extern "C" int vdk_resnet_forward(const vdk_resnet_net* net, const float* images, int batch, int l2_normalize,
+                                  float* embeddings, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_net(net);
+  if (rc != VDK_OK) return rc;
+  VDK_REQUIRE(images && embeddings && batch > 0, "vdk_resnet_forward: null image/embedding buffer");
+  VDK_REQUIRE(workspace && workspace_bytes >= vdk_resnet_workspace_bytes(net, batch), "vdk_resnet_forward: workspace too small");
+  VDK_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "vdk_resnet_forward: workspace must be 256-byte aligned");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const ResnetSizes z = resnet_sizes(net, batch);
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  __nv_bfloat16* buf[4];
+  for (int i = 0; i < 4; ++i) {
+    buf[i] = reinterpret_cast<__nv_bfloat16*>(ws);
+    ws += up256(z.act * 2);
+  }
+  __nv_bfloat16* rows = reinterpret_cast<__nv_bfloat16*>(ws);
+  __nv_bfloat16 *x = buf[0], *sc = buf[1], *t1 = buf[2], *t2 = buf[3];
+
+  auto conv = [&](const void* in, int H, int W, int Cin, const vdk_resnet_conv& c, int Cout, int k, int stride, int pad,
+                  int epi, const void* res, void* out) -> int {
+    vdk_conv_desc d{};
+    d.x = in; d.w = c.w; d.bias = c.b; d.residual = res; d.y = out;
+    d.B = batch; d.H = H; d.W = W; d.Cin = Cin; d.Cout = Cout;
+    d.kernel = k; d.stride = stride; d.pad = pad; d.epilogue = epi;
+    return conv_run(d, s);
+  };
+  // stem convolution over explicit patch rows: a 1x1 conv (plain GEMM) over [B, Ho, Wo, Kp] + bias + ReLU
+  auto stem_conv = [&](auto* in, bool nchw, int H, int C, int k, int stride, const vdk_resnet_conv& c, int Cout, void* out) -> int {
+    const int pad = k / 2, Ho = (H + 2 * pad - k) / stride + 1;
+    const int K = k * k * C, Kp = (K + 63) / 64 * 64;
+    const int64_t threads = static_cast<int64_t>(batch) * Ho * Ho * (Kp / 8);
+    using T = std::remove_cv_t<std::remove_pointer_t<decltype(in)>>;
+    if (nchw) patch_rows_kernel<T, true><<<grid_for(threads), 256, 0, s>>>(in, batch, H, H, C, k, stride, pad, Ho, Ho, K, Kp, rows);
+    else patch_rows_kernel<T, false><<<grid_for(threads), 256, 0, s>>>(in, batch, H, H, C, k, stride, pad, Ho, Ho, K, Kp, rows);
+    VDK_CUDA_OK(cudaGetLastError());
+    return conv(rows, Ho, Ho, Kp, c, Cout, 1, 1, 0, VDK_EPI_RELU, nullptr, out);
+  };
+
+  const int S = net->image_size;
+  int H = S / 2;
+  // ---- stem: conv 7x7/s2 + bn1 + ReLU, or the deep stem's three 3x3 convs (each + BN + ReLU) ----
+  if (net->deep_stem) {
+    if ((rc = stem_conv(images, true, S, 3, 3, 2, net->stem[0], 32, t1)) != VDK_OK) return rc;
+    if ((rc = stem_conv(static_cast<const __nv_bfloat16*>(t1), false, H, 32, 3, 1, net->stem[1], 32, t2)) != VDK_OK) return rc;
+    if ((rc = stem_conv(static_cast<const __nv_bfloat16*>(t2), false, H, 32, 3, 1, net->stem[2], 64, sc)) != VDK_OK) return rc;
+  } else {
+    if ((rc = stem_conv(images, true, S, 3, 7, 2, net->stem[0], 64, sc)) != VDK_OK) return rc;
+  }
+  // ---- max pool 3x3/s2 ----
+  {
+    const int Ho = H / 2;
+    maxpool3s2_kernel<<<grid_for(static_cast<int64_t>(batch) * Ho * Ho * 8), 256, 0, s>>>(sc, batch, H, H, 64, Ho, Ho, x);
+    VDK_CUDA_OK(cudaGetLastError());
+    H = Ho;
+  }
+  // ---- stages of Bottleneck blocks: conv1 1x1 + ReLU, conv2 3x3/stride + ReLU, conv3 1x1 + shortcut + ReLU ----
+  int C = 64, blk = 0;
+  for (int st = 0; st < 4; ++st) {
+    const int width = net->base_width << st, out = 256 << st;
+    for (int j = 0; j < net->depths[st]; ++j, ++blk) {
+      const vdk_resnet_block& b = net->blocks[blk];
+      const int stride = (st > 0 && j == 0) ? 2 : 1, Ho = H / stride;
+      if ((rc = conv(x, H, H, C, b.conv1, width, 1, 1, 0, VDK_EPI_RELU, nullptr, t1)) != VDK_OK) return rc;
+      if ((rc = conv(t1, H, H, width, b.conv2, width, 3, stride, 1, VDK_EPI_RELU, nullptr, t2)) != VDK_OK) return rc;
+      __nv_bfloat16* res = x;
+      if (b.down.w) {
+        // shortcut: 1x1/stride conv, or (avg_down, stride 2) AvgPool2d(2, 2) + 1x1 conv folded into one 2x2/s2 conv
+        const int k = (net->avg_down && stride == 2) ? 2 : 1;
+        if ((rc = conv(x, H, H, C, b.down, out, k, stride, 0, VDK_EPI_NONE, nullptr, sc)) != VDK_OK) return rc;
+        res = sc;
+      }
+      if ((rc = conv(t2, Ho, Ho, width, b.conv3, out, 1, 1, 0, VDK_EPI_RESIDUAL_RELU, res, res)) != VDK_OK) return rc;
+      if (res == sc) std::swap(x, sc);
+      H = Ho;
+      C = out;
+    }
+  }
+  // ---- neck: BN2d -> Flatten -> Linear -> BN1d folded into one split-K GEMM over the (h, w, c) features ----
+  return launch_neck(x, batch, H * H * C, net->feat_dim, net->neck_w, net->neck_b, l2_normalize, reinterpret_cast<float*>(t1),
+                     up256(z.act * 2), embeddings, s);
+}

@@ -43,6 +43,42 @@ static EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
+// cuTensorMapEncodeIm2col, resolved the same way
+using EncodeIm2colFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                    const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static EncodeIm2colFn encode_im2col_fn() {
+  static EncodeIm2colFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeIm2colFn>(p);
+  });
+  return fn;
+}
+
+int make_tma_im2col_16bit(CUtensorMap* map, const void* base, int B, int H, int W, int C, int kernel, int stride, int pad) {
+  EncodeIm2colFn fn = encode_im2col_fn();
+  if (!fn) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeIm2col entry point unavailable (no CUDA driver?)");
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || C % 64 != 0)
+    return fail(VDK_ERR_INVALID, "im2col TMA operand must be 16-byte aligned with C a multiple of 64 (C=%d)", C);
+  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  cuuint64_t gstride[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  // window origins run from -pad to (size - 1) + pad - (kernel - 1) in steps of `stride`: exactly the output positions
+  const int lower[2] = {-pad, -pad};
+  const int upper[2] = {pad - (kernel - 1), pad - (kernel - 1)};
+  cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), gdim, gstride, lower, upper, 64, 128, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeIm2col failed with CUresult %d", (int)r);
+  return VDK_OK;
+}
+
 int make_tma_2d_16bit(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
                       uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn fn = encode_tiled_fn();
@@ -166,6 +202,14 @@ int vdk_version(void) { return 100; }  // 0.1.0
 int vdk_struct_sizes(size_t* out, int n) {
   const size_t sizes[] = {sizeof(vdk_gemm_desc),        sizeof(vdk_topk_plan),  sizeof(vdk_head_desc), sizeof(vdk_convnext_net),
                           sizeof(vdk_convnext_tensors), sizeof(vdk_vit_net),   sizeof(vdk_vit_tensors)};
+  const int k = static_cast<int>(sizeof(sizes) / sizeof(sizes[0]));
+  for (int i = 0; i < n && i < k; ++i) out[i] = sizes[i];
+  return k;
+}
+
+// the same for the structs of the ResNet surface: vdk_conv_desc, vdk_resnet_net
+int vdk_resnet_struct_sizes(size_t* out, int n) {
+  const size_t sizes[] = {sizeof(vdk_conv_desc), sizeof(vdk_resnet_net)};
   const int k = static_cast<int>(sizeof(sizes) / sizeof(sizes[0]));
   for (int i = 0; i < n && i < k; ++i) out[i] = sizes[i];
   return k;

@@ -38,6 +38,11 @@ int make_tma_2d_16bit(CUtensorMap* map, const void* base, uint64_t rows, uint64_
 // (which is exactly the zero padding of a convolution).
 int make_tma_nhwc_16bit(CUtensorMap* map, const void* base, int B, int H, int W, int C, int box_h, int box_w, int box_c);
 
+// im2col map over an NHWC 16-bit tensor (C a multiple of 64) for a square kernel x kernel convolution with the given stride
+// and zero padding: one load = 128 consecutive output pixels (row-major over (b, ho, wo), crossing rows and images) x 64
+// channels of one filter tap, 128-byte swizzle — the K-major A stage of the GEMM.  Taps outside the image read as zero.
+int make_tma_im2col_16bit(CUtensorMap* map, const void* base, int B, int H, int W, int C, int kernel, int stride, int pad);
+
 // 4-D map over the qkv Linear's output, 16-bit [B][N][3H][D] (D contiguous), seen as (D, 3H, N, B): box = [1][box_rows][1]
 // [box_cols], box_cols 64 with 128-byte swizzle or 16 with 32-byte swizzle; out-of-bounds rows (past N) and columns (past D)
 // read as zero.  The attention kernel's view of its input.
@@ -68,4 +73,6 @@ struct ProfScope {
 namespace vdk {
 // Internal form of vdk_gemm used by the composite entry points (convnext forward, heads).
 int gemm_run(const vdk_gemm_desc& g, cudaStream_t stream);
+// Internal form of vdk_conv2d (the ResNet forward).
+int conv_run(const vdk_conv_desc& c, cudaStream_t stream);
 }  // namespace vdk

@@ -122,6 +122,20 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// im2col-mode load over an NHWC map (cuTensorMapEncodeIm2col): pixelsPerColumn pixels x channelsPerPixel channels starting
+// at channel c, pixel (n, h, w) — the map's bounding box walked in W, H, N order with its element strides — each pixel
+// shifted by the filter tap (off_w, off_h); positions outside the tensor read as zero
+__device__ __forceinline__ void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h,
+                                                   int n, uint16_t off_w, uint16_t off_h, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8}, %9;"
+      ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h),
+      "l"(policy)
+      : "memory");
+}
+
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
                                             int c2, int c3) {
   asm volatile(

@@ -1,0 +1,236 @@
+"""ResNet backbones of the faceX / CBIR extract path on H100 (timm 0.9.16 Bottleneck ResNets).
+
+`ResNetWrapper` is the reference's TimmWrapper for a `timm-resnet*` / `timm-wide_resnet*` backbone
+(models/faceX/backbone/timm_wrapper.py:16-54): the timm ResNet built with num_classes=0, global_pool='' under `model.`
+and the CNN neck `output_layer.{0: BatchNorm2d, 1: Flatten, 2: Linear, 3: BatchNorm1d}`; parameter names and shapes are
+timm's, so timm checkpoints load with strict=True.  The arithmetic is csrc/resnet.cu (vdk_resnet_forward): every eval
+BatchNorm folded into its convolution, the convolutions on the wgmma GEMM (implicit GEMM with TMA im2col tiles).
+Extraction only: a train-mode forward raises NotImplementedError.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+import os
+import warnings
+from typing import Dict, Optional
+
+import torch
+import torch.nn as nn
+
+from . import _lib
+
+# timm 0.9.16 resnet.py model_args; all Bottleneck (stride on the 3x3 conv, expansion 4)
+RESNET_ARCHS = {
+    "resnet50": dict(depths=(3, 4, 6, 3)),
+    "resnet101": dict(depths=(3, 4, 23, 3)),
+    "resnet152": dict(depths=(3, 8, 36, 3)),
+    "resnet50d": dict(depths=(3, 4, 6, 3), stem_width=32, stem_type="deep", avg_down=True),
+    "resnet101d": dict(depths=(3, 4, 23, 3), stem_width=32, stem_type="deep", avg_down=True),
+    "resnet152d": dict(depths=(3, 8, 36, 3), stem_width=32, stem_type="deep", avg_down=True),
+    "wide_resnet50_2": dict(depths=(3, 4, 6, 3), base_width=128),
+    "wide_resnet101_2": dict(depths=(3, 4, 23, 3), base_width=128),
+}
+
+
+class _Bottleneck(nn.Module):
+    def __init__(self, inplanes, planes, stride, downsample, base_width):
+        super().__init__()
+        width = int(math.floor(planes * (base_width / 64)))
+        self.stride = stride
+        self.conv1 = nn.Conv2d(inplanes, width, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(width)
+        self.conv2 = nn.Conv2d(width, width, 3, stride=stride, padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(width)
+        self.conv3 = nn.Conv2d(width, planes * 4, 1, bias=False)
+        self.bn3 = nn.BatchNorm2d(planes * 4)
+        self.downsample = downsample
+
+
+class ResNetParams(nn.Module):
+    """timm 0.9.16 `ResNet(Bottleneck, ..., num_classes=0, global_pool='')` parameter tree.  Parameter containers only:
+    their forward() is never used (the forward is vdk_resnet_forward)."""
+
+    def __init__(self, depths, base_width=64, stem_width=64, stem_type="", avg_down=False):
+        super().__init__()
+        self.depths, self.base_width, self.avg_down = tuple(depths), int(base_width), bool(avg_down)
+        self.deep_stem = "deep" in stem_type
+        inplanes = stem_width * 2 if self.deep_stem else 64
+        if self.deep_stem:
+            self.conv1 = nn.Sequential(
+                nn.Conv2d(3, stem_width, 3, stride=2, padding=1, bias=False), nn.BatchNorm2d(stem_width), nn.ReLU(),
+                nn.Conv2d(stem_width, stem_width, 3, padding=1, bias=False), nn.BatchNorm2d(stem_width), nn.ReLU(),
+                nn.Conv2d(stem_width, inplanes, 3, padding=1, bias=False))
+        else:
+            self.conv1 = nn.Conv2d(3, inplanes, 7, stride=2, padding=3, bias=False)
+        self.bn1 = nn.BatchNorm2d(inplanes)
+        for i, (planes, depth) in enumerate(zip((64, 128, 256, 512), depths)):
+            stride, blocks = (1 if i == 0 else 2), []
+            for j in range(depth):
+                down = None
+                if j == 0 and (stride != 1 or inplanes != planes * 4):
+                    conv, bn = nn.Conv2d(inplanes, planes * 4, 1, stride=1 if avg_down else stride, bias=False), nn.BatchNorm2d(planes * 4)
+                    if avg_down:
+                        pool = nn.AvgPool2d(2, stride, ceil_mode=True, count_include_pad=False) if stride != 1 else nn.Identity()
+                        down = nn.Sequential(pool, conv, bn)
+                    else:
+                        down = nn.Sequential(conv, bn)
+                blocks.append(_Bottleneck(inplanes, planes, stride if j == 0 else 1, down, base_width))
+                inplanes = planes * 4
+            setattr(self, f"layer{i + 1}", nn.Sequential(*blocks))
+        # timm's init: kaiming_normal(fan_out, relu) convs, unit BatchNorms, bn3.weight zeroed (zero_init_last)
+        for m in self.modules():
+            if isinstance(m, nn.Conv2d):
+                nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
+        for blk in self.blocks():
+            nn.init.zeros_(blk.bn3.weight)
+
+    def blocks(self):
+        return [b for i in range(4) for b in getattr(self, f"layer{i + 1}")]
+
+
+class _ConvC(C.Structure):
+    _fields_ = [("w", C.c_void_p), ("b", C.c_void_p)]
+
+
+class _ResBlockC(C.Structure):
+    _fields_ = [("conv1", _ConvC), ("conv2", _ConvC), ("conv3", _ConvC), ("down", _ConvC)]
+
+
+class ResNetNetC(C.Structure):
+    """vdk_resnet_net (include/vdk_b200.h)."""
+    _fields_ = [
+        ("image_size", C.c_int), ("feat_dim", C.c_int), ("depths", C.c_int * 4), ("base_width", C.c_int),
+        ("deep_stem", C.c_int), ("avg_down", C.c_int), ("stem", _ConvC * 3), ("blocks", _ResBlockC * 64),
+        ("neck_w", C.c_void_p), ("neck_b", C.c_void_p),
+    ]
+
+
+def fold_bn(conv: nn.Conv2d, bn: nn.BatchNorm2d):
+    """Eval BatchNorm folded into the bias-free conv before it, in fp32: w * g / sqrt(var + eps), b - mean * g / sqrt(var + eps)."""
+    s = bn.weight.detach().float() / torch.sqrt(bn.running_var.detach().float() + bn.eps)
+    w = conv.weight.detach().float() * s.view(-1, 1, 1, 1)
+    return w, bn.bias.detach().float() - bn.running_mean.detach().float() * s
+
+
+class ResNetWrapper(nn.Module):
+    """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm ResNet backbone (eval / extract only)."""
+
+    def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, **kwargs):
+        super().__init__()
+        if model_name not in RESNET_ARCHS:
+            raise ValueError(f"backbone '{model_name}' is not built for H100 yet; ResNets available: {sorted(RESNET_ARCHS)}")
+        if image_size % 32 != 0:
+            raise ValueError("image_size must be a multiple of 32")
+        args = dict(RESNET_ARCHS[model_name])
+        if depths is not None:
+            args["depths"] = tuple(depths)
+        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
+        self.model = ResNetParams(**args)
+        hw = image_size // 32
+        self.output_layer = nn.Sequential(nn.BatchNorm2d(2048), nn.Flatten(1), nn.Linear(2048 * hw * hw, feat_dim),
+                                          nn.BatchNorm1d(feat_dim))
+        self._packed: Optional[Dict] = None
+        self._packed_key = None
+        self._ws = None
+        if pretrained:
+            self._load_pretrained(model_name)
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if self.training:
+            raise NotImplementedError(f"{self.model_name}: ResNet backbones are extraction-only on H100 (call .eval() first)")
+        return self.embed(x, l2_normalize=False)
+
+    @torch.no_grad()
+    def embed(self, x: torch.Tensor, l2_normalize: bool = False) -> torch.Tensor:
+        """[B,3,S,S] fp32 NCHW -> fp32 [B, feat_dim] (TimmWrapper.forward in eval mode; optionally F.normalize fused)."""
+        lib = _lib.load()
+        if x.device.type != "cuda":
+            raise RuntimeError("visiondk_b200.ResNetWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
+        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
+            raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
+        x = x.contiguous().float()
+        net = self._pack(x.device)
+        B = x.shape[0]
+        out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
+        need = lib.vdk_resnet_workspace_bytes(C.byref(net), B)
+        if need == 0:
+            raise RuntimeError("vdk_resnet_workspace_bytes: invalid network")
+        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
+            self._ws = torch.empty((need,), dtype=torch.uint8, device=x.device)
+        with torch.cuda.device(x.device):
+            _lib.check(lib.vdk_resnet_forward(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(), self._ws.data_ptr(),
+                                              self._ws.numel(), _lib.stream_ptr()), "vdk_resnet_forward")
+        return out
+
+    def _version_key(self, device):
+        return (str(device),) + tuple(int(t._version) for t in list(self.parameters()) + list(self.buffers()))
+
+    def _pack(self, device) -> ResNetNetC:
+        """Kernel-side layouts (include/vdk_b200.h): BatchNorms folded once per weight version, bf16 conv weights
+        [Cout, kh, kw, Cin], stem weights as zero-padded (kh, kw, c) patch rows, the folded neck in (h, w, c) order."""
+        key = self._version_key(device)
+        if self._packed is not None and self._packed_key == key:
+            return self._packed["net"]
+        from .backbone import fold_cnn_neck
+        keep = []
+
+        def f32(t):
+            t = t.detach().to(device, torch.float32).contiguous()
+            keep.append(t)
+            return t.data_ptr()
+
+        def bf16(t):
+            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
+            keep.append(t)
+            return t.data_ptr()
+
+        def conv(dst, w, b, pool2=False):
+            w = w.permute(0, 2, 3, 1)  # [Cout, kh, kw, Cin]
+            if pool2:  # AvgPool2d(2, 2) then the 1x1 conv == a 2x2/s2 conv with w / 4 at every tap
+                w = w.expand(-1, 2, 2, -1) / 4
+            dst.w, dst.b = bf16(w), f32(b)
+
+        def stem(dst, w, b):
+            k = w[0].numel()
+            rows = w.permute(0, 2, 3, 1).reshape(w.shape[0], k)
+            kp = (k + 63) // 64 * 64
+            dst.w, dst.b = bf16(torch.cat([rows, rows.new_zeros(w.shape[0], kp - k)], dim=1)), f32(b)
+
+        m, net = self.model, ResNetNetC()
+        net.image_size, net.feat_dim = self.image_size, self.feat_dim
+        for i in range(4):
+            net.depths[i] = m.depths[i]
+        net.base_width, net.deep_stem, net.avg_down = m.base_width, int(m.deep_stem), int(m.avg_down)
+        if m.deep_stem:
+            stem(net.stem[0], *fold_bn(m.conv1[0], m.conv1[1]))
+            stem(net.stem[1], *fold_bn(m.conv1[3], m.conv1[4]))
+            stem(net.stem[2], *fold_bn(m.conv1[6], m.bn1))
+        else:
+            stem(net.stem[0], *fold_bn(m.conv1, m.bn1))
+        for i, blk in enumerate(m.blocks()):
+            b = net.blocks[i]
+            conv(b.conv1, *fold_bn(blk.conv1, blk.bn1))
+            conv(b.conv2, *fold_bn(blk.conv2, blk.bn2))
+            conv(b.conv3, *fold_bn(blk.conv3, blk.bn3))
+            if blk.downsample is not None:
+                if m.avg_down:
+                    conv(b.down, *fold_bn(blk.downsample[1], blk.downsample[2]), pool2=blk.stride == 2)
+                else:
+                    conv(b.down, *fold_bn(blk.downsample[0], blk.downsample[1]))
+        w, bias = fold_cnn_neck(self.output_layer, 2048, self.image_size // 32, self.feat_dim, device)
+        net.neck_w, net.neck_b = bf16(w), f32(bias)
+        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+        return net
+
+    def _load_pretrained(self, model_name: str) -> None:
+        """Like TimmWrapper._load_pretrained: a timm state_dict from $VDK_PRETRAINED_DIR/<model_name>.pth (no network here);
+        the classifier (fc.*) is dropped, as num_classes=0 does."""
+        root = os.environ.get("VDK_PRETRAINED_DIR")
+        path = os.path.join(root, f"{model_name}.pth") if root else None
+        if path and os.path.exists(path):
+            sd = torch.load(path, map_location="cpu")
+            sd = {k: v for k, v in sd.items() if not k.startswith("fc.")}
+            self.model.load_state_dict(sd, strict=True)
+        else:
+            warnings.warn(f"pretrained weights for '{model_name}' not found (set VDK_PRETRAINED_DIR); using random init")
