@@ -109,6 +109,14 @@ typedef struct vdk_conv_desc {
 } vdk_conv_desc;
 /* Cin a multiple of 64, Cout a multiple of 8, 1 <= kernel <= 16, 1 <= stride <= 8, 0 <= pad < kernel. */
 int vdk_conv2d(const vdk_conv_desc* desc, void* stream);
+/* Grouped form (`groups` groups of cg = Cin / groups channels): the 3x3 conv of timm's ResNeXt Bottleneck
+ * (timm/models/resnet.py, cardinality > 1) and of the legacy SE-ResNeXt (timm/models/senet.py).  Each 128-channel output
+ * tile contracts over the 128 input channels of its own groups, so desc->w is the block-diagonal weight [Cout, kernel,
+ * kernel, 128]: output channel n of group g = n / cg in tile t = n / 128 holds timm's w[n, j - g cg + 128 t] at tile
+ * channel j for j in group g, zero elsewhere.  K = kernel*kernel*128 are executed, 128 / cg times the useful MACs.
+ * Cin == Cout a multiple of 128, groups >= 2 with cg dividing 128, epilogue VDK_EPI_RELU (no residual); kernel, stride and
+ * pad as vdk_conv2d. */
+int vdk_conv2d_grouped(const vdk_conv_desc* desc, int groups, void* stream);
 
 /* ---- ResNet embedding forward (eval) --------------------------------------------------------- */
 /* Replaces TimmWrapper.forward for timm's Bottleneck ResNets (resnet50/101/152, their -D variants, wide_resnet50_2/101_2;
@@ -145,6 +153,54 @@ int vdk_resnet_forward(const vdk_resnet_net* net, const float* images, int batch
                        void* workspace, size_t workspace_bytes, void* stream);
 /* sizeof() of vdk_conv_desc and vdk_resnet_net, in that order (vdk_struct_sizes' contract for these two). */
 int vdk_resnet_struct_sizes(size_t* out, int n);
+
+/* ---- general Bottleneck network embedding forward (eval): ResNeXt, legacy SE-ResNet / SE-ResNeXt ---------------- */
+/* Replaces TimmWrapper.forward for timm's ResNeXt (resnext50_32x4d, resnext101_32x8d / 64x4d, resnext50d_32x4d;
+ * timm/models/resnet.py) and legacy SENet Bottleneck models (legacy_seresnet50/101/152, legacy_seresnext26/50/101_32x4d;
+ * timm/models/senet.py) — models/faceX/backbone/timm_wrapper.py:16-21, 30-38, 51-54 — followed by F.normalize
+ * (face_model.py:139).  Same layouts as vdk_resnet_net; a block's 3x3 conv is grouped when cardinality > 1, and a block
+ * with SE weights runs out = ReLU(conv3 * sigmoid(fc2(ReLU(fc1(mean_hw(conv3))))) + shortcut) (timm senet.py SEModule). */
+typedef struct vdk_bottleneck_block {
+  vdk_resnet_conv conv1, conv2, conv3, down; /* as vdk_resnet_block; conv2 with cardinality > 1: vdk_conv2d_grouped's
+                                                block-diagonal [width, 3, 3, 128] */
+  const float* se_fc1_w; /* fp32 [rd, C], C = 4 * planes, rd = C / se_reduction; NULL: no SE module */
+  const float* se_fc1_b; /* [rd] */
+  const float* se_fc2_w; /* [C, rd] */
+  const float* se_fc2_b; /* [C] */
+} vdk_bottleneck_block;
+#define VDK_STEM_POOL_PAD1 0 /* MaxPool2d(3, 2, padding=1) (timm ResNet) */
+#define VDK_STEM_POOL_CEIL 1 /* MaxPool2d(3, 2, ceil_mode=True), no padding (legacy SENet) */
+typedef struct vdk_bottleneck_net {
+  int image_size;      /* square input side, multiple of 32 */
+  int feat_dim;        /* embedding width, multiple of 8 */
+  int depths[4];
+  int width;           /* conv1 / conv2 width of stage 0, doubled per stage: 64 (ResNet, SE-ResNet), 128 (32x4d), 256 (32x8d,
+                          64x4d) */
+  int cardinality;     /* groups of the 3x3 conv: 1 dense, > 1 vdk_conv2d_grouped */
+  int stride_on_conv1; /* 1: a stride-2 block strides its 1x1 conv1 (legacy SEResNetBottleneck); 0: its 3x3 conv2 */
+  int stem_pool;       /* VDK_STEM_POOL_PAD1 or VDK_STEM_POOL_CEIL */
+  int deep_stem;       /* as vdk_resnet_net */
+  int avg_down;        /* as vdk_resnet_net */
+  int se_reduction;    /* rd = C / se_reduction for the blocks with SE weights (16 in the legacy SENets) */
+  vdk_resnet_conv stem[3];
+  vdk_bottleneck_block blocks[VDK_RESNET_MAX_BLOCKS]; /* stage-major */
+  const void* neck_w;  /* [feat_dim, h*w*2048] bf16, as vdk_resnet_net */
+  const float* neck_b; /* [feat_dim] */
+} vdk_bottleneck_net;
+size_t vdk_bottleneck_workspace_bytes(const vdk_bottleneck_net* net, int batch);
+/* images: fp32 NCHW [batch,3,S,S]; embeddings: fp32 [batch, feat_dim], L2-normalised when l2_normalize != 0. */
+int vdk_bottleneck_forward(const vdk_bottleneck_net* net, const float* images, int batch, int l2_normalize, float* embeddings,
+                           void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_bottleneck_net. */
+int vdk_bottleneck_struct_sizes(size_t* out, int n);
+/* The forward's stem pool alone: MaxPool2d(3, 2) over NHWC bf16 [B, H, W, C] (C a multiple of 8) with mode
+ * VDK_STEM_POOL_PAD1 (padding 1) or VDK_STEM_POOL_CEIL (ceil_mode=True, no padding) into y [B, Ho, Wo, C]. */
+int vdk_stem_maxpool(const void* x, int B, int H, int W, int C, int mode, void* y, void* stream);
+/* The forward's SE gate alone, on y = the BN-folded conv3 output [B, HW, C] bf16 (C a multiple of 64, <= 2048):
+ * mean [B, C] fp32 = the spatial mean, gate [B, C] fp32 = sigmoid(fc2_w ReLU(fc1_w mean + fc1_b) + fc2_b) (fc1_w [rd, C],
+ * fc2_w [C, rd]), then residual [B, HW, C] bf16 = ReLU(y * gate + residual) in place. */
+int vdk_se_gate(const void* y, int B, int HW, int C, int rd, const float* fc1_w, const float* fc1_b, const float* fc2_w,
+                const float* fc2_b, float* mean, float* gate, void* residual, void* stream);
 
 /* ---- ConvNeXt embedding forward (eval) ------------------------------------------------------ */
 /* Replaces TimmWrapper.forward (models/faceX/backbone/timm_wrapper.py:51-54: timm ConvNeXt features with

@@ -89,6 +89,12 @@ SIGNATURES = {
     "vdk_resnet_workspace_bytes": (_sz, [_p, _i]),
     "vdk_resnet_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
     "vdk_resnet_struct_sizes": (_i, [_p, _i]),
+    "vdk_conv2d_grouped": (_i, [_p, _i, _p]),
+    "vdk_bottleneck_workspace_bytes": (_sz, [_p, _i]),
+    "vdk_bottleneck_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
+    "vdk_bottleneck_struct_sizes": (_i, [_p, _i]),
+    "vdk_stem_maxpool": (_i, [_p, _i, _i, _i, _i, _i, _p, _p]),
+    "vdk_se_gate": (_i, [_p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "vdk_dwconv7_ln": (_i, [_p, _i, _i, _i, _i, _p, _p, _p, _p, C.c_float, _p, _p]),
     "vdk_layernorm_patchify": (_i, [_p, _i, _i, _i, _i, _p, _p, C.c_float, _i, _p, _p]),
     "vdk_dwconv7": (_i, [_i, _p, _i, _i, _i, _i, _p, _p, _p, _p, C.c_float, _p, _p, _p, _p]),

@@ -465,7 +465,10 @@ class BackboneFactory:
         if model_name.startswith("vit_"):  # Transformer backbones: eval / extract path (visiondk_b200/vit.py)
             from .vit import ViTWrapper
             return ViTWrapper(model_name=model_name, **self.backbone_param)
-        from .resnet import RESNET_ARCHS, ResNetWrapper
-        if model_name in RESNET_ARCHS:  # Bottleneck ResNets: eval / extract path (visiondk_b200/resnet.py)
-            return ResNetWrapper(model_name=model_name, **self.backbone_param)
+        from .resnet import RESNET_ARCHS, RESNEXT_ARCHS, ResNetWrapper
+        if model_name in RESNET_ARCHS or model_name in RESNEXT_ARCHS:  # Bottleneck ResNets / ResNeXts: eval / extract path
+            return ResNetWrapper(model_name=model_name, **self.backbone_param)  # (visiondk_b200/resnet.py)
+        from .senet import SENET_ARCHS, SENetWrapper
+        if model_name in SENET_ARCHS:  # legacy SE-ResNets / SE-ResNeXts: eval / extract path (visiondk_b200/senet.py)
+            return SENetWrapper(model_name=model_name, **self.backbone_param)
         return TimmWrapper(model_name=model_name, **self.backbone_param)

@@ -29,6 +29,9 @@ constexpr int kBoxBytes = 64 * 128;  // epilogue box: one warpgroup's 64 rows x 
 constexpr int kGemmPlain = 0;
 constexpr int kConvDense = 1;   // 1x1 / stride-1 convolution: a plain GEMM over [B*H*W, Cin]
 constexpr int kConvIm2col = 2;  // k x k / stride-s convolution: A tiles gathered from NHWC by TMA im2col loads
+// grouped k x k convolution (vdk_conv2d_grouped, BN = 128): the N tile at n0 contracts over input channels n0 .. n0 + 127
+// only (whole groups, block-diagonal B), so its K block kb = (tap kb / 2, channels n0 + (kb % 2) * 64)
+constexpr int kConvGrouped = 3;
 
 // The implicit-GEMM convolution modes (kConvIm2col) overlay their geometry on fields they do not use, so that the struct —
 // and with it the code of the plain GEMM instantiations — stays as it is.
@@ -215,7 +218,7 @@ __device__ __forceinline__ void epi_publish(const CUtensorMap* map, const uint8_
 __device__ __forceinline__ uint32_t box_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
 
 // kTA / kTB: operand stored with the contraction index as the slow dimension ([K,M] / [K,N] row-major: MN-major)
-// kMode: kGemmPlain, kConvDense or kConvIm2col (see above)
+// kMode: kGemmPlain, kConvDense, kConvIm2col or kConvGrouped (see above)
 template <int BN, bool kBf16, int kTA, int kTB, int kMode>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
@@ -274,7 +277,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         // im2col: the tile's first output pixel, as the input position of its filter window's top-left tap.  The TMA unit
         // walks the next 127 pixels through the map's bounding box (across rows and images); rows past M read as zero.
         int cw = 0, ch = 0, cn = 0;
-        if constexpr (kMode == kConvIm2col) {
+        if constexpr (kMode == kConvIm2col || kMode == kConvGrouped) {
           cn = m0 / p.cv_howo;
           const int r = m0 - cn * p.cv_howo, ho = r / p.cv_wo;
           ch = ho * p.cv_stride - p.cv_pad;
@@ -287,6 +290,10 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
           if constexpr (kMode == kConvIm2col) {  // K block kb = (filter tap, 64-channel block)
             const int tap = kb / p.cv_cpb, c0 = (kb - tap * p.cv_cpb) * kBK, dy = tap / p.cv_kw;
+            tma_load_im2col_4d(sa, &map_a, &full_bar[stage], c0, cw, ch, cn, static_cast<uint16_t>(tap - dy * p.cv_kw),
+                               static_cast<uint16_t>(dy), kEvictNormal);
+          } else if constexpr (kMode == kConvGrouped) {  // cv_cpb = 2: the tile's own 128 input channels at every tap
+            const int tap = kb >> 1, c0 = n0 + (kb & 1) * kBK, dy = tap / p.cv_kw;
             tma_load_im2col_4d(sa, &map_a, &full_bar[stage], c0, cw, ch, cn, static_cast<uint16_t>(tap - dy * p.cv_kw),
                                static_cast<uint16_t>(dy), kEvictNormal);
           } else if (kTA) {  // [K,M] storage: 64-wide M blocks x 64 contraction rows, 8 KB each
@@ -725,11 +732,57 @@ int conv_run(const vdk_conv_desc& c, cudaStream_t s) {
   return wide ? launch_gemm<256, true, 0, 0, kConvIm2col>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvIm2col>(maps, p, s);
 }
 
+int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t s) {
+  VDK_REQUIRE(c.x && c.w && c.y, "vdk_conv2d_grouped: null operand");
+  VDK_REQUIRE(c.B > 0 && c.H > 0 && c.W > 0, "vdk_conv2d_grouped: empty input B=%d H=%d W=%d", c.B, c.H, c.W);
+  VDK_REQUIRE(c.Cin == c.Cout && c.Cin > 0 && c.Cin % 128 == 0,
+              "vdk_conv2d_grouped: Cin must equal Cout and be a positive multiple of 128 (Cin=%d Cout=%d)", c.Cin, c.Cout);
+  VDK_REQUIRE(groups >= 2 && c.Cin % groups == 0 && 128 % (c.Cin / groups) == 0,
+              "vdk_conv2d_grouped: groups=%d must be >= 2 with Cin / groups dividing 128 (Cin=%d)", groups, c.Cin);
+  VDK_REQUIRE(c.kernel >= 1 && c.kernel <= 16 && c.stride >= 1 && c.stride <= 8 && c.pad >= 0 && c.pad < c.kernel,
+              "vdk_conv2d_grouped: unsupported kernel=%d stride=%d pad=%d", c.kernel, c.stride, c.pad);
+  VDK_REQUIRE(c.H + 2 * c.pad >= c.kernel && c.W + 2 * c.pad >= c.kernel,
+              "vdk_conv2d_grouped: kernel larger than the padded input");
+  VDK_REQUIRE(c.epilogue == VDK_EPI_RELU && c.residual == nullptr,
+              "vdk_conv2d_grouped: epilogue must be RELU, without a residual (got %d)", c.epilogue);
+  VDK_REQUIRE((reinterpret_cast<uintptr_t>(c.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.w) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(c.y) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.bias) & 15) == 0,
+              "vdk_conv2d_grouped: operands must be 16-byte aligned");
+  const int Ho = (c.H + 2 * c.pad - c.kernel) / c.stride + 1, Wo = (c.W + 2 * c.pad - c.kernel) / c.stride + 1;
+  const long long M = static_cast<long long>(c.B) * Ho * Wo;
+  const long long K = static_cast<long long>(c.kernel) * c.kernel * 128;  // executed: each tile's 128 input channels
+  VDK_REQUIRE(M < (1ll << 31), "vdk_conv2d_grouped: problem too large (M=%lld)", M);
+  CUtensorMap maps[5];  // A, B, D, aux_out and residual (unused)
+  int rc = make_tma_im2col_16bit(&maps[0], c.x, c.B, c.H, c.W, c.Cin, c.kernel, c.stride, c.pad);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_2d_16bit(&maps[1], c.w, (uint64_t)c.Cout, (uint64_t)K, (uint64_t)K, 128, kBK);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_epilogue_map(&maps[2], c.y, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
+  if (rc != VDK_OK) return rc;
+  maps[3] = maps[2];
+  maps[4] = maps[2];
+  GemmParams p{};
+  p.M = static_cast<int>(M); p.N = c.Cout; p.K = static_cast<int>(K);
+  p.D = c.y; p.ldd = c.Cout; p.bias = c.bias; p.residual = nullptr; p.ldr = c.Cout;
+  p.out_dtype = VDK_DTYPE_BF16; p.epilogue = c.epilogue; p.split_k = 1;
+  p.cv_cpb = 2; p.cv_kw = c.kernel; p.cv_stride = c.stride; p.cv_pad = c.pad;
+  p.cv_wo = Wo; p.cv_howo = Ho * Wo;
+  // executed FLOPs (the block-diagonal K); the useful ones are a factor 128 / (Cin / groups) fewer
+  ProfScope prof(kProfGemm, 2.0 * M * c.Cout * K,
+                 2.0 * (static_cast<double>(c.B) * c.H * c.W * c.Cin + static_cast<double>(c.Cout) * K + M * c.Cout), s);
+  return launch_gemm<128, true, 0, 0, kConvGrouped>(maps, p, s);
+}
+
 }  // namespace vdk
 
 extern "C" int vdk_conv2d(const vdk_conv_desc* desc, void* stream) {
   VDK_REQUIRE(desc, "vdk_conv2d: null descriptor");
   return vdk::conv_run(*desc, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vdk_conv2d_grouped(const vdk_conv_desc* desc, int groups, void* stream) {
+  VDK_REQUIRE(desc, "vdk_conv2d_grouped: null descriptor");
+  return vdk::conv_grouped_run(*desc, groups, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vdk_gemm_effective_splits(int K, int split_k) {

@@ -75,4 +75,6 @@ namespace vdk {
 int gemm_run(const vdk_gemm_desc& g, cudaStream_t stream);
 // Internal form of vdk_conv2d (the ResNet forward).
 int conv_run(const vdk_conv_desc& c, cudaStream_t stream);
+// Internal form of vdk_conv2d_grouped (the ResNeXt / SE-ResNeXt forward).
+int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t stream);
 }  // namespace vdk

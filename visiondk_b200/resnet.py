@@ -1,10 +1,11 @@
-"""ResNet backbones of the faceX / CBIR extract path on H100 (timm 0.9.16 Bottleneck ResNets).
+"""ResNet backbones of the faceX / CBIR extract path on H100 (timm 0.9.16 Bottleneck ResNets and ResNeXts).
 
-`ResNetWrapper` is the reference's TimmWrapper for a `timm-resnet*` / `timm-wide_resnet*` backbone
+`ResNetWrapper` is the reference's TimmWrapper for a `timm-resnet*` / `timm-wide_resnet*` / `timm-resnext*` backbone
 (models/faceX/backbone/timm_wrapper.py:16-54): the timm ResNet built with num_classes=0, global_pool='' under `model.`
 and the CNN neck `output_layer.{0: BatchNorm2d, 1: Flatten, 2: Linear, 3: BatchNorm1d}`; parameter names and shapes are
 timm's, so timm checkpoints load with strict=True.  The arithmetic is csrc/resnet.cu (vdk_resnet_forward): every eval
-BatchNorm folded into its convolution, the convolutions on the wgmma GEMM (implicit GEMM with TMA im2col tiles).
+BatchNorm folded into its convolution, the convolutions on the wgmma GEMM (implicit GEMM with TMA im2col tiles).  ResNeXts
+run through vdk_bottleneck_forward, their grouped 3x3 convs on vdk_conv2d_grouped with block-diagonal weights.
 Extraction only: a train-mode forward raises NotImplementedError.
 """
 from __future__ import annotations
@@ -31,16 +32,23 @@ RESNET_ARCHS = {
     "wide_resnet50_2": dict(depths=(3, 4, 6, 3), base_width=128),
     "wide_resnet101_2": dict(depths=(3, 4, 23, 3), base_width=128),
 }
+# timm 0.9.16 resnet.py ResNeXt model_args: the 3x3 conv has `cardinality` groups of `base_width` * 2^stage channels
+RESNEXT_ARCHS = {
+    "resnext50_32x4d": dict(depths=(3, 4, 6, 3), cardinality=32, base_width=4),
+    "resnext50d_32x4d": dict(depths=(3, 4, 6, 3), cardinality=32, base_width=4, stem_width=32, stem_type="deep", avg_down=True),
+    "resnext101_32x8d": dict(depths=(3, 4, 23, 3), cardinality=32, base_width=8),
+    "resnext101_64x4d": dict(depths=(3, 4, 23, 3), cardinality=64, base_width=4),
+}
 
 
 class _Bottleneck(nn.Module):
-    def __init__(self, inplanes, planes, stride, downsample, base_width):
+    def __init__(self, inplanes, planes, stride, downsample, base_width, cardinality=1):
         super().__init__()
-        width = int(math.floor(planes * (base_width / 64)))
+        width = int(math.floor(planes * (base_width / 64)) * cardinality)
         self.stride = stride
         self.conv1 = nn.Conv2d(inplanes, width, 1, bias=False)
         self.bn1 = nn.BatchNorm2d(width)
-        self.conv2 = nn.Conv2d(width, width, 3, stride=stride, padding=1, bias=False)
+        self.conv2 = nn.Conv2d(width, width, 3, stride=stride, padding=1, groups=cardinality, bias=False)
         self.bn2 = nn.BatchNorm2d(width)
         self.conv3 = nn.Conv2d(width, planes * 4, 1, bias=False)
         self.bn3 = nn.BatchNorm2d(planes * 4)
@@ -51,9 +59,10 @@ class ResNetParams(nn.Module):
     """timm 0.9.16 `ResNet(Bottleneck, ..., num_classes=0, global_pool='')` parameter tree.  Parameter containers only:
     their forward() is never used (the forward is vdk_resnet_forward)."""
 
-    def __init__(self, depths, base_width=64, stem_width=64, stem_type="", avg_down=False):
+    def __init__(self, depths, base_width=64, stem_width=64, stem_type="", avg_down=False, cardinality=1):
         super().__init__()
         self.depths, self.base_width, self.avg_down = tuple(depths), int(base_width), bool(avg_down)
+        self.cardinality = int(cardinality)
         self.deep_stem = "deep" in stem_type
         inplanes = stem_width * 2 if self.deep_stem else 64
         if self.deep_stem:
@@ -75,7 +84,7 @@ class ResNetParams(nn.Module):
                         down = nn.Sequential(pool, conv, bn)
                     else:
                         down = nn.Sequential(conv, bn)
-                blocks.append(_Bottleneck(inplanes, planes, stride if j == 0 else 1, down, base_width))
+                blocks.append(_Bottleneck(inplanes, planes, stride if j == 0 else 1, down, base_width, cardinality))
                 inplanes = planes * 4
             setattr(self, f"layer{i + 1}", nn.Sequential(*blocks))
         # timm's init: kaiming_normal(fan_out, relu) convs, unit BatchNorms, bn3.weight zeroed (zero_init_last)
@@ -106,6 +115,36 @@ class ResNetNetC(C.Structure):
     ]
 
 
+class _BottleneckBlockC(C.Structure):
+    _fields_ = [("conv1", _ConvC), ("conv2", _ConvC), ("conv3", _ConvC), ("down", _ConvC),
+                ("se_fc1_w", C.c_void_p), ("se_fc1_b", C.c_void_p), ("se_fc2_w", C.c_void_p), ("se_fc2_b", C.c_void_p)]
+
+
+class BottleneckNetC(C.Structure):
+    """vdk_bottleneck_net (include/vdk_b200.h)."""
+    _fields_ = [
+        ("image_size", C.c_int), ("feat_dim", C.c_int), ("depths", C.c_int * 4), ("width", C.c_int), ("cardinality", C.c_int),
+        ("stride_on_conv1", C.c_int), ("stem_pool", C.c_int), ("deep_stem", C.c_int), ("avg_down", C.c_int),
+        ("se_reduction", C.c_int), ("stem", _ConvC * 3), ("blocks", _BottleneckBlockC * 64), ("neck_w", C.c_void_p),
+        ("neck_b", C.c_void_p),
+    ]
+
+
+STEM_POOL_PAD1, STEM_POOL_CEIL = 0, 1
+
+
+def pack_grouped(w: torch.Tensor) -> torch.Tensor:
+    """timm's grouped conv weight [Cout, Cout / groups, k, k] -> vdk_conv2d_grouped's block-diagonal [Cout, k, k, 128]:
+    output channel n of group g = n // cg sits in the 128-channel tile t = n // 128, and its cg input channels go to tile
+    columns g*cg - 128*t .. + cg; every other column is zero."""
+    cout, cg, k = w.shape[0], w.shape[1], w.shape[2]
+    start = (torch.arange(cout, device=w.device) // cg * cg) % 128
+    cols = (start[:, None] + torch.arange(cg, device=w.device)[None, :])[:, None, :].expand(cout, k * k, cg)
+    out = w.new_zeros(cout, k * k, 128)
+    out.scatter_(2, cols, w.permute(0, 2, 3, 1).reshape(cout, k * k, cg))
+    return out.view(cout, k, k, 128)
+
+
 def fold_bn(conv: nn.Conv2d, bn: nn.BatchNorm2d):
     """Eval BatchNorm folded into the bias-free conv before it, in fp32: w * g / sqrt(var + eps), b - mean * g / sqrt(var + eps)."""
     s = bn.weight.detach().float() / torch.sqrt(bn.running_var.detach().float() + bn.eps)
@@ -116,13 +155,16 @@ def fold_bn(conv: nn.Conv2d, bn: nn.BatchNorm2d):
 class ResNetWrapper(nn.Module):
     """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm ResNet backbone (eval / extract only)."""
 
+    _classifier = "fc."  # timm's classifier keys, dropped from a checkpoint (num_classes=0)
+
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, **kwargs):
         super().__init__()
-        if model_name not in RESNET_ARCHS:
-            raise ValueError(f"backbone '{model_name}' is not built for H100 yet; ResNets available: {sorted(RESNET_ARCHS)}")
+        archs = {**RESNET_ARCHS, **RESNEXT_ARCHS}
+        if model_name not in archs:
+            raise ValueError(f"backbone '{model_name}' is not built for H100 yet; ResNets available: {sorted(archs)}")
         if image_size % 32 != 0:
             raise ValueError("image_size must be a multiple of 32")
-        args = dict(RESNET_ARCHS[model_name])
+        args = dict(archs[model_name])
         if depths is not None:
             args["depths"] = tuple(depths)
         self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
@@ -153,14 +195,15 @@ class ResNetWrapper(nn.Module):
         net = self._pack(x.device)
         B = x.shape[0]
         out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
-        need = lib.vdk_resnet_workspace_bytes(C.byref(net), B)
+        api = "vdk_bottleneck" if isinstance(net, BottleneckNetC) else "vdk_resnet"
+        need = getattr(lib, f"{api}_workspace_bytes")(C.byref(net), B)
         if need == 0:
-            raise RuntimeError("vdk_resnet_workspace_bytes: invalid network")
+            raise RuntimeError(f"{api}_workspace_bytes: invalid network")
         if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
             self._ws = torch.empty((need,), dtype=torch.uint8, device=x.device)
         with torch.cuda.device(x.device):
-            _lib.check(lib.vdk_resnet_forward(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(), self._ws.data_ptr(),
-                                              self._ws.numel(), _lib.stream_ptr()), "vdk_resnet_forward")
+            _lib.check(getattr(lib, f"{api}_forward")(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(),
+                                                      self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()), f"{api}_forward")
         return out
 
     def _version_key(self, device):
@@ -197,11 +240,16 @@ class ResNetWrapper(nn.Module):
             kp = (k + 63) // 64 * 64
             dst.w, dst.b = bf16(torch.cat([rows, rows.new_zeros(w.shape[0], kp - k)], dim=1)), f32(b)
 
-        m, net = self.model, ResNetNetC()
+        m = self.model
+        net = ResNetNetC() if m.cardinality == 1 else BottleneckNetC()
         net.image_size, net.feat_dim = self.image_size, self.feat_dim
         for i in range(4):
             net.depths[i] = m.depths[i]
-        net.base_width, net.deep_stem, net.avg_down = m.base_width, int(m.deep_stem), int(m.avg_down)
+        net.deep_stem, net.avg_down = int(m.deep_stem), int(m.avg_down)
+        if m.cardinality == 1:
+            net.base_width = m.base_width
+        else:
+            net.width, net.cardinality, net.stem_pool = m.base_width * m.cardinality, m.cardinality, STEM_POOL_PAD1
         if m.deep_stem:
             stem(net.stem[0], *fold_bn(m.conv1[0], m.conv1[1]))
             stem(net.stem[1], *fold_bn(m.conv1[3], m.conv1[4]))
@@ -211,7 +259,11 @@ class ResNetWrapper(nn.Module):
         for i, blk in enumerate(m.blocks()):
             b = net.blocks[i]
             conv(b.conv1, *fold_bn(blk.conv1, blk.bn1))
-            conv(b.conv2, *fold_bn(blk.conv2, blk.bn2))
+            if m.cardinality == 1:
+                conv(b.conv2, *fold_bn(blk.conv2, blk.bn2))
+            else:
+                w, bias = fold_bn(blk.conv2, blk.bn2)
+                b.conv2.w, b.conv2.b = bf16(pack_grouped(w)), f32(bias)
             conv(b.conv3, *fold_bn(blk.conv3, blk.bn3))
             if blk.downsample is not None:
                 if m.avg_down:
@@ -225,12 +277,12 @@ class ResNetWrapper(nn.Module):
 
     def _load_pretrained(self, model_name: str) -> None:
         """Like TimmWrapper._load_pretrained: a timm state_dict from $VDK_PRETRAINED_DIR/<model_name>.pth (no network here);
-        the classifier (fc.*) is dropped, as num_classes=0 does."""
+        the classifier (fc.*, the legacy SENets' last_linear.*) is dropped, as num_classes=0 does."""
         root = os.environ.get("VDK_PRETRAINED_DIR")
         path = os.path.join(root, f"{model_name}.pth") if root else None
         if path and os.path.exists(path):
             sd = torch.load(path, map_location="cpu")
-            sd = {k: v for k, v in sd.items() if not k.startswith("fc.")}
+            sd = {k: v for k, v in sd.items() if not k.startswith(self._classifier)}
             self.model.load_state_dict(sd, strict=True)
         else:
             warnings.warn(f"pretrained weights for '{model_name}' not found (set VDK_PRETRAINED_DIR); using random init")
