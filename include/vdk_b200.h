@@ -202,6 +202,61 @@ int vdk_stem_maxpool(const void* x, int B, int H, int W, int C, int mode, void* 
 int vdk_se_gate(const void* y, int B, int HW, int C, int rd, const float* fc1_w, const float* fc1_b, const float* fc2_w,
                 const float* fc2_b, float* mean, float* gate, void* residual, void* stream);
 
+/* ---- Swin Transformer V2 embedding forward (eval) ---------------------------------------------- */
+/* Replaces TimmWrapper.forward for timm's SwinTransformerV2 towers (swinv2_base_window8_256,
+ * swinv2_large_window12to16_192to256; models/faceX/backbone/timm_wrapper.py:16-21, 30-38, 51-54: timm 0.9.16 forward_features
+ * returns an NHWC [B, 8, 8, C] map, so the wrapper's rank rule builds BatchNorm2d(8) over the h axis -> Flatten in (h, w, c)
+ * order -> Linear -> BatchNorm1d) followed by F.normalize (face_model.py:139).  Head dim 32; every LayerNorm has eps 1e-5.
+ * Blocks are res-post-norm: x = x + norm1(proj(attn(qkv(x)))); x = x + norm2(fc2(GELU(fc1(x)))). */
+#define VDK_SWINV2_MAX_BLOCKS 24
+typedef struct vdk_swinv2_block {
+  const void* qkv_w;        /* [3C, C] bf16 (attn.qkv.weight) */
+  const float* qkv_b;       /* [3C] = cat(q_bias, 0, v_bias) */
+  const float* attn_scale;  /* [heads] exp(min(logit_scale, ln 100)) */
+  const float* attn_bias;   /* [heads, (2w-1)^2] 16 sigmoid(cpb_mlp(relative_coords_table)), idx = (dy+w-1)(2w-1) + dx+w-1 */
+  const void* proj_w;  const float* proj_b;   /* [C, C], [C] */
+  const float* norm1_w; const float* norm1_b; /* [C] */
+  const void* fc1_w;   const float* fc1_b;    /* [4C, C], [4C] (then exact GELU) */
+  const void* fc2_w;   const float* fc2_b;    /* [C, 4C], [C] */
+  const float* norm2_w; const float* norm2_b; /* [C] */
+} vdk_swinv2_block;
+typedef struct vdk_swinv2_net {
+  int image_size;  /* 256 (the towers' size; the map is 64 -> 32 -> 16 -> 8) */
+  int feat_dim;    /* embedding width, multiple of 8 */
+  int embed_dim;   /* C of stage 0 (multiple of 64, <= 256), doubled by every patch merging */
+  int depths[4];
+  int window[4];   /* w = min(window, map) per stage: 8 or 16, dividing the map */
+  int shift[4];    /* shift of the odd blocks of each stage: w/2, or 0 when the map is one window */
+  const void* stem_w;      /* [C, 48] bf16, K order (c, kh, kw) = patch_embed.proj.weight flattened */
+  const float* stem_b;     /* [C] */
+  const float* stem_ln_w;  /* [C] patch_embed.norm */
+  const float* stem_ln_b;
+  const void* merge_w[4];      /* stage s > 0: [2Cin, 2, 2, Cin] bf16, downsample.reduction.weight permuted from timm's K order
+                                  (w-offset, h-offset, c) to (kh, kw, c); index 0 unused */
+  const float* merge_ln_w[4];  /* [2Cin] downsample.norm */
+  const float* merge_ln_b[4];
+  vdk_swinv2_block blocks[VDK_SWINV2_MAX_BLOCKS]; /* stage-major */
+  const float* norm_w; const float* norm_b;  /* model.norm */
+  const void* neck_w;   /* [feat_dim, 8*8*C] bf16, K order (h, w, c), BatchNorm2d (on h) and BatchNorm1d eval statistics folded */
+  const float* neck_b;  /* [feat_dim] */
+} vdk_swinv2_net;
+size_t vdk_swinv2_workspace_bytes(const vdk_swinv2_net* net, int batch);
+/* images: fp32 NCHW [batch,3,256,256]; embeddings: fp32 [batch, feat_dim], L2-normalised when l2_normalize != 0. */
+int vdk_swinv2_forward(const vdk_swinv2_net* net, const float* images, int batch, int l2_normalize, float* embeddings,
+                       void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_swinv2_net. */
+int vdk_swinv2_struct_sizes(size_t* out, int n);
+/* Shifted-window cosine attention of timm's WindowAttention (swin_transformer_v2.py, with SwinTransformerV2Block._attn's roll,
+ * window_partition, window_reverse and attn_mask) on the qkv Linear's output as stored: qkv bf16 [batch, H, W, 3, heads, 32]
+ * in natural token order -> out bf16 [batch, H, W, heads*32] in natural order.  Per (window, head):
+ * softmax(normalize(q) normalize(k)^T * scale[h] + bias[h, idx] + mask) v, mask = -100 between timm's shift regions.
+ * window 8 or 16 dividing H and W; shift 0 or window/2, and 0 when H == window or W == window. */
+int vdk_window_attention_fwd(const void* qkv, int batch, int H, int W, int heads, int window, int shift, const float* scale,
+                             const float* bias, void* out, void* stream);
+/* The Swin V2 block's res-post-norm in place: x [rows, C] bf16 <- x + LayerNorm(y) * ln_w + ln_b (fp32 statistics; C a multiple
+ * of 8 in [8, 1536]) — timm SwinTransformerV2Block.forward's x + norm1(...) and x + norm2(...). */
+int vdk_postnorm_residual(void* x, const void* y, int64_t rows, int C, const float* ln_w, const float* ln_b, float eps, void* stream);
+
 /* ---- ConvNeXt embedding forward (eval) ------------------------------------------------------ */
 /* Replaces TimmWrapper.forward (models/faceX/backbone/timm_wrapper.py:51-54: timm ConvNeXt features with
  * num_classes=0, global_pool='' -> BatchNorm2d -> Flatten -> Linear -> BatchNorm1d, :30-38) followed by

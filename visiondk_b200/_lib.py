@@ -95,6 +95,11 @@ SIGNATURES = {
     "vdk_bottleneck_struct_sizes": (_i, [_p, _i]),
     "vdk_stem_maxpool": (_i, [_p, _i, _i, _i, _i, _i, _p, _p]),
     "vdk_se_gate": (_i, [_p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "vdk_swinv2_workspace_bytes": (_sz, [_p, _i]),
+    "vdk_swinv2_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
+    "vdk_swinv2_struct_sizes": (_i, [_p, _i]),
+    "vdk_window_attention_fwd": (_i, [_p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p]),
+    "vdk_postnorm_residual": (_i, [_p, _p, _i64, _i, _p, _p, C.c_float, _p]),
     "vdk_dwconv7_ln": (_i, [_p, _i, _i, _i, _i, _p, _p, _p, _p, C.c_float, _p, _p]),
     "vdk_layernorm_patchify": (_i, [_p, _i, _i, _i, _i, _p, _p, C.c_float, _i, _p, _p]),
     "vdk_dwconv7": (_i, [_i, _p, _i, _i, _i, _i, _p, _p, _p, _p, C.c_float, _p, _p, _p, _p]),

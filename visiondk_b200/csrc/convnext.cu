@@ -49,6 +49,14 @@ __global__ void __launch_bounds__(256) stem_patchify_kernel(const float* __restr
   }
 }
 
+int launch_stem_patchify(const float* images, int B, int S, __nv_bfloat16* out, cudaStream_t s) {
+  const int64_t total = static_cast<int64_t>(B) * (S / 4) * (S / 4) * 12;
+  const int blocks = static_cast<int>(std::min<int64_t>((total + 255) / 256, 132 * 16));
+  stem_patchify_kernel<<<blocks, 256, 0, s>>>(images, B, S, S, out);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // depthwise 7x7 + bias + LayerNorm(C)
 // ------------------------------------------------------------------------------------------------
@@ -1138,10 +1146,7 @@ extern "C" int vdk_convnext_forward(const vdk_convnext_net* net, const float* im
   int H = S / 4, W = S / 4, C = net->dims[0];
   int M = batch * H * W;
   {
-    const int64_t total = static_cast<int64_t>(M) * 12;
-    const int blocks = static_cast<int>(std::min<int64_t>((total + 255) / 256, 132 * 16));
-    stem_patchify_kernel<<<blocks, 256, 0, s>>>(images, batch, S, S, hbuf);
-    VDK_CUDA_OK(cudaGetLastError());
+    if ((rc = launch_stem_patchify(images, batch, S, hbuf, s)) != VDK_OK) return rc;
     rc = gemm(hbuf, net->stem_w, xbuf, M, C, 48, VDK_EPI_LAYERNORM, net->stem_b, net->stem_ln_w, net->stem_ln_b, nullptr,
               VDK_DTYPE_BF16, 1);
     if (rc != VDK_OK) return rc;

@@ -12,6 +12,9 @@ int launch_dwconv7(int mode, const __nv_bfloat16* x, int batch, int H, int W, in
                    const float* ln_w, const float* ln_b, float eps, __nv_bfloat16* y, float* rstd_out,
                    const __nv_bfloat16* addend, cudaStream_t s);
 
+// 4x4/stride-4 patches of the fp32 NCHW images [B, 3, S, S] -> bf16 rows [B*(S/4)^2, 48] in (c, kh, kw) order
+int launch_stem_patchify(const float* images, int B, int S, __nv_bfloat16* out, cudaStream_t s);
+
 // out = LayerNorm_C(x) per pixel, patch == 2: regrouped into 2x2/s2 patch rows (kh, kw, c); rstd_out optional
 int launch_ln_patchify(const __nv_bfloat16* x, int B, int H, int W, int C, const float* ln_w, const float* ln_b, float eps,
                        int patch, __nv_bfloat16* out, float* rstd_out, cudaStream_t s);

@@ -223,6 +223,14 @@ int vdk_bottleneck_struct_sizes(size_t* out, int n) {
   return k;
 }
 
+// the same for the Swin V2 network: vdk_swinv2_net
+int vdk_swinv2_struct_sizes(size_t* out, int n) {
+  const size_t sizes[] = {sizeof(vdk_swinv2_net)};
+  const int k = static_cast<int>(sizeof(sizes) / sizeof(sizes[0]));
+  for (int i = 0; i < n && i < k; ++i) out[i] = sizes[i];
+  return k;
+}
+
 const char* vdk_last_error_string(void) { return vdk::t_error; }
 
 int vdk_prof_begin(void) {
