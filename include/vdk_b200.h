@@ -76,6 +76,9 @@ typedef struct vdk_gemm_desc {
   int trans_b; /* 1: B is stored [K,N] row-major (pitch ldb >= N).  Backward GEMMs use these: dgrad
                   dX = dY . W (B = W stored [N_out,K_in] = [K,N] of this contraction) and wgrad dW = dY^T . X
                   (both operands stored with the token index slow) need no transposed copies. */
+  float* a_col_sums; /* may be NULL; trans_a with split_k > 1 and split_stride > 0 only: split s also stores the column
+                        sums of A over its K range, sum_k A[k,m] in fp32, to a_col_sums[s*M + m] (the bias gradient of
+                        the wgrad above, from the A tiles the GEMM streams anyway).  16-byte aligned. */
 } vdk_gemm_desc;
 int vdk_gemm(const vdk_gemm_desc* desc, void* stream);
 /* Number of K splits vdk_gemm will actually use for (K, split_k). */

@@ -54,6 +54,7 @@ b1 = torch.randn(4 * Cn, device=dev)
 gam = torch.randn(Cn, device=dev)
 out = torch.empty_like(x)
 slabs = torch.empty(64 * 1024 * 1024 // 4, device=dev)
+colsl = torch.empty(1024 * 1024, device=dev)  # per-split column sums of A (the bias gradient) of the "wgrad + bias" lines
 # downsample into the next stage: 2x2 / stride-2 patches of the LayerNorm output as a GEMM (tokens M/4, K = 4C, N = 2C)
 Md = M // 4
 dsw = bf(2 * Cn, 4 * Cn, scale=0.05)
@@ -68,10 +69,11 @@ def inst(N_, epi=_lib.EPI_NONE, ta=0, tb=0):
 
 
 def gemm(A, Bm, D, M_, N_, K_, lda, ldb, ldd, epi=_lib.EPI_NONE, bias=0, gamma=0, residual=0, ldr=0, out_dtype=_lib.DTYPE_BF16,
-         split=1, stride=0, aux=0, ta=0, tb=0):
+         split=1, stride=0, aux=0, ta=0, tb=0, colsums=0):
     g = _lib.GemmDesc(A=A.data_ptr(), B=Bm.data_ptr(), D=D.data_ptr(), M=M_, N=N_, K=K_, lda=lda, ldb=ldb, ldd=ldd,
                       in_dtype=_lib.DTYPE_BF16, out_dtype=out_dtype, epilogue=epi, bias=bias, gamma=gamma, beta=0, residual=residual,
-                      ldr=ldr, ln_eps=1e-6, split_k=split, split_stride=stride, aux_out=aux, trans_a=ta, trans_b=tb)
+                      ldr=ldr, ln_eps=1e-6, split_k=split, split_stride=stride, aux_out=aux, trans_a=ta, trans_b=tb,
+                      a_col_sums=colsums)
     _lib.check(lib.vdk_gemm(C.byref(g), sp), "gemm")
 
 
@@ -111,6 +113,12 @@ kernels = {
                                        stride=Cn * 4 * Cn, ta=1, tb=1), 8.0 * M * Cn * Cn, 2.0 * M * Cn * 5, inst(4 * Cn, ta=1, tb=1)),
     "fc1 wgrad (slabs)": (lambda: gemm(hpost, xf, slabs, 4 * Cn, Cn, M, 4 * Cn, Cn, Cn, out_dtype=_lib.DTYPE_FP32, split=split1,
                                        stride=4 * Cn * Cn, ta=1, tb=1), 8.0 * M * Cn * Cn, 2.0 * M * Cn * 5, inst(Cn, ta=1, tb=1)),
+    "fc2 wgrad + bias (slabs)": (lambda: gemm(dxf, hpost, slabs, Cn, 4 * Cn, M, Cn, 4 * Cn, 4 * Cn, out_dtype=_lib.DTYPE_FP32, split=split,
+                                              stride=Cn * 4 * Cn, ta=1, tb=1, colsums=colsl.data_ptr()), 8.0 * M * Cn * Cn,
+                                 2.0 * M * Cn * 5, inst(4 * Cn, ta=1, tb=1)),
+    "fc1 wgrad + bias (slabs)": (lambda: gemm(hpost, xf, slabs, 4 * Cn, Cn, M, 4 * Cn, Cn, Cn, out_dtype=_lib.DTYPE_FP32, split=split1,
+                                              stride=4 * Cn * Cn, ta=1, tb=1, colsums=colsl.data_ptr()), 8.0 * M * Cn * Cn,
+                                 2.0 * M * Cn * 5, inst(Cn, ta=1, tb=1)),
 }
 if stage < 3:
     kernels["downsample (bias)"] = (lambda: gemm(x.reshape(Md, 4 * Cn), dsw, dso, Md, 2 * Cn, 4 * Cn, 4 * Cn, 4 * Cn, 2 * Cn,

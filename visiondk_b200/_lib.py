@@ -60,7 +60,7 @@ class GemmDesc(C.Structure):
         ("in_dtype", C.c_int), ("out_dtype", C.c_int), ("epilogue", C.c_int),
         ("bias", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("residual", C.c_void_p),
         ("ldr", C.c_int), ("ln_eps", C.c_float), ("split_k", C.c_int), ("split_stride", C.c_longlong), ("aux_out", C.c_void_p), ("trans_a", C.c_int),
-        ("trans_b", C.c_int),
+        ("trans_b", C.c_int), ("a_col_sums", C.c_void_p),
     ]
 
 

@@ -33,7 +33,6 @@ int launch_neck_finalize(const float* slabs, int n_slabs, size_t slab_stride, in
 
 namespace vdk {
 // ---- training-side launchers (train_ops.cu) ----
-int launch_col_sum(const __nv_bfloat16* x, int64_t M, int C, int ld, float* out, cudaStream_t s);
 int launch_ln_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, const float* rstd, int B, int H, int W, int C,
                   const float* ln_w, const float* ln_b, int patch, __nv_bfloat16* dx, const __nv_bfloat16* addend,
                   float* dgamma, float* dbeta, cudaStream_t s);

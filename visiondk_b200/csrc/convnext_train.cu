@@ -410,35 +410,6 @@ extern "C" int vdk_convnext_train_backward_units(const vdk_convnext_net* net) {
   return n;
 }
 
-// A second stream for the bias-gradient column sums of dH ([tokens, 4C]: one full HBM pass over a tensor the next two GEMMs read
-// anyway).  The persistent GEMM CTAs leave ~11 k registers and no shared memory per SM — enough for one 256-thread block of the
-// (shared-memory-free) column-sum kernel — so the sum runs UNDER the weight- and data-gradient GEMMs of fc1 instead of in
-// front of them.  Fork: the side stream waits for the event recorded after the GEMM that produced dH; join: the caller's stream
-// waits for the side stream's last event before the call returns (the gradients it wrote are then ordered before anything the
-// caller enqueues next: the optimizer, an all-reduce, the next forward that overwrites dH).  It is OFF unless
-// VDK_TRAIN_SIDE_STREAM=1.
-struct SideStream {
-  cudaStream_t stream = nullptr;
-  cudaEvent_t fork = nullptr, join = nullptr;
-  bool ok = false, used = false;
-};
-static SideStream& side_stream() {
-  static thread_local SideStream ss;
-  static const bool enabled = [] {
-    const char* e = getenv("VDK_TRAIN_SIDE_STREAM");
-    return e ? atoi(e) != 0 : false;
-  }();
-  if (enabled && !ss.ok && ss.stream == nullptr) {
-    if (cudaStreamCreateWithFlags(&ss.stream, cudaStreamNonBlocking) == cudaSuccess &&
-        cudaEventCreateWithFlags(&ss.fork, cudaEventDisableTiming) == cudaSuccess &&
-        cudaEventCreateWithFlags(&ss.join, cudaEventDisableTiming) == cudaSuccess)
-      ss.ok = true;
-    else
-      cudaGetLastError();
-  }
-  return ss;
-}
-
 static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensors* p, const vdk_convnext_tensors* g,
                           const float* d_feats, int batch, void* workspace, size_t workspace_bytes, void* stream, int u_begin,
                           int u_end) {
@@ -456,8 +427,6 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
   auto F32 = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
   const Gemm G{s};
   const int F = net->feat_dim;
-  SideStream& side = side_stream();
-  side.used = false;
 
   // ---- neck ----
   const int H3 = L.st[3].H, W3 = L.st[3].W, C3 = L.st[3].C, M3 = static_cast<int>(L.st[3].M), Kn = H3 * W3 * C3;
@@ -495,24 +464,15 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
       const vdk_convnext_block* b = &net->blocks[k];
       const vdk_convnext_block_tensors* pb = &p->blocks[k];
       const vdk_convnext_block_tensors* gb = &g->blocks[k];
-      // fc2 + layer scale: G = dOut^T . h_post;  dW2 = diag(gamma) G;  dgamma, db2 from G, W2, colsum(dOut)
+      // fc2 + layer scale: G = dOut^T . h_post;  dW2 = diag(gamma) G;  dgamma, db2 from G, W2, colsum(dOut) (from the same GEMM)
       float* sdo = F32(L.sdo) + static_cast<size_t>(k) * 2048;
-      RC(launch_col_sum(B16(dx), M, C, C, sdo, s));
-      RC(G.wgrad(B16(dx), B16(L.hpost[k]), F32(L.G), C, 4 * C, M, C, 4 * C, F32(L.wslab), false));
+      RC(G.wgrad(B16(dx), B16(L.hpost[k]), F32(L.G), C, 4 * C, M, C, 4 * C, F32(L.wslab), false, sdo));
       RC(launch_layerscale_finalize(F32(L.G), pb->fc2_w, pb->fc2_b, pb->gamma, sdo, C, 4 * C, gb->fc2_w, gb->gamma, gb->fc2_b, s));
       // dH_pre = (dOut . diag(gamma) W2) * gelu'(h_pre)   -> overwrites the h_post buffer
       RC(G.run(B16(dx), b->fc2_wg, B16(L.hpost[k]), M, 4 * C, C, C, 4 * C, 4 * C, VDK_EPI_MUL_GELU_GRAD, nullptr, nullptr,
                B16(L.hpre[k]), 4 * C, VDK_DTYPE_BF16, 1, 0, 0, 1));
       __nv_bfloat16* dh = B16(L.hpost[k]);
-      if (side.ok) {  // bias gradient of fc1 on the side stream, under the two GEMMs below
-        VDK_CUDA_OK(cudaEventRecord(side.fork, s));
-        VDK_CUDA_OK(cudaStreamWaitEvent(side.stream, side.fork, 0));
-        RC(launch_col_sum(dh, M, 4 * C, 4 * C, gb->fc1_b, side.stream));
-        side.used = true;
-      } else {
-        RC(launch_col_sum(dh, M, 4 * C, 4 * C, gb->fc1_b, s));
-      }
-      RC(G.wgrad(dh, B16(L.y[k]), gb->fc1_w, 4 * C, C, M, 4 * C, C, F32(L.wslab), true));
+      RC(G.wgrad(dh, B16(L.y[k]), gb->fc1_w, 4 * C, C, M, 4 * C, C, F32(L.wslab), true, gb->fc1_b));
       RC(G.run(dh, b->fc1_w, B16(L.dy), M, C, 4 * C, 4 * C, C, C, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_BF16, 1, 0, 0, 1));
       // LayerNorm backward, depthwise weight gradient, depthwise data gradient (+ the residual branch)
       RC(launch_ln_bwd(B16(L.dy), B16(L.y[k]), F32(L.rstd[k]), batch, H, W, C, b->ln_w, b->ln_b, 1, B16(L.dconv), nullptr, gb->ln_w,
@@ -540,8 +500,7 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
       const vdk_convnext_down* d = &net->down[st];
       const vdk_convnext_down_tensors* gd = &g->down[st];
       const int Cin = L.st[st - 1].C;
-      RC(launch_col_sum(B16(dx), M, C, C, gd->conv_b, s));
-      RC(G.wgrad(B16(dx), B16(L.patch[st]), F32(L.gwc), C, 4 * Cin, M, C, 4 * Cin, F32(L.wslab), false));
+      RC(G.wgrad(B16(dx), B16(L.patch[st]), F32(L.gwc), C, 4 * Cin, M, C, 4 * Cin, F32(L.wslab), false, gd->conv_b));
       RC(launch_permute021(F32(L.gwc), C, 4, Cin, nullptr, nullptr, gd->conv_w, 1, s));  // [C][4][Cin] -> += [C][Cin][4]
       RC(G.run(B16(dx), d->conv_w, B16(L.dy), M, 4 * Cin, C, C, 4 * Cin, 4 * Cin, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0,
                VDK_DTYPE_BF16, 1, 0, 0, 1));
@@ -555,12 +514,7 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
     const int M0 = static_cast<int>(L.st[0].M), C0 = L.st[0].C;
     RC(launch_ln_bwd(B16(dx), B16(L.xs[0][0]), F32(L.rstd0), batch, L.st[0].H, L.st[0].W, C0, net->stem_ln_w, net->stem_ln_b, 1,
                      B16(L.dy), nullptr, g->stem_ln_w, g->stem_ln_b, s));
-    RC(launch_col_sum(B16(L.dy), M0, C0, C0, g->stem_b, s));
-    RC(G.wgrad(B16(L.dy), B16(L.p0), g->stem_w, C0, 48, M0, C0, 48, F32(L.wslab), true));
-  }
-  if (side.used) {  // join: everything the side stream wrote is ordered before whatever the caller enqueues next
-    VDK_CUDA_OK(cudaEventRecord(side.join, side.stream));
-    VDK_CUDA_OK(cudaStreamWaitEvent(s, side.join, 0));
+    RC(G.wgrad(B16(L.dy), B16(L.p0), g->stem_w, C0, 48, M0, C0, 48, F32(L.wslab), true, g->stem_b));
   }
   return VDK_OK;
 }

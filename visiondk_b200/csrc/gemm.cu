@@ -5,7 +5,8 @@
 //
 // One persistent CTA per SM, 384 threads:
 //   warpgroup 0    : TMA producer (one thread; A tile 128x64, B tile BNx64 per stage, 128-byte swizzle), registers
-//                    handed to the consumers with setmaxnreg
+//                    handed to the consumers with setmaxnreg; in the weight-gradient form, warps 1-2 also sum A's
+//                    columns from the stages (the bias gradient, `col_sums`)
 //   warpgroups 1-2 : consumers, 64 rows each: wgmma m64 x BN x 16 into registers (fp32), then the epilogue.  The
 //                    epilogue math (bias / GELU / layer-scale+residual / LayerNorm / GELU') runs on the accumulator
 //                    fragments; each 64-row x 128-byte box of results is written to a swizzled shared-memory ring
@@ -63,7 +64,12 @@ struct GemmParams {
       int cv_wo, cv_howo;  // convolution: output width, output pixels per image
     };
   };
-  void* aux;  // GELU only: also store the pre-activation (acc + bias) here, pitch ldd (saved for the backward)
+  union {
+    void* aux;  // GELU only: also store the pre-activation (acc + bias) here, pitch ldd (saved for the backward)
+    // split-K slabs with an MN-major A only (the weight-gradient form): split s also stores the column sums of A over
+    // its K range, sum_k A[k, m], to col_sums[s * M + m] (the bias gradient, summed in the producer warpgroup)
+    float* col_sums;
+  };
   int partial_out;  // the caller asked for split-K: raw fp32 partials are added / slab-stored even if one split remains
 };
 
@@ -236,6 +242,9 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(par_all + 2 * Cfg::kParFloats);
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* res_bar = empty_bar + kStages;  // [2]: a consumer warpgroup's residual boxes have landed
+  // A's column sums: two producer warps read every A stage as well and release it on the empty barrier
+  constexpr bool kColSums = kTA && kMode == kGemmPlain;
+  const bool col_sums = kColSums && p.partial_out && p.split_stride > 0 && p.col_sums != nullptr;
 
 
   if (threadIdx.x == 0) {
@@ -248,7 +257,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       prefetch_tensormap(&map_r);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
+      mbar_init(&empty_bar[i], col_sums ? 10 : 8);  // one arrival per consumer warp (and per column-sum warp)
     }
     mbar_init(&res_bar[0], 1);
     mbar_init(&res_bar[1], 1);
@@ -312,6 +321,71 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             stage = 0;
             phase ^= 1;
           }
+        }
+      }
+    } else if (col_sums && threadIdx.x >= 32 && threadIdx.x < 96) {
+      // column sums of A (bias gradient of the weight gradient): warps 1-2 walk the consumers' stage / phase sequence.
+      // Warp 1 + j sums box j of each A stage (64 contraction rows x 64 M columns, 128-byte rows) in fp32, of the 16-bit
+      // values as stored: lane = 8-byte piece lane % 16 (4 columns) of rows lane / 16 + 2 i.  8-byte pieces keep four
+      // accumulators per thread, so that four loads fit in flight within the producer's 40 registers.  They read the
+      // stages of the work items with n0 == 0 only (one per M tile and split), but release every stage, so empty_bar's
+      // arrival count is fixed.
+      const int j = (threadIdx.x >> 5) - 1, lane = threadIdx.x & 31;
+      const int piece = lane & 15, r0 = lane >> 4;
+      // row r0 + 2 i sits at (r0 + 2 i) * 128 bytes, its 16-byte chunk c at c ^ (r0 + 2 (i % 4)) = (c ^ r0) ^ 2 (i % 4)
+      // (r0 <= 1): four base offsets, one per i % 4; the rest are immediates
+      uint32_t off[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        off[q] = j * 8192 + r0 * 128 + q * 256 + (((((piece >> 1) ^ r0) << 4)) ^ (q << 5)) + (piece & 1) * 8;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int mn = tile % (num_m * num_n), split = tile / (num_m * num_n);
+        const int m0 = (mn / num_n) * kBM;
+        const bool mine = (mn % num_n) == 0;
+        const int kb0 = split * kb_per_split;
+        const int kb1 = min(kb0 + kb_per_split, num_kb_total);
+        float s[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait<true>(&full_bar[stage], phase);
+          if (mine) {
+            const uint8_t* sa = smem + stage * Cfg::kStageBytes;
+#pragma unroll
+            for (int i0 = 0; i0 < 32; i0 += 4) {  // four loads in flight, then their 16 additions
+              uint2 v[4];
+#pragma unroll
+              for (int q = 0; q < 4; ++q) v[q] = *reinterpret_cast<const uint2*>(sa + off[q] + i0 * 256);
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const uint32_t w[2] = {v[q].x, v[q].y};
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  if constexpr (kBf16) {  // a bf16 is the top half of its fp32
+                    s[2 * e] += __uint_as_float(w[e] << 16);
+                    s[2 * e + 1] += __uint_as_float(w[e] & 0xffff0000u);
+                  } else {
+                    const float2 f = unpack2(w[e], VDK_DTYPE_FP16);
+                    s[2 * e] += f.x;
+                    s[2 * e + 1] += f.y;
+                  }
+                }
+              }
+            }
+          }
+          __syncwarp();  // the warp's reads of the stage are done before it is released
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+        if (mine) {  // the two row groups of a piece meet
+#pragma unroll
+          for (int e = 0; e < 4; ++e) s[e] += __shfl_xor_sync(0xffffffffu, s[e], 16);
+          const int m = m0 + j * 64 + piece * 4;
+          if (lane < 16 && m < p.M)  // M % 8 == 0 (MN-major A): the 4 columns are all in or all out
+            *reinterpret_cast<float4*>(p.col_sums + static_cast<size_t>(split) * p.M + m) = make_float4(s[0], s[1], s[2], s[3]);
         }
       }
     }
@@ -627,6 +701,9 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   if (g.split_k > 1)
     VDK_REQUIRE(g.out_dtype == VDK_DTYPE_FP32 && g.epilogue == VDK_EPI_NONE && !g.bias,
                 "vdk_gemm: split_k > 1 needs fp32 output, no bias and no epilogue (partials are atomically added)");
+  if (g.a_col_sums)
+    VDK_REQUIRE(g.trans_a && g.split_k > 1 && g.split_stride != 0 && (reinterpret_cast<uintptr_t>(g.a_col_sums) & 15) == 0,
+                "vdk_gemm: a_col_sums needs trans_a, split_k > 1 with split_stride > 0, and 16-byte alignment");
 
   // LayerNorm needs the whole row in one tile; otherwise narrow outputs use 128-column tiles (more tiles to
   // balance over 132 SMs) and wide ones 256.
@@ -667,6 +744,7 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   }
   GemmParams p{g.M, g.N, g.K, g.D, g.ldd, g.bias, g.gamma, g.beta, g.residual, g.ldr, g.out_dtype, g.epilogue,
                g.ln_eps, split, g.split_k > 1 ? (long long)g.split_stride : 0ll, g.aux_out, (g.split_k > 1) ? 1 : 0};
+  if (g.a_col_sums) p.col_sums = g.a_col_sums;  // aux_out needs split_k <= 1: the union's other member is unused here
   const bool bf = g.in_dtype == VDK_DTYPE_BF16;
   // algorithmic bytes: both operands once, the output once (x2 for an auxiliary 16-bit output), a 16-bit residual / saved tile once
   const double osz = g.out_dtype == VDK_DTYPE_FP32 ? 4.0 : 2.0;

@@ -17,32 +17,40 @@ inline int wgrad_splits(int M, int N, size_t K) {
   const int want = std::max(2, (2 * sm_count()) / std::max(1, tiles));
   return vdk_gemm_effective_splits(static_cast<int>(K), want);
 }
+// the dW slabs [splits][M][N], then the column-sum slabs [splits][M] of a bias gradient
 inline size_t wgrad_slab_bytes(int M, int N, size_t K) {
-  return static_cast<size_t>(std::max(2, wgrad_splits(M, N, K))) * M * N * 4;
+  return static_cast<size_t>(std::max(2, wgrad_splits(M, N, K))) * M * (static_cast<size_t>(N) + 1) * 4;
 }
 
 struct Gemm {
   cudaStream_t s;
   int run(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb, int ldd, int epi, const float* bias,
           const float* gamma, const void* res, int ldr, int out_dtype, int split, long long stride, int ta, int tb,
-          void* aux_out = nullptr) const {
+          void* aux_out = nullptr, float* a_col_sums = nullptr) const {
     vdk_gemm_desc g{};
     g.A = A; g.B = B; g.D = D;
     g.M = M; g.N = N; g.K = K; g.lda = lda; g.ldb = ldb; g.ldd = ldd;
     g.in_dtype = VDK_DTYPE_BF16; g.out_dtype = out_dtype; g.epilogue = epi;
     g.bias = bias; g.gamma = gamma; g.residual = res; g.ldr = ldr;
     g.ln_eps = 1e-6f; g.split_k = split; g.split_stride = stride; g.trans_a = ta; g.trans_b = tb; g.aux_out = aux_out;
+    g.a_col_sums = a_col_sums;
     return gemm_run(g, s);
   }
-  // weight gradient D[M,N] (+)= A^T B over a long K (A stored [K,M], B stored [K,N]): split-K partial slabs + fixed-order reduction
-  int wgrad(const void* A, const void* B, float* D, int M, int N, int K, int lda, int ldb, float* slabs, bool accumulate) const {
+  // weight gradient D[M,N] (+)= A^T B over a long K (A stored [K,M], B stored [K,N]): split-K partial slabs + fixed-order
+  // reduction.  bias_grad (optional): += the column sums of A, sum_k A[k,m] (the bias gradient of the layer whose output
+  // gradient A is), which the GEMM computes from the A tiles it streams and which are reduced over the splits the same way.
+  int wgrad(const void* A, const void* B, float* D, int M, int N, int K, int lda, int ldb, float* slabs, bool accumulate,
+            float* bias_grad = nullptr) const {
     VDK_REQUIRE((static_cast<size_t>(M) * N) % 4 == 0, "wgrad: M*N must be a multiple of 4");
     const int split = wgrad_splits(M, N, static_cast<size_t>(K));
     const size_t stride = static_cast<size_t>(M) * N;
+    float* col_slabs = bias_grad ? slabs + static_cast<size_t>(split) * stride : nullptr;
     int rc = run(A, B, slabs, M, N, K, lda, ldb, N, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_FP32, std::max(2, split),
-                 static_cast<long long>(stride), 1, 1);
+                 static_cast<long long>(stride), 1, 1, nullptr, col_slabs);
     if (rc != VDK_OK) return rc;
-    return launch_slab_reduce(slabs, split, stride, static_cast<int64_t>(stride / 4), D, accumulate ? 1 : 0, s);
+    rc = launch_slab_reduce(slabs, split, stride, static_cast<int64_t>(stride / 4), D, accumulate ? 1 : 0, s);
+    if (rc != VDK_OK || !bias_grad) return rc;
+    return launch_slab_reduce(col_slabs, split, static_cast<size_t>(M), M / 4, bias_grad, 1, s);
   }
 };
 

@@ -35,44 +35,6 @@ __device__ __forceinline__ uint4 pack8(const float (&v)[8]) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// column sums of a bf16 [M, C] matrix into fp32 out[C] (+=): bias gradients
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-col_sum_bf16_kernel(const __nv_bfloat16* __restrict__ x, int64_t M, int C, int ld, float* __restrict__ out) {
-  // a warp owns 32 x 8 = 256 consecutive columns (16-byte loads); the 8 warps of a block stride over rows
-  __shared__ float red[8][256];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int c0 = blockIdx.x * 256 + lane * 8;
-  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  if (c0 < C) {
-    for (int64_t r = static_cast<int64_t>(blockIdx.y) * 8 + warp; r < M; r += static_cast<int64_t>(gridDim.y) * 8) {
-      float v[8];
-      unpack8(*reinterpret_cast<const uint4*>(x + r * ld + c0), v);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] += v[j];
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) red[warp][lane * 8 + j] = acc[j];
-  __syncthreads();
-  const int c = blockIdx.x * 256 + threadIdx.x;
-  if (c < C) {
-    float s = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) s += red[w][threadIdx.x];
-    atomicAdd(out + c, s);
-  }
-}
-
-int launch_col_sum(const __nv_bfloat16* x, int64_t M, int C, int ld, float* out, cudaStream_t s) {
-  VDK_REQUIRE(C % 8 == 0 && ld % 8 == 0, "col_sum: C and pitch must be multiples of 8");
-  dim3 grid((C + 255) / 256, static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((M + 63) / 64, 592))));
-  col_sum_bf16_kernel<<<grid, 256, 0, s>>>(x, M, C, ld, out);
-  VDK_CUDA_OK(cudaGetLastError());
-  return VDK_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
 // LayerNorm backward over C (optionally through the 2x2/s2 patch regrouping of the downsample layers)
 // ------------------------------------------------------------------------------------------------
 // dy, y: [rows, patch*patch*C] (grad of / saved LayerNorm output, patch-row layout), rstd[pixel], dx: NHWC [B,H,W,C].

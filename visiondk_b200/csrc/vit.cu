@@ -967,23 +967,19 @@ static int vit_backward_range(const vdk_vit_net* net, const vdk_vit_tensors* p, 
     const vdk_vit_block* b = &net->blocks[i];
     const vdk_vit_block_tensors* gb = &g->blocks[i];
     // MLP: x_out = x_mid + fc2(gelu(fc1(LN2(x_mid))))
-    RC(launch_col_sum(B16(dx), M, C, C, gb->fc2_b, s));
-    RC(G.wgrad(B16(dx), B16(L.hpost[i]), gb->fc2_w, C, 4 * C, M, C, 4 * C, slabs, true));
+    RC(G.wgrad(B16(dx), B16(L.hpost[i]), gb->fc2_w, C, 4 * C, M, C, 4 * C, slabs, true, gb->fc2_b));
     RC(G.run(B16(dx), b->fc2_w, B16(L.dbig), M, 4 * C, C, C, 4 * C, 4 * C, VDK_EPI_MUL_GELU_GRAD, nullptr, nullptr, B16(L.hpre[i]), 4 * C,
              VDK_DTYPE_BF16, 1, 0, 0, 1));
-    RC(launch_col_sum(B16(L.dbig), M, 4 * C, 4 * C, gb->fc1_b, s));
-    RC(G.wgrad(B16(L.dbig), B16(L.y2[i]), gb->fc1_w, 4 * C, C, M, 4 * C, C, slabs, true));
+    RC(G.wgrad(B16(L.dbig), B16(L.y2[i]), gb->fc1_w, 4 * C, C, M, 4 * C, C, slabs, true, gb->fc1_b));
     RC(G.run(B16(L.dbig), b->fc1_w, B16(L.dy), M, C, 4 * C, 4 * C, C, C, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_BF16, 1, 0, 0, 1));
     RC(launch_ln_bwd(B16(L.dy), B16(L.y2[i]), F32(L.r2[i]), batch, T, 1, C, b->ln2_w, b->ln2_b, 1, B16(dx_other), B16(dx), gb->ln2_w,
                      gb->ln2_b, s));  // d x_mid = LN2 backward + the residual branch
     std::swap(dx, dx_other);
     // attention: x_mid = x_in + proj(attn(qkv(LN1(x_in))))
-    RC(launch_col_sum(B16(dx), M, C, C, gb->proj_b, s));
-    RC(G.wgrad(B16(dx), B16(L.att[i]), gb->proj_w, C, C, M, C, C, slabs, true));
+    RC(G.wgrad(B16(dx), B16(L.att[i]), gb->proj_w, C, C, M, C, C, slabs, true, gb->proj_b));
     RC(G.run(B16(dx), b->proj_w, B16(L.dy), M, C, C, C, C, C, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_BF16, 1, 0, 0, 1));
     RC(launch_attention_bwd(B16(L.qkv[i]), B16(L.att[i]), B16(L.dy), F32(L.lse[i]), batch, T, net->heads, kAttD, B16(L.dbig), s));
-    RC(launch_col_sum(B16(L.dbig), M, 3 * C, 3 * C, gb->qkv_b, s));
-    RC(G.wgrad(B16(L.dbig), B16(L.y1[i]), gb->qkv_w, 3 * C, C, M, 3 * C, C, slabs, true));
+    RC(G.wgrad(B16(L.dbig), B16(L.y1[i]), gb->qkv_w, 3 * C, C, M, 3 * C, C, slabs, true, gb->qkv_b));
     RC(G.run(B16(L.dbig), b->qkv_w, B16(L.dy), M, C, 3 * C, 3 * C, C, C, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_BF16, 1, 0, 0, 1));
     RC(launch_ln_bwd(B16(L.dy), B16(L.y1[i]), F32(L.r1[i]), batch, T, 1, C, b->ln1_w, b->ln1_b, 1, B16(dx_other), B16(dx), gb->ln1_w,
                      gb->ln1_b, s));
@@ -995,8 +991,7 @@ static int vit_backward_range(const vdk_vit_net* net, const vdk_vit_tensors* p, 
     vit_assemble_bwd_kernel<<<static_cast<int>(std::min<int64_t>((tot + 255) / 256, 132 * 8)), 256, 0, s>>>(B16(dx), batch, N, C, B16(L.dtok),
                                                                                                            g->pos_embed, g->cls_token);
     VDK_CUDA_OK(cudaGetLastError());
-    RC(launch_col_sum(B16(L.dtok), static_cast<int64_t>(batch) * N, C, C, g->patch_b, s));
-    RC(G.wgrad(B16(L.dtok), B16(L.rows), g->patch_w, C, L.Kp, batch * N, C, L.Kp, slabs, true));
+    RC(G.wgrad(B16(L.dtok), B16(L.rows), g->patch_w, C, L.Kp, batch * N, C, L.Kp, slabs, true, g->patch_b));
   }
   return VDK_OK;
 }
