@@ -52,6 +52,10 @@ int vdk_device_check(void);
 /* vdk_conv2d only (vdk_gemm rejects them): */
 #define VDK_EPI_RELU 5           /* D = max(acc + bias[n], 0)  (conv + folded BatchNorm + ReLU) */
 #define VDK_EPI_RESIDUAL_RELU 6  /* D = max(residual[m,n] + (acc + bias[n]), 0)  (last conv of a ResNet bottleneck) */
+/* vdk_conv2d_ex only (vdk_gemm and vdk_conv2d reject them).  SiLU x / (1 + e^-x) with the approximate exp2 and reciprocal:
+ * relative error <= 1e-6 for |x| <= 64 before the output rounding. */
+#define VDK_EPI_SILU 7           /* D = silu(acc + bias[n])  (conv + folded BatchNorm + SiLU) */
+#define VDK_EPI_SILU_RESIDUAL 8  /* D = residual[m,n] + silu(acc + bias[n])  (timm's ConvBnAct with skip: the activation first) */
 
 typedef struct vdk_gemm_desc {
   const void* A; /* [M,K] 16-bit, pitch lda */
@@ -120,6 +124,25 @@ int vdk_conv2d(const vdk_conv_desc* desc, void* stream);
  * Cin == Cout a multiple of 128, groups >= 2 with cg dividing 128, epilogue VDK_EPI_RELU (no residual); kernel, stride and
  * pad as vdk_conv2d. */
 int vdk_conv2d_grouped(const vdk_conv_desc* desc, int groups, void* stream);
+/* Extended form for TensorFlow-"same" padded MBConv networks (timm's tf_efficientnetv2_*, timm/models/_efficientnet_blocks.py
+ * with Conv2dSame): separate low and high zero padding per axis, the SiLU epilogues, and Cin any multiple of 8.
+ * Ho = (H + pad_h_lo + pad_h_hi - kernel) / stride + 1, likewise Wo.  1x1 / stride-1 / unpadded convolutions run as a plain
+ * GEMM over [B*H*W, Cin] with w [Cout, Cin]; every other shape is an implicit GEMM whose K blocks are 64 channels of one
+ * tap, so w is [Cout, kernel, kernel, Cinp] with Cinp = Cin rounded up to a multiple of 64 and zero columns from Cin on
+ * (executed MACs: Cinp / Cin times the useful ones; the input is read once, its padding channels are never stored). */
+typedef struct vdk_conv_ex_desc {
+  const void* x;        /* [B, H, W, Cin] bf16 */
+  const void* w;        /* [Cout, Cin] (1x1 / stride 1 / unpadded) or [Cout, kernel, kernel, Cinp] bf16 */
+  const float* bias;    /* [Cout] or NULL */
+  const void* residual; /* [B, Ho, Wo, Cout] bf16, VDK_EPI_SILU_RESIDUAL only; may be y itself (in place) */
+  void* y;              /* [B, Ho, Wo, Cout] bf16 */
+  int B, H, W, Cin, Cout;
+  int kernel, stride;
+  int pad_h_lo, pad_h_hi, pad_w_lo, pad_w_hi; /* each in [0, kernel) */
+  int epilogue; /* VDK_EPI_NONE, VDK_EPI_SILU or VDK_EPI_SILU_RESIDUAL */
+} vdk_conv_ex_desc;
+/* Cin and Cout multiples of 8, 1 <= kernel <= 16, 1 <= stride <= 8. */
+int vdk_conv2d_ex(const vdk_conv_ex_desc* desc, void* stream);
 
 /* ---- ResNet embedding forward (eval) --------------------------------------------------------- */
 /* Replaces TimmWrapper.forward for timm's Bottleneck ResNets (resnet50/101/152, their -D variants, wide_resnet50_2/101_2;
@@ -204,6 +227,64 @@ int vdk_stem_maxpool(const void* x, int B, int H, int W, int C, int mode, void* 
  * fc2_w [C, rd]), then residual [B, HW, C] bf16 = ReLU(y * gate + residual) in place. */
 int vdk_se_gate(const void* y, int B, int HW, int C, int rd, const float* fc1_w, const float* fc1_b, const float* fc2_w,
                 const float* fc2_b, float* mean, float* gate, void* residual, void* stream);
+
+/* ---- EfficientNetV2 embedding forward (eval) ---------------------------------------------------- */
+/* Replaces TimmWrapper.forward for timm's tf_efficientnetv2_s / _m / _l (timm/models/efficientnet.py,
+ * _efficientnet_blocks.py; models/faceX/backbone/timm_wrapper.py:16-21, 30-38, 51-54) followed by F.normalize
+ * (face_model.py:139).  Every eval BatchNorm (eps 1e-3) folded into its conv; NHWC bf16 activations in `workspace`; every
+ * convolution TF-"same" padded: per axis total = max((ceil(H / s) - 1) s + k - H, 0), lo = total / 2, hi = total - lo.
+ * Blocks (timm kinds), with a shortcut when stride == 1 and cin == cout:
+ *   CN (ConvBnAct)      out = silu(conv3x3(x)) [+ x]
+ *   ER (EdgeResidual)   out = conv_pwl(silu(conv3x3/s(x))) [+ x]
+ *   IR (InvertedResid.) e = silu(conv_pw(x)); d = silu(dwconv3x3/s(e)); g = sigmoid(W2 silu(W1 mean_hw(d) + b1) + b2);
+ *                       out = conv_pwl(d * g) [+ x]
+ * then conv_head 1x1 + SiLU and the folded CNN neck over the (h, w, c) map. */
+#define VDK_EFFNETV2_MAX_BLOCKS 80
+#define VDK_EFFNET_CN 0
+#define VDK_EFFNET_ER 1
+#define VDK_EFFNET_IR 2
+typedef struct vdk_effnetv2_block {
+  int kind;   /* VDK_EFFNET_CN, _ER or _IR */
+  int stride; /* 1 or 2 */
+  int cin, cout;
+  int mid;    /* ER, IR: the expanded width (IR: of the depthwise conv and the SE gate); CN: cout */
+  int se_rd;  /* IR: the SE bottleneck width */
+  vdk_resnet_conv conv;     /* CN conv / ER conv_exp: [out, 3, 3, Cinp] (vdk_conv2d_ex layout); IR conv_pw: [mid, cin] */
+  const float* dw_w;        /* IR: fp32 [9, mid] taps in (dy, dx) order */
+  const float* dw_b;        /* IR: [mid] */
+  const float* se_w1;       /* IR: fp32 [se_rd, mid] conv_reduce */
+  const float* se_b1;       /* [se_rd] */
+  const float* se_w2;       /* [mid, se_rd] conv_expand */
+  const float* se_b2;       /* [mid] */
+  vdk_resnet_conv conv_pwl; /* ER, IR: [cout, mid] */
+} vdk_effnetv2_block;
+typedef struct vdk_effnetv2_net {
+  int image_size; /* square input side, multiple of 32 */
+  int feat_dim;   /* embedding width, multiple of 8 */
+  int num_blocks;
+  int stem_ch;    /* conv_stem 3x3/s2 3 -> stem_ch, as a GEMM over zero-padded (kh, kw, c) rows: stem.w [stem_ch, 64] */
+  int head_ch;    /* conv_head 1x1 width (1280) */
+  vdk_resnet_conv stem;
+  vdk_effnetv2_block blocks[VDK_EFFNETV2_MAX_BLOCKS];
+  vdk_resnet_conv head; /* [head_ch, cout of the last block] */
+  const void* neck_w;   /* [feat_dim, h*w*head_ch] bf16, K order (h, w, c), BN2d/BN1d eval statistics folded in */
+  const float* neck_b;  /* [feat_dim] */
+} vdk_effnetv2_net;
+size_t vdk_effnetv2_workspace_bytes(const vdk_effnetv2_net* net, int batch);
+/* images: fp32 NCHW [batch,3,S,S]; embeddings: fp32 [batch, feat_dim], L2-normalised when l2_normalize != 0. */
+int vdk_effnetv2_forward(const vdk_effnetv2_net* net, const float* images, int batch, int l2_normalize, float* embeddings,
+                         void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_conv_ex_desc and vdk_effnetv2_net, in that order. */
+int vdk_effnetv2_struct_sizes(size_t* out, int n);
+/* The IR block's depthwise conv alone: y [B, Ho, Wo, C] bf16 = silu(dwconv3x3(x) + b) over x [B, H, W, C] bf16 (C a
+ * multiple of 32, <= 4096), stride 1 or 2 with TF-"same" padding, w fp32 [9, C]; and mean [B, C] fp32 = the spatial mean of
+ * the bf16 y, summed in a fixed order (bit-reproducible). */
+int vdk_dwconv3_silu(const void* x, int B, int H, int W, int C, int stride, const float* w, const float* b, void* y, float* mean,
+                     void* stream);
+/* The IR block's SE gate alone, on the depthwise output d [B, HW, C] bf16 and its mean [B, C] fp32 (C a multiple of 8,
+ * <= 4096): gate [B, C] fp32 = sigmoid(w2 silu(w1 mean + b1) + b2) (w1 [rd, C], w2 [C, rd]), then d = d * gate in place. */
+int vdk_effnet_se(void* d, const float* mean, int B, int HW, int C, int rd, const float* w1, const float* b1, const float* w2,
+                  const float* b2, float* gate, void* stream);
 
 /* ---- Swin Transformer V2 embedding forward (eval) ---------------------------------------------- */
 /* Replaces TimmWrapper.forward for timm's SwinTransformerV2 towers (swinv2_base_window8_256,

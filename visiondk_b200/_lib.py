@@ -16,6 +16,7 @@ VDK_ERR_INVALID, VDK_ERR_CUDA, VDK_ERR_WORKSPACE, VDK_ERR_OVERFLOW = -1, -2, -3,
 DTYPE_BF16, DTYPE_FP16, DTYPE_FP32 = 0, 1, 2
 EPI_NONE, EPI_GELU, EPI_SCALE_RESIDUAL, EPI_LAYERNORM, EPI_MUL_GELU_GRAD = 0, 1, 2, 3, 4
 EPI_RELU, EPI_RESIDUAL_RELU = 5, 6  # vdk_conv2d only
+EPI_SILU, EPI_SILU_RESIDUAL = 7, 8  # vdk_conv2d_ex only
 
 
 class HeadDesc(C.Structure):
@@ -95,6 +96,12 @@ SIGNATURES = {
     "vdk_bottleneck_struct_sizes": (_i, [_p, _i]),
     "vdk_stem_maxpool": (_i, [_p, _i, _i, _i, _i, _i, _p, _p]),
     "vdk_se_gate": (_i, [_p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "vdk_conv2d_ex": (_i, [_p, _p]),
+    "vdk_effnetv2_workspace_bytes": (_sz, [_p, _i]),
+    "vdk_effnetv2_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
+    "vdk_effnetv2_struct_sizes": (_i, [_p, _i]),
+    "vdk_dwconv3_silu": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "vdk_effnet_se": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
     "vdk_swinv2_workspace_bytes": (_sz, [_p, _i]),
     "vdk_swinv2_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
     "vdk_swinv2_struct_sizes": (_i, [_p, _i]),

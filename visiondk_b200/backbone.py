@@ -474,4 +474,7 @@ class BackboneFactory:
         if model_name.startswith("swinv2_"):  # Swin V2 towers: eval / extract path (visiondk_b200/swin.py); other variants refused
             from .swin import SwinV2Wrapper
             return SwinV2Wrapper(model_name=model_name, **self.backbone_param)
+        if model_name.startswith("tf_efficientnetv2_"):  # EfficientNetV2: eval / extract path (visiondk_b200/efficientnet.py)
+            from .efficientnet import EfficientNetV2Wrapper
+            return EfficientNetV2Wrapper(model_name=model_name, **self.backbone_param)
         return TimmWrapper(model_name=model_name, **self.backbone_param)

@@ -29,6 +29,15 @@ int launch_neck(const __nv_bfloat16* feats, int batch, int Kn, int F, const void
 int launch_neck_finalize(const float* slabs, int n_slabs, size_t slab_stride, int B, int F, const float* bias, int l2norm,
                          float* out, cudaStream_t s);
 
+// ---- CNN pieces of resnet.cu shared with effnet.cu ----
+// gate[b, :] = sigmoid(w2 act(w1 mean[b, :] + b1) + b2) in fp32, act = ReLU (silu_hidden 0) or SiLU (1); C + rd floats of
+// shared memory
+int launch_se_excite(const float* mean, int batch, int C, int rd, int silu_hidden, const float* w1, const float* b1,
+                     const float* w2, const float* b2, float* gate, cudaStream_t s);
+// explicit im2col rows of fp32 NCHW images: out[m][(dy k + dx) C + c] bf16, zero outside the image and from k*k*C to Kp
+int launch_patch_rows_nchw(const float* x, int B, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo, int Kp,
+                           __nv_bfloat16* out, cudaStream_t s);
+
 }  // namespace vdk
 
 namespace vdk {

@@ -33,6 +33,11 @@ constexpr int kConvIm2col = 2;  // k x k / stride-s convolution: A tiles gathere
 // grouped k x k convolution (vdk_conv2d_grouped, BN = 128): the N tile at n0 contracts over input channels n0 .. n0 + 127
 // only (whole groups, block-diagonal B), so its K block kb = (tap kb / 2, channels n0 + (kb % 2) * 64)
 constexpr int kConvGrouped = 3;
+// vdk_conv2d_ex (TF-"same" padded MBConv convolutions): as kConvDense / kConvIm2col, plus the SiLU epilogues.  cv_pad holds
+// the low padding of both axes (h | w << 8); the high padding only shapes the im2col map.  Cin a multiple of 8: a K block
+// still loads 64 channels of one tap, the channels past Cin arrive as TMA zero fill and meet zero weight columns.
+constexpr int kConvExDense = 4;
+constexpr int kConvExIm2col = 5;
 
 // The implicit-GEMM convolution modes (kConvIm2col) overlay their geometry on fields they do not use, so that the struct —
 // and with it the code of the plain GEMM instantiations — stays as it is.
@@ -101,6 +106,10 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// SiLU x / (1 + e^-x) with ex2.approx and rcp.approx (relative errors 2^-22 and 2^-23): relative error <= 1e-6 for
+// |x| <= 64 before the output rounding (the fp32 product -x log2(e) adds |x| 2^-24 to the exponent); x -> -0 for x < -126.
+__device__ __forceinline__ float silu_fast(float x) { return x * rcp_approx(1.f + ex2_approx(-1.4426950409f * x)); }
+
 // erf-GELU for the forward epilogue.  The fc1 epilogue applies 4C x tokens GELUs per block, so the activation has to
 // cost few issue slots and at most one SFU op per pair of elements or the epilogue, not the MMA, sets the pace.
 // y = 0.5 x (1 + tanh(u)), u = x (c1 + c3 x^2) with (c1, c3) refitted to the erf form (max |dev| 3.1e-4 instead of the
@@ -201,6 +210,15 @@ __device__ __forceinline__ void epi_pair(const GemmParams& p, float& x0, float& 
       x1 = fmaxf(x1 + r.y, 0.f);
     }
   }
+  if constexpr (kMode == kConvExDense || kMode == kConvExIm2col) {
+    if (p.epilogue == VDK_EPI_SILU) {
+      x0 = silu_fast(x0);
+      x1 = silu_fast(x1);
+    } else if (p.epilogue == VDK_EPI_SILU_RESIDUAL) {
+      x0 = silu_fast(x0) + r.x;
+      x1 = silu_fast(x1) + r.y;
+    }
+  }
 }
 
 // A warpgroup's box in ring slot `slot` is written: make it visible to the async proxy, let the leader hand it to TMA
@@ -245,6 +263,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   // A's column sums: two producer warps read every A stage as well and release it on the empty barrier
   constexpr bool kColSums = kTA && kMode == kGemmPlain;
   const bool col_sums = kColSums && p.partial_out && p.split_stride > 0 && p.col_sums != nullptr;
+  constexpr bool kConvEx = kMode == kConvExDense || kMode == kConvExIm2col;
 
 
   if (threadIdx.x == 0) {
@@ -253,7 +272,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     prefetch_tensormap(&map_d);
     if (p.aux != nullptr) prefetch_tensormap(&map_aux);
     if (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
-        (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU))
+        (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU) || (kConvEx && p.epilogue == VDK_EPI_SILU_RESIDUAL))
       prefetch_tensormap(&map_r);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
@@ -291,13 +310,18 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
           const int r = m0 - cn * p.cv_howo, ho = r / p.cv_wo;
           ch = ho * p.cv_stride - p.cv_pad;
           cw = (r - ho * p.cv_wo) * p.cv_stride - p.cv_pad;
+        } else if constexpr (kMode == kConvExIm2col) {
+          cn = m0 / p.cv_howo;
+          const int r = m0 - cn * p.cv_howo, ho = r / p.cv_wo;
+          ch = ho * p.cv_stride - (p.cv_pad & 0xff);
+          cw = (r - ho * p.cv_wo) * p.cv_stride - (p.cv_pad >> 8);
         }
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait_relaxed<true>(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kStageA;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          if constexpr (kMode == kConvIm2col) {  // K block kb = (filter tap, 64-channel block)
+          if constexpr (kMode == kConvIm2col || kMode == kConvExIm2col) {  // K block kb = (filter tap, 64-channel block)
             const int tap = kb / p.cv_cpb, c0 = (kb - tap * p.cv_cpb) * kBK, dy = tap / p.cv_kw;
             tma_load_im2col_4d(sa, &map_a, &full_bar[stage], c0, cw, ch, cn, static_cast<uint16_t>(tap - dy * p.cv_kw),
                                static_cast<uint16_t>(dy), kEvictNormal);
@@ -413,7 +437,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     const bool f32 = p.out_dtype == VDK_DTYPE_FP32;
     const int box_cols = f32 ? 32 : 64;
     const bool has_res = p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
-                         (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU);
+                         (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU) ||
+                         (kConvEx && p.epilogue == VDK_EPI_SILU_RESIDUAL);
     const bool reduce = p.partial_out && p.split_stride == 0;  // atomic split-K: TMA reduce-add into D
     int slot = 0;  // ring slot of the next box
     uint32_t res_phase = 0;
@@ -757,6 +782,64 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   return bf ? launch_gemm_major<128, true>(maps, p, ta, tb, s) : launch_gemm_major<128, false>(maps, p, ta, tb, s);
 }
 
+// The launcher behind vdk_conv2d and vdk_conv2d_ex, on arguments its entry point has validated.  pad: low / high padding
+// of the h and w axes.  ex: the vdk_conv2d_ex instantiations (SiLU epilogues, Cin a multiple of 8 with the weight's
+// channels padded to Cinp = a multiple of 64 for k x k / strided convolutions).
+struct ConvArgs {
+  const void* x;
+  const void* w;
+  const float* bias;
+  const void* residual;
+  void* y;
+  int B, H, W, Cin, Cout, kernel, stride, epilogue;
+  int pad_h[2], pad_w[2];
+  bool ex;
+};
+
+static int conv_launch(const ConvArgs& c, cudaStream_t s) {
+  const int Ho = (c.H + c.pad_h[0] + c.pad_h[1] - c.kernel) / c.stride + 1;
+  const int Wo = (c.W + c.pad_w[0] + c.pad_w[1] - c.kernel) / c.stride + 1;
+  const bool dense = c.kernel == 1 && c.stride == 1 && (c.pad_h[0] | c.pad_h[1] | c.pad_w[0] | c.pad_w[1]) == 0;
+  const int Cinp = dense ? c.Cin : (c.Cin + kBK - 1) / kBK * kBK;
+  const long long M = static_cast<long long>(c.B) * Ho * Wo;
+  const long long K = static_cast<long long>(c.kernel) * c.kernel * Cinp;
+  VDK_REQUIRE(M < (1ll << 31) && K < (1ll << 31), "vdk_conv2d: problem too large (M=%lld K=%lld)", M, K);
+  const bool wide = (c.Cout % 256 == 0) || c.Cout > 512;
+  CUtensorMap maps[5];  // A, B, D, aux_out (unused), residual
+  int rc = dense ? make_tma_2d_16bit(&maps[0], c.x, (uint64_t)M, (uint64_t)c.Cin, (uint64_t)c.Cin, kBM, kBK)
+         : c.ex  ? make_tma_im2col_16bit_pads(&maps[0], c.x, c.B, c.H, c.W, c.Cin, c.kernel, c.stride, c.pad_h, c.pad_w)
+                 : make_tma_im2col_16bit(&maps[0], c.x, c.B, c.H, c.W, c.Cin, c.kernel, c.stride, c.pad_h[0]);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_2d_16bit(&maps[1], c.w, (uint64_t)c.Cout, (uint64_t)K, (uint64_t)K, wide ? 256 : 128, kBK);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_epilogue_map(&maps[2], c.y, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
+  if (rc != VDK_OK) return rc;
+  maps[3] = maps[2];
+  maps[4] = maps[2];
+  if (c.residual != nullptr) {
+    rc = make_tma_epilogue_map(&maps[4], c.residual, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
+    if (rc != VDK_OK) return rc;
+  }
+  GemmParams p{};
+  p.M = static_cast<int>(M); p.N = c.Cout; p.K = static_cast<int>(K);
+  p.D = c.y; p.ldd = c.Cout; p.bias = c.bias; p.residual = c.residual; p.ldr = c.Cout;
+  p.out_dtype = VDK_DTYPE_BF16; p.epilogue = c.epilogue; p.split_k = 1;
+  p.cv_cpb = Cinp / kBK; p.cv_kw = c.kernel; p.cv_stride = c.stride;
+  p.cv_pad = c.ex ? (c.pad_h[0] | c.pad_w[0] << 8) : c.pad_h[0];
+  p.cv_wo = Wo; p.cv_howo = Ho * Wo;
+  // algorithmic bytes: the input once, the weights once, the output once, the residual once (FLOPs: the executed K)
+  ProfScope prof(kProfGemm, 2.0 * M * c.Cout * K,
+                 2.0 * (static_cast<double>(c.B) * c.H * c.W * c.Cin + static_cast<double>(c.Cout) * K + M * c.Cout) +
+                     (c.residual ? 2.0 * M * c.Cout : 0.0),
+                 s);
+  if (c.ex) {
+    if (dense) return wide ? launch_gemm<256, true, 0, 0, kConvExDense>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvExDense>(maps, p, s);
+    return wide ? launch_gemm<256, true, 0, 0, kConvExIm2col>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvExIm2col>(maps, p, s);
+  }
+  if (dense) return wide ? launch_gemm<256, true, 0, 0, kConvDense>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvDense>(maps, p, s);
+  return wide ? launch_gemm<256, true, 0, 0, kConvIm2col>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvIm2col>(maps, p, s);
+}
+
 int conv_run(const vdk_conv_desc& c, cudaStream_t s) {
   VDK_REQUIRE(c.x && c.w && c.y, "vdk_conv2d: null operand");
   VDK_REQUIRE(c.B > 0 && c.H > 0 && c.W > 0, "vdk_conv2d: empty input B=%d H=%d W=%d", c.B, c.H, c.W);
@@ -774,40 +857,36 @@ int conv_run(const vdk_conv_desc& c, cudaStream_t s) {
                   (reinterpret_cast<uintptr_t>(c.y) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.residual) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(c.bias) & 15) == 0,
               "vdk_conv2d: operands must be 16-byte aligned");
-  const int Ho = (c.H + 2 * c.pad - c.kernel) / c.stride + 1, Wo = (c.W + 2 * c.pad - c.kernel) / c.stride + 1;
-  const long long M = static_cast<long long>(c.B) * Ho * Wo;
-  const long long K = static_cast<long long>(c.kernel) * c.kernel * c.Cin;
-  VDK_REQUIRE(M < (1ll << 31) && K < (1ll << 31), "vdk_conv2d: problem too large (M=%lld K=%lld)", M, K);
-  const bool dense = c.kernel == 1 && c.stride == 1;  // pad < kernel: no padding either
-  const bool wide = (c.Cout % 256 == 0) || c.Cout > 512;
-  const int BN = wide ? 256 : 128;
-  CUtensorMap maps[5];  // A, B, D, aux_out (unused), residual
-  int rc = dense ? make_tma_2d_16bit(&maps[0], c.x, (uint64_t)M, (uint64_t)c.Cin, (uint64_t)c.Cin, kBM, kBK)
-                 : make_tma_im2col_16bit(&maps[0], c.x, c.B, c.H, c.W, c.Cin, c.kernel, c.stride, c.pad);
-  if (rc != VDK_OK) return rc;
-  rc = make_tma_2d_16bit(&maps[1], c.w, (uint64_t)c.Cout, (uint64_t)K, (uint64_t)K, BN, kBK);
-  if (rc != VDK_OK) return rc;
-  rc = make_tma_epilogue_map(&maps[2], c.y, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
-  if (rc != VDK_OK) return rc;
-  maps[3] = maps[2];
-  maps[4] = maps[2];
-  if (c.residual != nullptr) {
-    rc = make_tma_epilogue_map(&maps[4], c.residual, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
-    if (rc != VDK_OK) return rc;
-  }
-  GemmParams p{};
-  p.M = static_cast<int>(M); p.N = c.Cout; p.K = static_cast<int>(K);
-  p.D = c.y; p.ldd = c.Cout; p.bias = c.bias; p.residual = c.residual; p.ldr = c.Cout;
-  p.out_dtype = VDK_DTYPE_BF16; p.epilogue = c.epilogue; p.split_k = 1;
-  p.cv_cpb = c.Cin / kBK; p.cv_kw = c.kernel; p.cv_stride = c.stride; p.cv_pad = c.pad;
-  p.cv_wo = Wo; p.cv_howo = Ho * Wo;
-  // algorithmic bytes: the input once, the weights once, the output once, the residual once
-  ProfScope prof(kProfGemm, 2.0 * M * c.Cout * K,
-                 2.0 * (static_cast<double>(c.B) * c.H * c.W * c.Cin + static_cast<double>(c.Cout) * K + M * c.Cout) +
-                     (c.residual ? 2.0 * M * c.Cout : 0.0),
-                 s);
-  if (dense) return wide ? launch_gemm<256, true, 0, 0, kConvDense>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvDense>(maps, p, s);
-  return wide ? launch_gemm<256, true, 0, 0, kConvIm2col>(maps, p, s) : launch_gemm<128, true, 0, 0, kConvIm2col>(maps, p, s);
+  // pad < kernel: a 1x1 convolution has no padding
+  return conv_launch(ConvArgs{c.x, c.w, c.bias, c.residual, c.y, c.B, c.H, c.W, c.Cin, c.Cout, c.kernel, c.stride, c.epilogue,
+                              {c.pad, c.pad}, {c.pad, c.pad}, false},
+                     s);
+}
+
+int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t s) {
+  VDK_REQUIRE(c.x && c.w && c.y, "vdk_conv2d_ex: null operand");
+  VDK_REQUIRE(c.B > 0 && c.H > 0 && c.W > 0, "vdk_conv2d_ex: empty input B=%d H=%d W=%d", c.B, c.H, c.W);
+  VDK_REQUIRE(c.Cin > 0 && c.Cin % 8 == 0, "vdk_conv2d_ex: Cin must be a positive multiple of 8 (Cin=%d)", c.Cin);
+  VDK_REQUIRE(c.Cout > 0 && c.Cout % 8 == 0, "vdk_conv2d_ex: Cout must be a positive multiple of 8 (Cout=%d)", c.Cout);
+  VDK_REQUIRE(c.kernel >= 1 && c.kernel <= 16 && c.stride >= 1 && c.stride <= 8, "vdk_conv2d_ex: unsupported kernel=%d stride=%d",
+              c.kernel, c.stride);
+  // the low pads go to 8 bits of cv_pad each; every pad stays below the kernel, as the im2col map's corners need
+  VDK_REQUIRE(c.pad_h_lo >= 0 && c.pad_h_hi >= 0 && c.pad_w_lo >= 0 && c.pad_w_hi >= 0 && c.pad_h_lo < c.kernel &&
+                  c.pad_h_hi < c.kernel && c.pad_w_lo < c.kernel && c.pad_w_hi < c.kernel,
+              "vdk_conv2d_ex: pads (%d, %d, %d, %d) must lie in [0, kernel)", c.pad_h_lo, c.pad_h_hi, c.pad_w_lo, c.pad_w_hi);
+  VDK_REQUIRE(c.H + c.pad_h_lo + c.pad_h_hi >= c.kernel && c.W + c.pad_w_lo + c.pad_w_hi >= c.kernel,
+              "vdk_conv2d_ex: kernel larger than the padded input");
+  VDK_REQUIRE(c.epilogue == VDK_EPI_NONE || c.epilogue == VDK_EPI_SILU || c.epilogue == VDK_EPI_SILU_RESIDUAL,
+              "vdk_conv2d_ex: epilogue must be NONE, SILU or SILU_RESIDUAL (got %d)", c.epilogue);
+  VDK_REQUIRE((c.epilogue == VDK_EPI_SILU_RESIDUAL) == (c.residual != nullptr),
+              "vdk_conv2d_ex: a residual is given exactly with the SILU_RESIDUAL epilogue");
+  VDK_REQUIRE((reinterpret_cast<uintptr_t>(c.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.w) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(c.y) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.residual) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(c.bias) & 15) == 0,
+              "vdk_conv2d_ex: operands must be 16-byte aligned");
+  return conv_launch(ConvArgs{c.x, c.w, c.bias, c.residual, c.y, c.B, c.H, c.W, c.Cin, c.Cout, c.kernel, c.stride, c.epilogue,
+                              {c.pad_h_lo, c.pad_h_hi}, {c.pad_w_lo, c.pad_w_hi}, true},
+                     s);
 }
 
 int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t s) {
@@ -856,6 +935,11 @@ int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t s) {
 extern "C" int vdk_conv2d(const vdk_conv_desc* desc, void* stream) {
   VDK_REQUIRE(desc, "vdk_conv2d: null descriptor");
   return vdk::conv_run(*desc, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vdk_conv2d_ex(const vdk_conv_ex_desc* desc, void* stream) {
+  VDK_REQUIRE(desc, "vdk_conv2d_ex: null descriptor");
+  return vdk::conv_ex_run(*desc, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vdk_conv2d_grouped(const vdk_conv_desc* desc, int groups, void* stream) {

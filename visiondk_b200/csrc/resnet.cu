@@ -146,12 +146,13 @@ __global__ void __launch_bounds__(256) se_mean_kernel(const __nv_bfloat16* __res
   }
 }
 
-// se_excite: s[b, :] = sigmoid(fc2(ReLU(fc1(mean[b, :]) + b1)) + b2) in fp32, one block of 256 threads per image.  fc1: one
-// warp per hidden unit, lanes over C, a fixed shuffle tree; fc2: one thread per channel, sequential over rd.
+// se_excite: s[b, :] = sigmoid(fc2(act(fc1(mean[b, :]) + b1)) + b2) in fp32, one block of 256 threads per image; act is
+// ReLU (the legacy SENets) or SiLU (EfficientNetV2, silu_hidden).  fc1: one warp per hidden unit, lanes over C, a fixed
+// shuffle tree; fc2: one thread per channel, sequential over rd.
 __global__ void __launch_bounds__(256) se_excite_kernel(const float* __restrict__ mean, int C, int rd,
                                                         const float* __restrict__ w1, const float* __restrict__ b1,
                                                         const float* __restrict__ w2, const float* __restrict__ b2,
-                                                        float* __restrict__ s) {
+                                                        float* __restrict__ s, int silu_hidden) {
   extern __shared__ float se_smem[];
   float* m = se_smem;       // [C]
   float* hid = se_smem + C;  // [rd]
@@ -164,7 +165,10 @@ __global__ void __launch_bounds__(256) se_excite_kernel(const float* __restrict_
     for (int c = lane; c < C; c += 32) a = fmaf(wr[c], m[c], a);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-    if (lane == 0) hid[j] = fmaxf(a + b1[j], 0.f);
+    if (lane == 0) {
+      const float v = a + b1[j];
+      hid[j] = silu_hidden ? v / (1.f + expf(-v)) : fmaxf(v, 0.f);
+    }
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -208,6 +212,21 @@ __global__ void __launch_bounds__(256) se_scale_kernel(const __nv_bfloat16* __re
 static size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 
 static int grid_for(int64_t threads) { return static_cast<int>(std::min<int64_t>((threads + 255) / 256, 132 * 16)); }
+
+int launch_se_excite(const float* mean, int batch, int C, int rd, int silu_hidden, const float* w1, const float* b1,
+                     const float* w2, const float* b2, float* gate, cudaStream_t s) {
+  se_excite_kernel<<<batch, 256, (C + rd) * sizeof(float), s>>>(mean, C, rd, w1, b1, w2, b2, gate, silu_hidden);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
+int launch_patch_rows_nchw(const float* x, int B, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo, int Kp,
+                           __nv_bfloat16* out, cudaStream_t s) {
+  const int64_t threads = static_cast<int64_t>(B) * Ho * Wo * (Kp / 8);
+  patch_rows_kernel<float, true><<<grid_for(threads), 256, 0, s>>>(x, B, H, W, C, k, stride, pad, Ho, Wo, k * k * C, Kp, out);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
 
 static int check_net(const vdk_resnet_net* n) {
   VDK_REQUIRE(n, "vdk_resnet: null network");
@@ -356,10 +375,10 @@ namespace vdk {
 
 static int se_gate(const __nv_bfloat16* y, int batch, int HW, int C, int rd, const float* w1, const float* b1, const float* w2,
                    const float* b2, float* mean, float* sc, __nv_bfloat16* res, cudaStream_t s) {
+  int rc;
   se_mean_kernel<<<dim3(C / 64, batch), 256, 0, s>>>(y, HW, C, mean);
   VDK_CUDA_OK(cudaGetLastError());
-  se_excite_kernel<<<batch, 256, (C + rd) * sizeof(float), s>>>(mean, C, rd, w1, b1, w2, b2, sc);
-  VDK_CUDA_OK(cudaGetLastError());
+  if ((rc = launch_se_excite(mean, batch, C, rd, 0, w1, b1, w2, b2, sc, s)) != VDK_OK) return rc;
   const int64_t M = static_cast<int64_t>(batch) * HW;
   se_scale_kernel<<<grid_for(M * (C / 8)), 256, 0, s>>>(y, sc, M, HW, C, res);
   VDK_CUDA_OK(cudaGetLastError());

@@ -62,15 +62,23 @@ static EncodeIm2colFn encode_im2col_fn() {
 }
 
 int make_tma_im2col_16bit(CUtensorMap* map, const void* base, int B, int H, int W, int C, int kernel, int stride, int pad) {
+  if (C % 64 != 0) return fail(VDK_ERR_INVALID, "im2col TMA operand must have C a multiple of 64 (C=%d)", C);
+  const int p[2] = {pad, pad};
+  return make_tma_im2col_16bit_pads(map, base, B, H, W, C, kernel, stride, p, p);
+}
+
+int make_tma_im2col_16bit_pads(CUtensorMap* map, const void* base, int B, int H, int W, int C, int kernel, int stride,
+                               const int pad_h[2], const int pad_w[2]) {
   EncodeIm2colFn fn = encode_im2col_fn();
   if (!fn) return fail(VDK_ERR_CUDA, "cuTensorMapEncodeIm2col entry point unavailable (no CUDA driver?)");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || C % 64 != 0)
-    return fail(VDK_ERR_INVALID, "im2col TMA operand must be 16-byte aligned with C a multiple of 64 (C=%d)", C);
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || C % 8 != 0)
+    return fail(VDK_ERR_INVALID, "im2col TMA operand must be 16-byte aligned with C a multiple of 8 (C=%d)", C);
   cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
   cuuint64_t gstride[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  // window origins run from -pad to (size - 1) + pad - (kernel - 1) in steps of `stride`: exactly the output positions
-  const int lower[2] = {-pad, -pad};
-  const int upper[2] = {pad - (kernel - 1), pad - (kernel - 1)};
+  // window origins run from -lo to (size - 1) + hi - (kernel - 1) in steps of `stride`: exactly the output positions
+  // (the corners are ordered (w, h), like the tensor's dimensions)
+  const int lower[2] = {-pad_w[0], -pad_h[0]};
+  const int upper[2] = {pad_w[1] - (kernel - 1), pad_h[1] - (kernel - 1)};
   cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), gdim, gstride, lower, upper, 64, 128, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -226,6 +234,14 @@ int vdk_bottleneck_struct_sizes(size_t* out, int n) {
 // the same for the Swin V2 network: vdk_swinv2_net
 int vdk_swinv2_struct_sizes(size_t* out, int n) {
   const size_t sizes[] = {sizeof(vdk_swinv2_net)};
+  const int k = static_cast<int>(sizeof(sizes) / sizeof(sizes[0]));
+  for (int i = 0; i < n && i < k; ++i) out[i] = sizes[i];
+  return k;
+}
+
+// the same for the EfficientNetV2 surface: vdk_conv_ex_desc, vdk_effnetv2_net
+int vdk_effnetv2_struct_sizes(size_t* out, int n) {
+  const size_t sizes[] = {sizeof(vdk_conv_ex_desc), sizeof(vdk_effnetv2_net)};
   const int k = static_cast<int>(sizeof(sizes) / sizeof(sizes[0]));
   for (int i = 0; i < n && i < k; ++i) out[i] = sizes[i];
   return k;

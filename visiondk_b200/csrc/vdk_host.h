@@ -42,6 +42,10 @@ int make_tma_nhwc_16bit(CUtensorMap* map, const void* base, int B, int H, int W,
 // and zero padding: one load = 128 consecutive output pixels (row-major over (b, ho, wo), crossing rows and images) x 64
 // channels of one filter tap, 128-byte swizzle — the K-major A stage of the GEMM.  Taps outside the image read as zero.
 int make_tma_im2col_16bit(CUtensorMap* map, const void* base, int B, int H, int W, int C, int kernel, int stride, int pad);
+// The same with C a multiple of 8 and separate low / high padding per axis (pad_h = {top, bottom}, pad_w = {left, right}):
+// a load still takes 64 channels, those past C read as zero.
+int make_tma_im2col_16bit_pads(CUtensorMap* map, const void* base, int B, int H, int W, int C, int kernel, int stride,
+                               const int pad_h[2], const int pad_w[2]);
 
 // 4-D map over the qkv Linear's output, 16-bit [B][N][3H][D] (D contiguous), seen as (D, 3H, N, B): box = [1][box_rows][1]
 // [box_cols], box_cols 64 with 128-byte swizzle or 16 with 32-byte swizzle; out-of-bounds rows (past N) and columns (past D)
@@ -77,4 +81,6 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t stream);
 int conv_run(const vdk_conv_desc& c, cudaStream_t stream);
 // Internal form of vdk_conv2d_grouped (the ResNeXt / SE-ResNeXt forward).
 int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t stream);
+// Internal form of vdk_conv2d_ex (the EfficientNetV2 forward).
+int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t stream);
 }  // namespace vdk
