@@ -124,6 +124,17 @@ int vdk_conv2d(const vdk_conv_desc* desc, void* stream);
  * Cin == Cout a multiple of 128, groups >= 2 with cg dividing 128, epilogue VDK_EPI_RELU (no residual); kernel, stride and
  * pad as vdk_conv2d. */
 int vdk_conv2d_grouped(const vdk_conv_desc* desc, int groups, void* stream);
+/* Grouped form for any group widths: cgi = Cin / groups input and cgo = Cout / groups output channels per group (the
+ * split-attention conv of timm's ResNeSt, timm/layers/split_attn.py, has Cout = radix * Cin and cgi as small as 10).  The
+ * 128-channel output tile t (n0 = 128 t) contracts over the input channels of the groups its output channels belong to,
+ * from c_lo(t) = (n0 / cgo) * cgi rounded down to a multiple of 8 on, as cpb 64-channel blocks per tap; cpb is the maximum
+ * over the tiles of ceil(((min(n0 + 127, Cout - 1) / cgo + 1) * cgi - c_lo(t)) / 64).  desc->w is [Cout, kernel, kernel, cpb * 64] bf16:
+ * output channel n of group g = n / cgo holds timm's w[n, j + c_lo(n / 128) - g cgi] at column j when that index lies in
+ * [0, cgi), zero elsewhere.  Executed MACs: cpb * 64 / cgi times the useful ones.
+ * Cin and Cout multiples of 8, groups >= 1 dividing both; epilogue VDK_EPI_NONE, VDK_EPI_RELU or VDK_EPI_RESIDUAL_RELU;
+ * kernel, stride and pad as vdk_conv2d.  groups = 1 takes a 1x1 / stride-1 kernel only and runs as vdk_conv2d's plain GEMM
+ * with K = Cin (w [Cout, Cin]), so that Cin need not be a multiple of 64 (ResNeSt's conv3). */
+int vdk_conv2d_grouped_ex(const vdk_conv_desc* desc, int groups, void* stream);
 /* Extended form for TensorFlow-"same" padded MBConv networks (timm's tf_efficientnetv2_*, timm/models/_efficientnet_blocks.py
  * with Conv2dSame): separate low and high zero padding per axis, the SiLU epilogues, and Cin any multiple of 8.
  * Ho = (H + pad_h_lo + pad_h_hi - kernel) / stride + 1, likewise Wo.  1x1 / stride-1 / unpadded convolutions run as a plain
@@ -285,6 +296,59 @@ int vdk_dwconv3_silu(const void* x, int B, int H, int W, int C, int stride, cons
  * <= 4096): gate [B, C] fp32 = sigmoid(w2 silu(w1 mean + b1) + b2) (w1 [rd, C], w2 [C, rd]), then d = d * gate in place. */
 int vdk_effnet_se(void* d, const float* mean, int B, int HW, int C, int rd, const float* w1, const float* b1, const float* w2,
                   const float* b2, float* gate, void* stream);
+
+/* ---- ResNeSt embedding forward (eval) ------------------------------------------------------------ */
+/* Replaces TimmWrapper.forward for timm's ResNeSts with the width-32 deep stem (resnest14d, 26d, 50d, 50d_1s4x24d,
+ * 50d_4s2x40d; timm/models/resnest.py, timm/layers/split_attn.py; models/faceX/backbone/timm_wrapper.py:16-21, 30-38,
+ * 51-54) followed by F.normalize (face_model.py:139).  Stem, stem pool, avg_down shortcuts and neck as vdk_resnet_net with
+ * deep_stem = avg_down = 1.  A block of stage s (planes = 64 << s, gw = floor(planes * base_width / 64) * cardinality,
+ * C = gw, R = radix, A = attn[s]):
+ *   t = ReLU(conv1(x));  on stride-2 blocks with avd_first: t = AvgPool2d(3, 2, 1)(t)   (count_include_pad: / 9)
+ *   u = ReLU(conv(t)) 3x3 / s1 / p1, C -> R C, cardinality * R groups, output channel r C + c
+ *   gap = mean_hw sum_r u_r;  z = fc2(ReLU(fc1(gap)))  (1x1, cardinality groups, with bias; bn1 folded into fc1)
+ *   a[r, g C / card + i] = softmax_r z[g R C / card + r C / card + i]  (R > 1), sigmoid(z) (R = 1)
+ *   v = sum_r a_r u_r;  on stride-2 blocks without avd_first: v = AvgPool2d(3, 2, 1)(v)
+ *   out = ReLU(conv3(v) + shortcut(x)) */
+typedef struct vdk_resnest_block {
+  vdk_resnet_conv conv1; /* [gw, Cin] 1x1, bn1 folded */
+  vdk_resnet_conv conv2; /* the split conv [R gw, 3, 3, cpb * 64] in vdk_conv2d_grouped_ex's layout, bn0 folded */
+  const float* fc1_w;    /* fp32 [A, gw / cardinality], bn1 of the attention folded */
+  const float* fc1_b;    /* [A] */
+  const float* fc2_w;    /* fp32 [R gw, A / cardinality] */
+  const float* fc2_b;    /* [R gw] */
+  vdk_resnet_conv conv3; /* [4 planes, gw] 1x1, bn3 folded */
+  vdk_resnet_conv down;  /* as vdk_resnet_block (avg_down) */
+} vdk_resnest_block;
+typedef struct vdk_resnest_net {
+  int image_size;  /* square input side, multiple of 32 */
+  int feat_dim;    /* embedding width, multiple of 8 */
+  int depths[4];
+  int radix;       /* 1 .. 4 */
+  int cardinality; /* >= 1 */
+  int base_width;  /* gw of stage s = floor((64 << s) * base_width / 64) * cardinality, a multiple of 8 */
+  int avd_first;   /* 1: the stride-2 average pool before the split conv; 0: after the radix combine */
+  int attn[4];     /* A per stage: make_divisible(gw R / 4, 8, min 32), a multiple of cardinality */
+  vdk_resnet_conv stem[3]; /* the deep stem as vdk_resnet_net's */
+  vdk_resnest_block blocks[VDK_RESNET_MAX_BLOCKS]; /* stage-major */
+  const void* neck_w;  /* [feat_dim, h*w*2048] bf16, as vdk_resnet_net */
+  const float* neck_b; /* [feat_dim] */
+} vdk_resnest_net;
+size_t vdk_resnest_workspace_bytes(const vdk_resnest_net* net, int batch);
+/* images: fp32 NCHW [batch,3,S,S]; embeddings: fp32 [batch, feat_dim], L2-normalised when l2_normalize != 0. */
+int vdk_resnest_forward(const vdk_resnest_net* net, const float* images, int batch, int l2_normalize, float* embeddings,
+                        void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_resnest_net. */
+int vdk_resnest_struct_sizes(size_t* out, int n);
+/* The forward's split-attention gate alone, on u = the split conv's output [B, HW, R C] bf16 (C a multiple of 8, R C <= 4096,
+ * 1 <= R <= 4; A a multiple of cardinality, cardinality dividing C): gap [B, C] fp32 = mean_hw sum_r u_r (fixed order),
+ * attn [B, R C] fp32 = a[r, c] at r C + c as above, then v [B, Ho, Wo, C] bf16 = sum_r a_r u_r, over the H x W map
+ * (HW = H W) when pool == 0, or AvgPool2d(3, 2, 1, count_include_pad) of it when pool == 1 (Ho = (H - 1) / 2 + 1). */
+int vdk_split_attn_gate(const void* u, int B, int H, int W, int C, int radix, int cardinality, int A, const float* fc1_w,
+                        const float* fc1_b, const float* fc2_w, const float* fc2_b, float* gap, float* attn, int pool, void* v,
+                        void* stream);
+/* AvgPool2d(3, 2, padding 1, count_include_pad=True) over NHWC bf16 x [B, H, W, C] (C a multiple of 8) into
+ * y [B, (H - 1) / 2 + 1, (W - 1) / 2 + 1, C]: the fp32 sum of the nine taps (zeros outside) / 9, rounded once. */
+int vdk_avgpool3s2(const void* x, int B, int H, int W, int C, void* y, void* stream);
 
 /* ---- Swin Transformer V2 embedding forward (eval) ---------------------------------------------- */
 /* Replaces TimmWrapper.forward for timm's SwinTransformerV2 towers (swinv2_base_window8_256,

@@ -97,6 +97,12 @@ SIGNATURES = {
     "vdk_stem_maxpool": (_i, [_p, _i, _i, _i, _i, _i, _p, _p]),
     "vdk_se_gate": (_i, [_p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "vdk_conv2d_ex": (_i, [_p, _p]),
+    "vdk_conv2d_grouped_ex": (_i, [_p, _i, _p]),
+    "vdk_resnest_workspace_bytes": (_sz, [_p, _i]),
+    "vdk_resnest_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
+    "vdk_resnest_struct_sizes": (_i, [_p, _i]),
+    "vdk_split_attn_gate": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _i, _p, _p]),
+    "vdk_avgpool3s2": (_i, [_p, _i, _i, _i, _i, _p, _p]),
     "vdk_effnetv2_workspace_bytes": (_sz, [_p, _i]),
     "vdk_effnetv2_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
     "vdk_effnetv2_struct_sizes": (_i, [_p, _i]),

@@ -471,6 +471,9 @@ class BackboneFactory:
         from .senet import SENET_ARCHS, SENetWrapper
         if model_name in SENET_ARCHS:  # legacy SE-ResNets / SE-ResNeXts: eval / extract path (visiondk_b200/senet.py)
             return SENetWrapper(model_name=model_name, **self.backbone_param)
+        from .resnest import RESNEST_ARCHS, ResNeStWrapper
+        if model_name in RESNEST_ARCHS:  # ResNeSts: eval / extract path (visiondk_b200/resnest.py)
+            return ResNeStWrapper(model_name=model_name, **self.backbone_param)
         if model_name.startswith("swinv2_"):  # Swin V2 towers: eval / extract path (visiondk_b200/swin.py); other variants refused
             from .swin import SwinV2Wrapper
             return SwinV2Wrapper(model_name=model_name, **self.backbone_param)

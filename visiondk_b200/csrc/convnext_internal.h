@@ -37,6 +37,11 @@ int launch_se_excite(const float* mean, int batch, int C, int rd, int silu_hidde
 // explicit im2col rows of fp32 NCHW images: out[m][(dy k + dx) C + c] bf16, zero outside the image and from k*k*C to Kp
 int launch_patch_rows_nchw(const float* x, int B, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo, int Kp,
                            __nv_bfloat16* out, cudaStream_t s);
+// the same rows of NHWC bf16 maps (the deep stem's second and third convs)
+int launch_patch_rows_nhwc(const __nv_bfloat16* x, int B, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo, int Kp,
+                           __nv_bfloat16* out, cudaStream_t s);
+// timm's ResNet stem pool MaxPool2d(3, 2, padding 1) over NHWC bf16 (C a multiple of 8)
+int launch_stem_maxpool(const __nv_bfloat16* x, int B, int H, int W, int C, __nv_bfloat16* y, cudaStream_t s);
 
 }  // namespace vdk
 

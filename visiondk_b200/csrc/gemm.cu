@@ -17,6 +17,7 @@
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
 
+#include <algorithm>
 #include <cstdlib>
 
 namespace vdk {
@@ -38,6 +39,12 @@ constexpr int kConvGrouped = 3;
 // still loads 64 channels of one tap, the channels past Cin arrive as TMA zero fill and meet zero weight columns.
 constexpr int kConvExDense = 4;
 constexpr int kConvExIm2col = 5;
+// grouped k x k convolution with any group widths (vdk_conv2d_grouped_ex, BN = 128; ResNeSt's split-attention conv,
+// Cout = radix * Cin): the N tile at n0 contracts over the input channels of the groups its output channels belong to,
+// from c_lo = (n0 / cv_cg_out) * cv_cg_in rounded down to a multiple of 8 on (the im2col load's channel coordinate must
+// be 16-byte aligned), as cv_cpb 64-channel blocks per tap (channels past Cin are TMA zero fill; the packed weight is
+// zero outside each output channel's own group)
+constexpr int kConvGroupedEx = 6;
 
 // The implicit-GEMM convolution modes (kConvIm2col) overlay their geometry on fields they do not use, so that the struct —
 // and with it the code of the plain GEMM instantiations — stays as it is.
@@ -58,10 +65,16 @@ struct GemmParams {
     };
   };
   const void* residual;  // SCALE_RESIDUAL: added; MUL_GELU_GRAD: the saved 16-bit pre-activation whose GELU' scales the output
-  int ldr;
+  union {
+    int ldr;        // host side only: the kernel reads the residual through its TMA map
+    int cv_cg_out;  // kConvGroupedEx: output channels per group
+  };
   int out_dtype;
   int epilogue;
-  float ln_eps;
+  union {
+    float ln_eps;
+    int cv_cg_in;  // kConvGroupedEx: input channels per group
+  };
   int split_k;  // > 1: each tile's K range is split over split_k work items, fp32 partials are atomically added
   union {
     long long split_stride;  // > 0: split s writes its partial tile to D + s*split_stride with plain stores (deterministic)
@@ -305,7 +318,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         // im2col: the tile's first output pixel, as the input position of its filter window's top-left tap.  The TMA unit
         // walks the next 127 pixels through the map's bounding box (across rows and images); rows past M read as zero.
         int cw = 0, ch = 0, cn = 0;
-        if constexpr (kMode == kConvIm2col || kMode == kConvGrouped) {
+        if constexpr (kMode == kConvIm2col || kMode == kConvGrouped || kMode == kConvGroupedEx) {
           cn = m0 / p.cv_howo;
           const int r = m0 - cn * p.cv_howo, ho = r / p.cv_wo;
           ch = ho * p.cv_stride - p.cv_pad;
@@ -327,6 +340,11 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                                static_cast<uint16_t>(dy), kEvictNormal);
           } else if constexpr (kMode == kConvGrouped) {  // cv_cpb = 2: the tile's own 128 input channels at every tap
             const int tap = kb >> 1, c0 = n0 + (kb & 1) * kBK, dy = tap / p.cv_kw;
+            tma_load_im2col_4d(sa, &map_a, &full_bar[stage], c0, cw, ch, cn, static_cast<uint16_t>(tap - dy * p.cv_kw),
+                               static_cast<uint16_t>(dy), kEvictNormal);
+          } else if constexpr (kMode == kConvGroupedEx) {  // K block kb = (tap, 64-channel block from the tile's c_lo)
+            const int tap = kb / p.cv_cpb, dy = tap / p.cv_kw;
+            const int c0 = ((n0 / p.cv_cg_out * p.cv_cg_in) & ~7) + (kb - tap * p.cv_cpb) * kBK;
             tma_load_im2col_4d(sa, &map_a, &full_bar[stage], c0, cw, ch, cn, static_cast<uint16_t>(tap - dy * p.cv_kw),
                                static_cast<uint16_t>(dy), kEvictNormal);
           } else if (kTA) {  // [K,M] storage: 64-wide M blocks x 64 contraction rows, 8 KB each
@@ -930,6 +948,78 @@ int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t s) {
   return launch_gemm<128, true, 0, 0, kConvGrouped>(maps, p, s);
 }
 
+int conv_grouped_ex_cpb(int Cin, int Cout, int groups) {
+  const int cgi = Cin / groups, cgo = Cout / groups;
+  int cpb = 1;
+  for (int n0 = 0; n0 < Cout; n0 += 128) {
+    const int n1 = std::min(n0 + 128, Cout) - 1;
+    const int span = (n1 / cgo + 1) * cgi - ((n0 / cgo * cgi) & ~7);  // from the tile's 16-byte-aligned c_lo
+    cpb = std::max(cpb, (span + kBK - 1) / kBK);
+  }
+  return cpb;
+}
+
+int conv_grouped_ex_run(const vdk_conv_desc& c, int groups, cudaStream_t s) {
+  VDK_REQUIRE(c.x && c.w && c.y, "vdk_conv2d_grouped_ex: null operand");
+  VDK_REQUIRE(c.B > 0 && c.H > 0 && c.W > 0, "vdk_conv2d_grouped_ex: empty input B=%d H=%d W=%d", c.B, c.H, c.W);
+  VDK_REQUIRE(c.Cin > 0 && c.Cin % 8 == 0 && c.Cout > 0 && c.Cout % 8 == 0,
+              "vdk_conv2d_grouped_ex: Cin and Cout must be positive multiples of 8 (Cin=%d Cout=%d)", c.Cin, c.Cout);
+  VDK_REQUIRE(groups >= 1 && c.Cin % groups == 0 && c.Cout % groups == 0,
+              "vdk_conv2d_grouped_ex: groups=%d must be >= 1 and divide Cin=%d and Cout=%d", groups, c.Cin, c.Cout);
+  VDK_REQUIRE(c.kernel >= 1 && c.kernel <= 16 && c.stride >= 1 && c.stride <= 8 && c.pad >= 0 && c.pad < c.kernel,
+              "vdk_conv2d_grouped_ex: unsupported kernel=%d stride=%d pad=%d", c.kernel, c.stride, c.pad);
+  VDK_REQUIRE(c.H + 2 * c.pad >= c.kernel && c.W + 2 * c.pad >= c.kernel,
+              "vdk_conv2d_grouped_ex: kernel larger than the padded input");
+  VDK_REQUIRE(c.epilogue == VDK_EPI_NONE || c.epilogue == VDK_EPI_RELU || c.epilogue == VDK_EPI_RESIDUAL_RELU,
+              "vdk_conv2d_grouped_ex: epilogue must be NONE, RELU or RESIDUAL_RELU (got %d)", c.epilogue);
+  VDK_REQUIRE((c.epilogue == VDK_EPI_RESIDUAL_RELU) == (c.residual != nullptr),
+              "vdk_conv2d_grouped_ex: a residual is given exactly with the RESIDUAL_RELU epilogue");
+  VDK_REQUIRE((reinterpret_cast<uintptr_t>(c.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.w) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(c.y) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.residual) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(c.bias) & 15) == 0,
+              "vdk_conv2d_grouped_ex: operands must be 16-byte aligned");
+  if (groups == 1) {
+    // a dense 1x1 / stride-1 convolution: the plain GEMM over [B*H*W, Cin], K = Cin (TMA zero-fills the last K block)
+    VDK_REQUIRE(c.kernel == 1 && c.stride == 1,
+                "vdk_conv2d_grouped_ex: groups=1 takes a 1x1 / stride-1 kernel only (kernel=%d stride=%d)", c.kernel, c.stride);
+    return conv_launch(ConvArgs{c.x, c.w, c.bias, c.residual, c.y, c.B, c.H, c.W, c.Cin, c.Cout, 1, 1, c.epilogue, {0, 0}, {0, 0},
+                                false},
+                       s);
+  }
+  const int Ho = (c.H + 2 * c.pad - c.kernel) / c.stride + 1, Wo = (c.W + 2 * c.pad - c.kernel) / c.stride + 1;
+  const int cpb = conv_grouped_ex_cpb(c.Cin, c.Cout, groups);
+  const long long M = static_cast<long long>(c.B) * Ho * Wo;
+  const long long K = static_cast<long long>(c.kernel) * c.kernel * cpb * kBK;  // executed per output channel
+  VDK_REQUIRE(M < (1ll << 31), "vdk_conv2d_grouped_ex: problem too large (M=%lld)", M);
+  CUtensorMap maps[5];  // A, B, D, aux_out (unused), residual
+  const int pads[2] = {c.pad, c.pad};
+  int rc = make_tma_im2col_16bit_pads(&maps[0], c.x, c.B, c.H, c.W, c.Cin, c.kernel, c.stride, pads, pads);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_2d_16bit(&maps[1], c.w, (uint64_t)c.Cout, (uint64_t)K, (uint64_t)K, 128, kBK);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_epilogue_map(&maps[2], c.y, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
+  if (rc != VDK_OK) return rc;
+  maps[3] = maps[2];
+  maps[4] = maps[2];
+  if (c.residual != nullptr) {
+    rc = make_tma_epilogue_map(&maps[4], c.residual, 2, (uint64_t)M, (uint64_t)c.Cout, (uint64_t)c.Cout, 1, 0);
+    if (rc != VDK_OK) return rc;
+  }
+  GemmParams p{};
+  p.M = static_cast<int>(M); p.N = c.Cout; p.K = static_cast<int>(K);
+  p.D = c.y; p.ldd = c.Cout; p.bias = c.bias; p.residual = c.residual;
+  p.out_dtype = VDK_DTYPE_BF16; p.epilogue = c.epilogue; p.split_k = 1;
+  p.cv_cpb = cpb; p.cv_kw = c.kernel; p.cv_stride = c.stride; p.cv_pad = c.pad;
+  p.cv_wo = Wo; p.cv_howo = Ho * Wo;
+  p.cv_cg_in = c.Cin / groups; p.cv_cg_out = c.Cout / groups;
+  // executed FLOPs; the useful ones are a factor cpb * 64 / (Cin / groups) fewer
+  ProfScope prof(kProfGemm, 2.0 * M * c.Cout * K,
+                 2.0 * (static_cast<double>(c.B) * c.H * c.W * c.Cin + static_cast<double>(c.Cout) * K + M * c.Cout) +
+                     (c.residual ? 2.0 * M * c.Cout : 0.0),
+                 s);
+  return launch_gemm<128, true, 0, 0, kConvGroupedEx>(maps, p, s);
+}
+
 }  // namespace vdk
 
 extern "C" int vdk_conv2d(const vdk_conv_desc* desc, void* stream) {
@@ -945,6 +1035,11 @@ extern "C" int vdk_conv2d_ex(const vdk_conv_ex_desc* desc, void* stream) {
 extern "C" int vdk_conv2d_grouped(const vdk_conv_desc* desc, int groups, void* stream) {
   VDK_REQUIRE(desc, "vdk_conv2d_grouped: null descriptor");
   return vdk::conv_grouped_run(*desc, groups, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vdk_conv2d_grouped_ex(const vdk_conv_desc* desc, int groups, void* stream) {
+  VDK_REQUIRE(desc, "vdk_conv2d_grouped_ex: null descriptor");
+  return vdk::conv_grouped_ex_run(*desc, groups, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vdk_gemm_effective_splits(int K, int split_k) {

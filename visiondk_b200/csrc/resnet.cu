@@ -552,6 +552,22 @@ extern "C" int vdk_bottleneck_forward(const vdk_bottleneck_net* net, const float
                      up256(z.act * 2), embeddings, s);
 }
 
+namespace vdk {
+
+int launch_patch_rows_nhwc(const __nv_bfloat16* x, int B, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo, int Kp,
+                           __nv_bfloat16* out, cudaStream_t s) {
+  const int64_t threads = static_cast<int64_t>(B) * Ho * Wo * (Kp / 8);
+  patch_rows_kernel<__nv_bfloat16, false><<<grid_for(threads), 256, 0, s>>>(x, B, H, W, C, k, stride, pad, Ho, Wo, k * k * C, Kp, out);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
+int launch_stem_maxpool(const __nv_bfloat16* x, int B, int H, int W, int C, __nv_bfloat16* y, cudaStream_t s) {
+  return stem_pool_run(x, B, H, W, C, VDK_STEM_POOL_PAD1, y, s);
+}
+
+}  // namespace vdk
+
 // Kernel-level entry points of the pieces above, for their tests.
 extern "C" int vdk_stem_maxpool(const void* x, int B, int H, int W, int C, int mode, void* y, void* stream) {
   VDK_REQUIRE(x && y && B > 0 && H >= 3 && W >= 3 && C > 0 && C % 8 == 0, "vdk_stem_maxpool: bad arguments");

@@ -83,4 +83,7 @@ int conv_run(const vdk_conv_desc& c, cudaStream_t stream);
 int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t stream);
 // Internal form of vdk_conv2d_ex (the EfficientNetV2 forward).
 int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t stream);
+// Internal form of vdk_conv2d_grouped_ex (the ResNeSt forward), and the 64-channel blocks per tap its packed weight holds.
+int conv_grouped_ex_run(const vdk_conv_desc& c, int groups, cudaStream_t stream);
+int conv_grouped_ex_cpb(int Cin, int Cout, int groups);
 }  // namespace vdk

@@ -108,6 +108,7 @@ class _ResBlockC(C.Structure):
 
 class ResNetNetC(C.Structure):
     """vdk_resnet_net (include/vdk_b200.h)."""
+    api = "vdk_resnet"  # prefix of the network's workspace / forward entry points
     _fields_ = [
         ("image_size", C.c_int), ("feat_dim", C.c_int), ("depths", C.c_int * 4), ("base_width", C.c_int),
         ("deep_stem", C.c_int), ("avg_down", C.c_int), ("stem", _ConvC * 3), ("blocks", _ResBlockC * 64),
@@ -122,6 +123,7 @@ class _BottleneckBlockC(C.Structure):
 
 class BottleneckNetC(C.Structure):
     """vdk_bottleneck_net (include/vdk_b200.h)."""
+    api = "vdk_bottleneck"
     _fields_ = [
         ("image_size", C.c_int), ("feat_dim", C.c_int), ("depths", C.c_int * 4), ("width", C.c_int), ("cardinality", C.c_int),
         ("stride_on_conv1", C.c_int), ("stem_pool", C.c_int), ("deep_stem", C.c_int), ("avg_down", C.c_int),
@@ -195,7 +197,7 @@ class ResNetWrapper(nn.Module):
         net = self._pack(x.device)
         B = x.shape[0]
         out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
-        api = "vdk_bottleneck" if isinstance(net, BottleneckNetC) else "vdk_resnet"
+        api = net.api
         need = getattr(lib, f"{api}_workspace_bytes")(C.byref(net), B)
         if need == 0:
             raise RuntimeError(f"{api}_workspace_bytes: invalid network")
