@@ -15,14 +15,12 @@ parameter containers only; their own forward() is never used on the hot path, an
 from __future__ import annotations
 
 import ctypes as C
-import os
-import warnings
-from typing import Dict, Optional
 
 import torch
 import torch.nn as nn
 
 from . import _lib
+from .wrapper import BackboneWrapper, cnn_neck
 
 CONVNEXT_ARCHS = {
     "convnext_atto": ((2, 2, 6, 2), (40, 80, 160, 320)),
@@ -92,21 +90,6 @@ class ConvNeXtParams(nn.Module):
                 nn.init.zeros_(m.bias)
 
 
-@torch.no_grad()
-def fold_cnn_neck(output_layer: nn.Sequential, c_last: int, hw: int, feat_dim: int, device):
-    """The CNN neck BatchNorm2d -> Flatten -> Linear -> BatchNorm1d (eval statistics) as one Linear over the final map in
-    (h, w, c) order: (weight [feat_dim, hw*hw*c_last], bias [feat_dim]) in fp64."""
-    bn2, lin, bn1 = output_layer[0], output_layer[2], output_layer[3]
-    s2 = (bn2.weight.double() / torch.sqrt(bn2.running_var.double() + bn2.eps)).to(device)
-    t2 = (bn2.bias.double().to(device) - bn2.running_mean.double().to(device) * s2)
-    s1 = (bn1.weight.double() / torch.sqrt(bn1.running_var.double() + bn1.eps)).to(device)
-    w = lin.weight.detach().double().to(device).reshape(feat_dim, c_last, hw, hw)
-    bias = lin.bias.detach().double().to(device) + (w * t2.view(1, -1, 1, 1)).sum(dim=(1, 2, 3))
-    bias = s1 * (bias - bn1.running_mean.double().to(device)) + bn1.bias.double().to(device)
-    w = w * s2.view(1, -1, 1, 1) * s1.view(-1, 1, 1, 1)
-    return w.permute(0, 2, 3, 1).reshape(feat_dim, hw * hw * c_last), bias
-
-
 class _BlockC(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("dw_w", "dw_b", "ln_w", "ln_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b", "gamma",
                                           "dw_w_flip", "fc2_wg")]
@@ -137,6 +120,7 @@ class _DownC(C.Structure):
 
 
 class ConvNeXtNetC(C.Structure):
+    api = "vdk_convnext"
     _fields_ = [
         ("image_size", C.c_int), ("feat_dim", C.c_int), ("depths", C.c_int * 4), ("dims", C.c_int * 4),
         ("stem_w", C.c_void_p), ("stem_b", C.c_void_p), ("stem_ln_w", C.c_void_p), ("stem_ln_b", C.c_void_p),
@@ -145,62 +129,27 @@ class ConvNeXtNetC(C.Structure):
     ]
 
 
-class TimmWrapper(nn.Module):
+class TimmWrapper(BackboneWrapper):
     """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper (ConvNeXt family)."""
+
+    _dropped = ("head.fc",)
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, dims=None,
                  **kwargs):
-        super().__init__()
         if depths is None:
             if model_name not in CONVNEXT_ARCHS:
                 raise ValueError(f"backbone '{model_name}' is not built for H100 yet; available: {sorted(CONVNEXT_ARCHS)}")
             depths, dims = CONVNEXT_ARCHS[model_name]
         if image_size % 32 != 0:
             raise ValueError("image_size must be a multiple of 32")
-        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = ConvNeXtParams(depths, dims)
         hw = image_size // 32
-        self.output_layer = nn.Sequential(nn.BatchNorm2d(dims[-1]), nn.Flatten(1),
-                                          nn.Linear(dims[-1] * hw * hw, feat_dim), nn.BatchNorm1d(feat_dim))
-        self._packed: Optional[Dict] = None
-        self._packed_key = None
-        self._ws = None
-        self._train = None
-        if pretrained:
-            self._load_pretrained(model_name)
+        super().__init__(model_name, feat_dim, image_size, ConvNeXtParams(depths, dims),
+                         cnn_neck(dims[-1], dims[-1] * hw * hw, feat_dim), pretrained)
 
-    # ---- reference surface ---------------------------------------------------------------------
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.training:
-            return _ConvNeXtTrainFn.apply(self, x, *self._ordered_params())
-        return self.embed(x, l2_normalize=False)
-
-    # ---- H100 path -------------------------------------------------------------------------------
-    @torch.no_grad()
-    def embed(self, x: torch.Tensor, l2_normalize: bool = False) -> torch.Tensor:
-        """[B,3,S,S] fp32 (NCHW, already normalised like the reference's transforms) -> fp32 [B, feat_dim]."""
-        lib = _lib.load()
-        if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.TimmWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
-        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
-            raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
-        x = x.contiguous().float()
-        net = self._pack(x.device)
-        B = x.shape[0]
-        out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
-        need = lib.vdk_convnext_workspace_bytes(C.byref(net), B)
-        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
-            self._ws = torch.empty((need,), dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(lib.vdk_convnext_forward(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(),
-                                                self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()),
-                       "vdk_convnext_forward")
-        return out
+    def _train_refusal(self) -> str:
+        return ""
 
     # ---- training path (csrc/convnext_train.cu) ------------------------------------------------------
-    def _ordered_params(self):
-        return [p for _, p in self.named_parameters()]
-
     def _tensors_struct(self, get) -> ConvNeXtTensorsC:
         """vdk_convnext_tensors whose pointers are `get(name)` for every parameter / BN buffer name."""
         t = ConvNeXtTensorsC()
@@ -249,12 +198,7 @@ class TimmWrapper(nn.Module):
 
     def _train_structs(self, device):
         st = self._train_state(device)
-        named = dict(self.named_parameters())
-        named.update(dict(self.named_buffers()))
-        for n, t in named.items():
-            if t.is_floating_point() and (t.device != device or t.dtype != torch.float32 or not t.is_contiguous()):
-                raise RuntimeError(f"{n}: training needs contiguous fp32 parameters on {device}")
-        params = self._tensors_struct(lambda n: named[n].data_ptr())
+        params = self._master_tensors(device)
         bufs, m = st["bufs"], self.model
         net = ConvNeXtNetC()
         net.image_size, net.feat_dim = self.image_size, self.feat_dim
@@ -301,49 +245,6 @@ class TimmWrapper(nn.Module):
         st["last"] = (net, params, B)
         return out
 
-    def _train_backward(self, dout: torch.Tensor):
-        """Gradients of every parameter.  When the parameters already own fp32 `.grad` buffers (the fused optimizer
-        re-points them into its flat gradient buffer) the kernels accumulate straight into those and autograd receives
-        None; otherwise the gradients are produced in a scratch buffer and returned."""
-        lib = _lib.load()
-        st = self._train
-        net, params, B = st["last"]
-        plist = list(self.named_parameters())
-        direct = all(p.grad is not None and p.grad.dtype == torch.float32 and p.grad.is_contiguous() and
-                     p.grad.device == dout.device for _, p in plist)
-        if direct:
-            ptrs = {n: p.grad.data_ptr() for n, p in plist}
-        else:
-            total = sum(p.numel() for _, p in plist)
-            if st["gflat"] is None or st["gflat"].numel() != total:
-                st["gflat"] = torch.empty((total,), dtype=torch.float32, device=dout.device)
-            gflat = st["gflat"]
-            gflat.zero_()
-            offs, off = {}, 0
-            for n, p in plist:
-                offs[n] = off
-                off += p.numel()
-            ptrs = {n: gflat.data_ptr() + 4 * offs[n] for n, _ in plist}
-        grads = self._tensors_struct(lambda n: ptrs.get(n, 0))
-        dout = dout.contiguous().float()
-        hook = getattr(self, "grad_section_hook", None)
-        with torch.cuda.device(dout.device):
-            if hook is not None and direct:
-                # DDP overlap: the backward runs in a few unit ranges; after each one the parameters whose gradients are now
-                # final are handed to the hook (FaceTrainer starts their all-reduce while the next range computes)
-                for (u0, u1), names in self.backward_sections():
-                    _lib.check(lib.vdk_convnext_train_backward_range(C.byref(net), C.byref(params), C.byref(grads), dout.data_ptr(),
-                                                                     B, st["ws"].data_ptr(), st["ws"].numel(), _lib.stream_ptr(),
-                                                                     u0, u1), "vdk_convnext_train_backward_range")
-                    hook(names)
-            else:
-                _lib.check(lib.vdk_convnext_train_backward(C.byref(net), C.byref(params), C.byref(grads), dout.data_ptr(), B,
-                                                           st["ws"].data_ptr(), st["ws"].numel(), _lib.stream_ptr()),
-                           "vdk_convnext_train_backward")
-        if direct:
-            return [None] * len(plist)
-        return [gflat[offs[n]:offs[n] + p.numel()].view_as(p) for n, p in plist]
-
     def backward_sections(self):
         """[((unit_begin, unit_end), [parameter names whose gradients are final after that range]), ...] in execution order
         (units: include/vdk_b200.h, vdk_convnext_train_backward_range).  Four ranges: neck + head norm + stage 4; the second
@@ -375,80 +276,34 @@ class TimmWrapper(nn.Module):
         return [x for x in sec if x[0][0] < x[0][1]]
 
     # ---- weight packing --------------------------------------------------------------------------
-    def _version_key(self, device):
-        return (str(device),) + tuple(int(t._version) for t in list(self.parameters()) + list(self.buffers()))
-
-    def _pack(self, device) -> ConvNeXtNetC:
+    def _build(self, p) -> ConvNeXtNetC:
         """Kernel-side layouts (include/vdk_b200.h): bf16 GEMM weights, fp32 vectors, depthwise taps [49][C],
         downsample conv K order (kh,kw,cin), neck with BN2d/BN1d eval statistics folded and K order (h,w,c)."""
-        key = self._version_key(device)
-        if self._packed is not None and self._packed_key == key:
-            return self._packed["net"]
-        keep = []
-
-        def f32(t):
-            t = t.detach().to(device, torch.float32).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def bf16(t):
-            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
-            keep.append(t)
-            return t.data_ptr()
-
         m, net = self.model, ConvNeXtNetC()
         net.image_size, net.feat_dim = self.image_size, self.feat_dim
         for i in range(4):
             net.depths[i], net.dims[i] = m.depths[i], m.dims[i]
-        net.stem_w = bf16(m.stem[0].weight.reshape(m.dims[0], 48))
-        net.stem_b, net.stem_ln_w, net.stem_ln_b = f32(m.stem[0].bias), f32(m.stem[1].weight), f32(m.stem[1].bias)
+        net.stem_w = p.bf16(m.stem[0].weight.reshape(m.dims[0], 48))
+        net.stem_b, net.stem_ln_w, net.stem_ln_b = p.f32(m.stem[0].bias), p.f32(m.stem[1].weight), p.f32(m.stem[1].bias)
         bi = 0
         for si, stage in enumerate(m.stages):
             if si > 0:
                 ln, conv = stage.downsample[0], stage.downsample[1]
-                net.down[si].ln_w, net.down[si].ln_b = f32(ln.weight), f32(ln.bias)
-                net.down[si].conv_w = bf16(conv.weight.permute(0, 2, 3, 1).reshape(conv.weight.shape[0], -1))
-                net.down[si].conv_b = f32(conv.bias)
+                net.down[si].ln_w, net.down[si].ln_b = p.f32(ln.weight), p.f32(ln.bias)
+                net.down[si].conv_w = p.bf16(conv.weight.permute(0, 2, 3, 1).reshape(conv.weight.shape[0], -1))
+                net.down[si].conv_b = p.f32(conv.bias)
             for blk in stage.blocks:
                 b = net.blocks[bi]
                 c = blk.conv_dw.weight.shape[0]
-                b.dw_w = f32(blk.conv_dw.weight.reshape(c, 49).t())
-                b.dw_b, b.ln_w, b.ln_b = f32(blk.conv_dw.bias), f32(blk.norm.weight), f32(blk.norm.bias)
-                b.fc1_w, b.fc1_b = bf16(blk.mlp.fc1.weight), f32(blk.mlp.fc1.bias)
-                b.fc2_w, b.fc2_b = bf16(blk.mlp.fc2.weight), f32(blk.mlp.fc2.bias)
-                b.gamma = f32(blk.gamma)
+                b.dw_w = p.f32(blk.conv_dw.weight.reshape(c, 49).t())
+                b.dw_b, b.ln_w, b.ln_b = p.f32(blk.conv_dw.bias), p.f32(blk.norm.weight), p.f32(blk.norm.bias)
+                b.fc1_w, b.fc1_b = p.bf16(blk.mlp.fc1.weight), p.f32(blk.mlp.fc1.bias)
+                b.fc2_w, b.fc2_b = p.bf16(blk.mlp.fc2.weight), p.f32(blk.mlp.fc2.bias)
+                b.gamma = p.f32(blk.gamma)
                 bi += 1
-        net.head_ln_w, net.head_ln_b = f32(m.head.norm.weight), f32(m.head.norm.bias)
-        w, bias = fold_cnn_neck(self.output_layer, m.dims[-1], self.image_size // 32, self.feat_dim, device)
-        net.neck_w, net.neck_b = bf16(w), f32(bias)
-        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+        net.head_ln_w, net.head_ln_b = p.f32(m.head.norm.weight), p.f32(m.head.norm.bias)
+        net.neck_w, net.neck_b = self._pack_cnn_neck(p)
         return net
-
-    def _load_pretrained(self, model_name: str) -> None:
-        """The reference downloads timm weights (timm_wrapper.py:16-21); this box has no network, so weights come
-        from $VDK_PRETRAINED_DIR/<model_name>.pth (a timm state_dict) when present."""
-        root = os.environ.get("VDK_PRETRAINED_DIR")
-        path = os.path.join(root, f"{model_name}.pth") if root else None
-        if path and os.path.exists(path):
-            sd = torch.load(path, map_location="cpu")
-            sd = {k: v for k, v in sd.items() if not k.startswith("head.fc")}
-            self.model.load_state_dict(sd, strict=True)
-        else:
-            warnings.warn(f"pretrained weights for '{model_name}' not found (set VDK_PRETRAINED_DIR); using random init")
-
-
-class _ConvNeXtTrainFn(torch.autograd.Function):
-    """Train-mode forward/backward of the whole backbone + neck as one autograd node (csrc/convnext_train.cu)."""
-
-    @staticmethod
-    def forward(ctx, module, x, *params):
-        ctx.module = module
-        return module._train_forward(x)
-
-    @staticmethod
-    def backward(ctx, dout):
-        grads = ctx.module._train_backward(dout)
-        return (None, None, *grads)
 
 
 class BackboneFactory:

@@ -12,15 +12,12 @@ NotImplementedError.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import warnings
-from typing import Dict, Optional
 
 import torch
 import torch.nn as nn
 
-from . import _lib
-from .resnet import _ConvC, fold_bn
+from .resnet import _ConvC
+from .wrapper import BackboneWrapper, cnn_neck, fold_bn
 
 # timm 0.9.16 efficientnet.py _gen_efficientnetv2_{s,m,l} arch_def: per stage (kind, repeats, stride, expansion, out
 # channels); every `ir` stage has se0.25 of the block's input width.  stem width, conv_head width 1280, BN eps 1e-3.
@@ -115,6 +112,7 @@ MAX_BLOCKS = 80
 
 class EffNetV2NetC(C.Structure):
     """vdk_effnetv2_net (include/vdk_b200.h)."""
+    api = "vdk_effnetv2"
     _fields_ = [("image_size", C.c_int), ("feat_dim", C.c_int), ("num_blocks", C.c_int), ("stem_ch", C.c_int),
                 ("head_ch", C.c_int), ("stem", _ConvC), ("blocks", _EffBlockC * MAX_BLOCKS), ("head", _ConvC),
                 ("neck_w", C.c_void_p), ("neck_b", C.c_void_p)]
@@ -140,87 +138,31 @@ def pack_conv_ex(w: torch.Tensor) -> torch.Tensor:
     return out
 
 
-class EfficientNetV2Wrapper(nn.Module):
+class EfficientNetV2Wrapper(BackboneWrapper):
     """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm tf_efficientnetv2 backbone (eval /
     extract only)."""
 
-    _classifier = "classifier."  # timm's classifier keys, dropped from a checkpoint (num_classes=0)
+    _dropped = ("classifier.",)
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, **kwargs):
-        super().__init__()
         if model_name not in EFFNETV2_ARCHS:
             raise ValueError(f"backbone '{model_name}' is not built for H100 yet; EfficientNetV2s available: {sorted(EFFNETV2_ARCHS)}")
         if image_size % 32 != 0:
             raise ValueError("image_size must be a multiple of 32")
-        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = EfficientNetV2Params(**EFFNETV2_ARCHS[model_name], depths=depths)
         hw = image_size // 32
-        self.output_layer = nn.Sequential(nn.BatchNorm2d(HEAD_CH), nn.Flatten(1), nn.Linear(HEAD_CH * hw * hw, feat_dim),
-                                          nn.BatchNorm1d(feat_dim))
-        self._packed: Optional[Dict] = None
-        self._packed_key = None
-        self._ws = None
-        if pretrained:
-            self._load_pretrained(model_name)
+        super().__init__(model_name, feat_dim, image_size, EfficientNetV2Params(**EFFNETV2_ARCHS[model_name], depths=depths),
+                         cnn_neck(HEAD_CH, HEAD_CH * hw * hw, feat_dim), pretrained)
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.training:
-            raise NotImplementedError(f"{self.model_name}: EfficientNetV2 backbones are extraction-only on H100 (call .eval() first)")
-        return self.embed(x, l2_normalize=False)
-
-    @torch.no_grad()
-    def embed(self, x: torch.Tensor, l2_normalize: bool = False) -> torch.Tensor:
-        """[B,3,S,S] fp32 NCHW -> fp32 [B, feat_dim] (TimmWrapper.forward in eval mode; optionally F.normalize fused)."""
-        lib = _lib.load()
-        if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.EfficientNetV2Wrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
-        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
-            raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
-        x = x.contiguous().float()
-        net = self._pack(x.device)
-        B = x.shape[0]
-        out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
-        need = lib.vdk_effnetv2_workspace_bytes(C.byref(net), B)
-        if need == 0:
-            raise RuntimeError("vdk_effnetv2_workspace_bytes: invalid network")
-        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
-            self._ws = torch.empty((need,), dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(lib.vdk_effnetv2_forward(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(),
-                                                self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()), "vdk_effnetv2_forward")
-        return out
-
-    def _version_key(self, device):
-        return (str(device),) + tuple(int(t._version) for t in list(self.parameters()) + list(self.buffers()))
-
-    def _pack(self, device) -> EffNetV2NetC:
+    def _build(self, p) -> EffNetV2NetC:
         """vdk_effnetv2_net: BatchNorms folded once per weight version; bf16 conv weights in vdk_conv2d_ex's layouts, the stem
         as zero-padded (kh, kw, c) patch rows [stem, 64], fp32 depthwise taps [9, mid] and SE weights, the folded neck in
         (h, w, c) order."""
-        key = self._version_key(device)
-        if self._packed is not None and self._packed_key == key:
-            return self._packed["net"]
-        from .backbone import fold_cnn_neck
-        keep = []
-
-        def f32(t):
-            t = t.detach().to(device, torch.float32).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def bf16(t):
-            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
-            keep.append(t)
-            return t.data_ptr()
-
         def conv(dst, w, b):
-            dst.w, dst.b = bf16(pack_conv_ex(w)), f32(b)
+            dst.w, dst.b = p.bf16(pack_conv_ex(w)), p.f32(b)
 
         m, net = self.model, EffNetV2NetC()
         net.image_size, net.feat_dim, net.stem_ch, net.head_ch = self.image_size, self.feat_dim, m.stem_ch, HEAD_CH
-        w, b = fold_bn(m.conv_stem, m.bn1)
-        rows = w.permute(0, 2, 3, 1).reshape(m.stem_ch, 27)
-        net.stem.w, net.stem.b = bf16(torch.cat([rows, rows.new_zeros(m.stem_ch, 64 - 27)], dim=1)), f32(b)
+        net.stem.w, net.stem.b = p.stem_rows(*fold_bn(m.conv_stem, m.bn1), 64)
         blocks = [blk for stage in m.blocks for blk in stage]
         if len(blocks) > MAX_BLOCKS:
             raise ValueError(f"{len(blocks)} blocks exceed vdk_effnetv2_net's {MAX_BLOCKS}")
@@ -236,26 +178,12 @@ class EfficientNetV2Wrapper(nn.Module):
             else:
                 conv(c.conv, *fold_bn(blk.conv_pw, blk.bn1))
                 w, b = fold_bn(blk.conv_dw, blk.bn2)
-                c.dw_w, c.dw_b = f32(w.reshape(blk.mid, 9).t()), f32(b)
+                c.dw_w, c.dw_b = p.f32(w.reshape(blk.mid, 9).t()), p.f32(b)
                 se = blk.se
                 c.se_rd = se.conv_reduce.out_channels
-                c.se_w1, c.se_b1 = f32(se.conv_reduce.weight.flatten(1)), f32(se.conv_reduce.bias)
-                c.se_w2, c.se_b2 = f32(se.conv_expand.weight.flatten(1)), f32(se.conv_expand.bias)
+                c.se_w1, c.se_b1 = p.f32(se.conv_reduce.weight.flatten(1)), p.f32(se.conv_reduce.bias)
+                c.se_w2, c.se_b2 = p.f32(se.conv_expand.weight.flatten(1)), p.f32(se.conv_expand.bias)
                 conv(c.conv_pwl, *fold_bn(blk.conv_pwl, blk.bn3))
         conv(net.head, *fold_bn(m.conv_head, m.bn2))
-        w, bias = fold_cnn_neck(self.output_layer, HEAD_CH, self.image_size // 32, self.feat_dim, device)
-        net.neck_w, net.neck_b = bf16(w), f32(bias)
-        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+        net.neck_w, net.neck_b = self._pack_cnn_neck(p)
         return net
-
-    def _load_pretrained(self, model_name: str) -> None:
-        """Like TimmWrapper._load_pretrained: a timm state_dict from $VDK_PRETRAINED_DIR/<model_name>.pth (no network here);
-        the classifier (classifier.*) is dropped, as num_classes=0 does."""
-        root = os.environ.get("VDK_PRETRAINED_DIR")
-        path = os.path.join(root, f"{model_name}.pth") if root else None
-        if path and os.path.exists(path):
-            sd = torch.load(path, map_location="cpu")
-            sd = {k: v for k, v in sd.items() if not k.startswith(self._classifier)}
-            self.model.load_state_dict(sd, strict=True)
-        else:
-            warnings.warn(f"pretrained weights for '{model_name}' not found (set VDK_PRETRAINED_DIR); using random init")

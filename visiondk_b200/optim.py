@@ -15,6 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .wrapper import BackboneWrapper
 
 
 class _FlatGroup:
@@ -113,15 +114,15 @@ class FusedSGDClipEMA:
 
     def _invalidate_packed(self) -> None:
         """The kernels above write parameters, EMA parameters and EMA buffers through raw pointers, which does not bump
-        torch's `_version` counters — the key the backbones' packed inference weights (`TimmWrapper._pack`,
-        `ViTWrapper._pack`) are cached under.  Drop those caches explicitly so that the next `embed()` of the live model or
-        of the EMA copy (the in-training eval, engine/procedure/train.py:244-262) re-packs the CURRENT weights."""
+        torch's `_version` counters — the key every backbone wrapper's packed inference weights (`BackboneWrapper._pack`)
+        are cached under.  Drop those caches explicitly so that the next `embed()` of the live model or of the EMA copy
+        (the in-training eval, engine/procedure/train.py:244-262) re-packs the CURRENT weights."""
         for root in (self.model, self.ema_model):
             if root is None:
                 continue
             for m in root.modules():
-                if hasattr(m, "_packed_key"):
-                    m._packed_key = None
+                if isinstance(m, BackboneWrapper):
+                    m.invalidate_pack()
 
     def state_dict(self) -> dict:
         """What torch.optim.SGD.state_dict() carries for the reference's checkpoint (engine/procedure/train.py:273): the

@@ -15,7 +15,8 @@ import ctypes as C
 import torch
 import torch.nn as nn
 
-from .resnet import ResNetWrapper, _ConvC, fold_bn
+from .resnet import _ConvC
+from .wrapper import BackboneWrapper, cnn_neck, fold_bn
 
 # timm 0.9.16 resnest.py model_args: deep stem of width 32, avg_down shortcuts, avd (the stride-2 3x3 average pool)
 RESNEST_ARCHS = {
@@ -144,12 +145,12 @@ class ResNeStNetC(C.Structure):
     ]
 
 
-class ResNeStWrapper(ResNetWrapper):
-    """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm ResNeSt backbone (eval / extract only);
-    embed / forward / the train-mode refusal / the checkpoint load (fc.* dropped) are ResNetWrapper's."""
+class ResNeStWrapper(BackboneWrapper):
+    """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm ResNeSt backbone (eval / extract only)."""
+
+    _dropped = ("fc.",)
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, **kwargs):
-        nn.Module.__init__(self)
         if model_name not in RESNEST_ARCHS:
             raise ValueError(f"backbone '{model_name}' is not built for H100 yet; ResNeSts available: {sorted(RESNEST_ARCHS)}")
         if image_size % 32 != 0:
@@ -157,71 +158,40 @@ class ResNeStWrapper(ResNetWrapper):
         args = dict(RESNEST_ARCHS[model_name])
         if depths is not None:
             args["depths"] = tuple(depths)
-        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = ResNeStParams(**args)
         hw = image_size // 32
-        self.output_layer = nn.Sequential(nn.BatchNorm2d(2048), nn.Flatten(1), nn.Linear(2048 * hw * hw, feat_dim),
-                                          nn.BatchNorm1d(feat_dim))
-        self._packed = None
-        self._packed_key = None
-        self._ws = None
-        if pretrained:
-            self._load_pretrained(model_name)
+        super().__init__(model_name, feat_dim, image_size, ResNeStParams(**args), cnn_neck(2048, 2048 * hw * hw, feat_dim),
+                         pretrained)
 
-    def _pack(self, device) -> ResNeStNetC:
+    def _build(self, p) -> ResNeStNetC:
         """vdk_resnest_net: BatchNorms folded in fp32 once per weight version, bf16 conv weights [Cout, kh, kw, Cin] (the split
         conv in vdk_conv2d_grouped_ex's layout), the deep stem as zero-padded (kh, kw, c) patch rows, fp32 attention weights,
         the folded neck in (h, w, c) order."""
-        key = self._version_key(device)
-        if self._packed is not None and self._packed_key == key:
-            return self._packed["net"]
-        from .backbone import fold_cnn_neck
-        keep = []
-
-        def f32(t):
-            t = t.detach().to(device, torch.float32).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def bf16(t):
-            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
-            keep.append(t)
-            return t.data_ptr()
-
-        def stem(dst, w, b):
-            k = w[0].numel()
-            rows = w.permute(0, 2, 3, 1).reshape(w.shape[0], k)
-            kp = (k + 63) // 64 * 64
-            dst.w, dst.b = bf16(torch.cat([rows, rows.new_zeros(w.shape[0], kp - k)], dim=1)), f32(b)
-
         m, net = self.model, ResNeStNetC()
         net.image_size, net.feat_dim = self.image_size, self.feat_dim
         net.radix, net.cardinality, net.base_width, net.avd_first = m.radix, m.cardinality, m.base_width, int(m.avd_first)
         for i in range(4):
             net.depths[i] = m.depths[i]
             net.attn[i] = attn_width(group_width(64 << i, m.base_width, m.cardinality), m.radix)
-        stem(net.stem[0], *fold_bn(m.conv1[0], m.conv1[1]))
-        stem(net.stem[1], *fold_bn(m.conv1[3], m.conv1[4]))
-        stem(net.stem[2], *fold_bn(m.conv1[6], m.bn1))
+        net.stem[0].w, net.stem[0].b = p.stem_rows(*fold_bn(m.conv1[0], m.conv1[1]), 64)
+        net.stem[1].w, net.stem[1].b = p.stem_rows(*fold_bn(m.conv1[3], m.conv1[4]), 64)
+        net.stem[2].w, net.stem[2].b = p.stem_rows(*fold_bn(m.conv1[6], m.bn1), 64)
         for i, blk in enumerate(m.blocks()):
             c, sa = net.blocks[i], blk.conv2
             w, b = fold_bn(blk.conv1, blk.bn1)
-            c.conv1.w, c.conv1.b = bf16(w.flatten(1)), f32(b)
+            c.conv1.w, c.conv1.b = p.bf16(w.flatten(1)), p.f32(b)
             w, b = fold_bn(sa.conv, sa.bn0)
-            c.conv2.w, c.conv2.b = bf16(pack_split(w, sa.conv.groups)), f32(b)
+            c.conv2.w, c.conv2.b = p.bf16(pack_split(w, sa.conv.groups)), p.f32(b)
             s = sa.bn1.weight.detach().float() / torch.sqrt(sa.bn1.running_var.detach().float() + sa.bn1.eps)
-            c.fc1_w = f32(sa.fc1.weight.detach().float().flatten(1) * s[:, None])
-            c.fc1_b = f32((sa.fc1.bias.detach().float() - sa.bn1.running_mean.detach().float()) * s + sa.bn1.bias.detach().float())
-            c.fc2_w, c.fc2_b = f32(sa.fc2.weight.flatten(1)), f32(sa.fc2.bias)
+            c.fc1_w = p.f32(sa.fc1.weight.detach().float().flatten(1) * s[:, None])
+            c.fc1_b = p.f32((sa.fc1.bias.detach().float() - sa.bn1.running_mean.detach().float()) * s + sa.bn1.bias.detach().float())
+            c.fc2_w, c.fc2_b = p.f32(sa.fc2.weight.flatten(1)), p.f32(sa.fc2.bias)
             w, b = fold_bn(blk.conv3, blk.bn3)
-            c.conv3.w, c.conv3.b = bf16(w.flatten(1)), f32(b)
+            c.conv3.w, c.conv3.b = p.bf16(w.flatten(1)), p.f32(b)
             if blk.downsample is not None:
                 w, b = fold_bn(blk.downsample[1], blk.downsample[2])
                 w = w.permute(0, 2, 3, 1)
                 if blk.stride == 2:  # AvgPool2d(2, 2) then the 1x1 conv == a 2x2/s2 conv with w / 4 at every tap
                     w = w.expand(-1, 2, 2, -1) / 4
-                c.down.w, c.down.b = bf16(w), f32(b)
-        w, bias = fold_cnn_neck(self.output_layer, 2048, self.image_size // 32, self.feat_dim, device)
-        net.neck_w, net.neck_b = bf16(w), f32(bias)
-        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+                c.down.w, c.down.b = p.bf16(w), p.f32(b)
+        net.neck_w, net.neck_b = self._pack_cnn_neck(p)
         return net

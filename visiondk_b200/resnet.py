@@ -12,14 +12,11 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import warnings
-from typing import Dict, Optional
 
 import torch
 import torch.nn as nn
 
-from . import _lib
+from .wrapper import BackboneWrapper, cnn_neck, fold_bn
 
 # timm 0.9.16 resnet.py model_args; all Bottleneck (stride on the 3x3 conv, expansion 4)
 RESNET_ARCHS = {
@@ -147,20 +144,12 @@ def pack_grouped(w: torch.Tensor) -> torch.Tensor:
     return out.view(cout, k, k, 128)
 
 
-def fold_bn(conv: nn.Conv2d, bn: nn.BatchNorm2d):
-    """Eval BatchNorm folded into the bias-free conv before it, in fp32: w * g / sqrt(var + eps), b - mean * g / sqrt(var + eps)."""
-    s = bn.weight.detach().float() / torch.sqrt(bn.running_var.detach().float() + bn.eps)
-    w = conv.weight.detach().float() * s.view(-1, 1, 1, 1)
-    return w, bn.bias.detach().float() - bn.running_mean.detach().float() * s
-
-
-class ResNetWrapper(nn.Module):
+class ResNetWrapper(BackboneWrapper):
     """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm ResNet backbone (eval / extract only)."""
 
-    _classifier = "fc."  # timm's classifier keys, dropped from a checkpoint (num_classes=0)
+    _dropped = ("fc.",)
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, **kwargs):
-        super().__init__()
         archs = {**RESNET_ARCHS, **RESNEXT_ARCHS}
         if model_name not in archs:
             raise ValueError(f"backbone '{model_name}' is not built for H100 yet; ResNets available: {sorted(archs)}")
@@ -169,78 +158,18 @@ class ResNetWrapper(nn.Module):
         args = dict(archs[model_name])
         if depths is not None:
             args["depths"] = tuple(depths)
-        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = ResNetParams(**args)
         hw = image_size // 32
-        self.output_layer = nn.Sequential(nn.BatchNorm2d(2048), nn.Flatten(1), nn.Linear(2048 * hw * hw, feat_dim),
-                                          nn.BatchNorm1d(feat_dim))
-        self._packed: Optional[Dict] = None
-        self._packed_key = None
-        self._ws = None
-        if pretrained:
-            self._load_pretrained(model_name)
+        super().__init__(model_name, feat_dim, image_size, ResNetParams(**args), cnn_neck(2048, 2048 * hw * hw, feat_dim),
+                         pretrained)
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.training:
-            raise NotImplementedError(f"{self.model_name}: ResNet backbones are extraction-only on H100 (call .eval() first)")
-        return self.embed(x, l2_normalize=False)
-
-    @torch.no_grad()
-    def embed(self, x: torch.Tensor, l2_normalize: bool = False) -> torch.Tensor:
-        """[B,3,S,S] fp32 NCHW -> fp32 [B, feat_dim] (TimmWrapper.forward in eval mode; optionally F.normalize fused)."""
-        lib = _lib.load()
-        if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.ResNetWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
-        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
-            raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
-        x = x.contiguous().float()
-        net = self._pack(x.device)
-        B = x.shape[0]
-        out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
-        api = net.api
-        need = getattr(lib, f"{api}_workspace_bytes")(C.byref(net), B)
-        if need == 0:
-            raise RuntimeError(f"{api}_workspace_bytes: invalid network")
-        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
-            self._ws = torch.empty((need,), dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(getattr(lib, f"{api}_forward")(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(),
-                                                      self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()), f"{api}_forward")
-        return out
-
-    def _version_key(self, device):
-        return (str(device),) + tuple(int(t._version) for t in list(self.parameters()) + list(self.buffers()))
-
-    def _pack(self, device) -> ResNetNetC:
+    def _build(self, p) -> ResNetNetC:
         """Kernel-side layouts (include/vdk_b200.h): BatchNorms folded once per weight version, bf16 conv weights
         [Cout, kh, kw, Cin], stem weights as zero-padded (kh, kw, c) patch rows, the folded neck in (h, w, c) order."""
-        key = self._version_key(device)
-        if self._packed is not None and self._packed_key == key:
-            return self._packed["net"]
-        from .backbone import fold_cnn_neck
-        keep = []
-
-        def f32(t):
-            t = t.detach().to(device, torch.float32).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def bf16(t):
-            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
-            keep.append(t)
-            return t.data_ptr()
-
         def conv(dst, w, b, pool2=False):
             w = w.permute(0, 2, 3, 1)  # [Cout, kh, kw, Cin]
             if pool2:  # AvgPool2d(2, 2) then the 1x1 conv == a 2x2/s2 conv with w / 4 at every tap
                 w = w.expand(-1, 2, 2, -1) / 4
-            dst.w, dst.b = bf16(w), f32(b)
-
-        def stem(dst, w, b):
-            k = w[0].numel()
-            rows = w.permute(0, 2, 3, 1).reshape(w.shape[0], k)
-            kp = (k + 63) // 64 * 64
-            dst.w, dst.b = bf16(torch.cat([rows, rows.new_zeros(w.shape[0], kp - k)], dim=1)), f32(b)
+            dst.w, dst.b = p.bf16(w), p.f32(b)
 
         m = self.model
         net = ResNetNetC() if m.cardinality == 1 else BottleneckNetC()
@@ -253,11 +182,11 @@ class ResNetWrapper(nn.Module):
         else:
             net.width, net.cardinality, net.stem_pool = m.base_width * m.cardinality, m.cardinality, STEM_POOL_PAD1
         if m.deep_stem:
-            stem(net.stem[0], *fold_bn(m.conv1[0], m.conv1[1]))
-            stem(net.stem[1], *fold_bn(m.conv1[3], m.conv1[4]))
-            stem(net.stem[2], *fold_bn(m.conv1[6], m.bn1))
+            net.stem[0].w, net.stem[0].b = p.stem_rows(*fold_bn(m.conv1[0], m.conv1[1]), 64)
+            net.stem[1].w, net.stem[1].b = p.stem_rows(*fold_bn(m.conv1[3], m.conv1[4]), 64)
+            net.stem[2].w, net.stem[2].b = p.stem_rows(*fold_bn(m.conv1[6], m.bn1), 64)
         else:
-            stem(net.stem[0], *fold_bn(m.conv1, m.bn1))
+            net.stem[0].w, net.stem[0].b = p.stem_rows(*fold_bn(m.conv1, m.bn1), 64)
         for i, blk in enumerate(m.blocks()):
             b = net.blocks[i]
             conv(b.conv1, *fold_bn(blk.conv1, blk.bn1))
@@ -265,26 +194,12 @@ class ResNetWrapper(nn.Module):
                 conv(b.conv2, *fold_bn(blk.conv2, blk.bn2))
             else:
                 w, bias = fold_bn(blk.conv2, blk.bn2)
-                b.conv2.w, b.conv2.b = bf16(pack_grouped(w)), f32(bias)
+                b.conv2.w, b.conv2.b = p.bf16(pack_grouped(w)), p.f32(bias)
             conv(b.conv3, *fold_bn(blk.conv3, blk.bn3))
             if blk.downsample is not None:
                 if m.avg_down:
                     conv(b.down, *fold_bn(blk.downsample[1], blk.downsample[2]), pool2=blk.stride == 2)
                 else:
                     conv(b.down, *fold_bn(blk.downsample[0], blk.downsample[1]))
-        w, bias = fold_cnn_neck(self.output_layer, 2048, self.image_size // 32, self.feat_dim, device)
-        net.neck_w, net.neck_b = bf16(w), f32(bias)
-        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+        net.neck_w, net.neck_b = self._pack_cnn_neck(p)
         return net
-
-    def _load_pretrained(self, model_name: str) -> None:
-        """Like TimmWrapper._load_pretrained: a timm state_dict from $VDK_PRETRAINED_DIR/<model_name>.pth (no network here);
-        the classifier (fc.*, the legacy SENets' last_linear.*) is dropped, as num_classes=0 does."""
-        root = os.environ.get("VDK_PRETRAINED_DIR")
-        path = os.path.join(root, f"{model_name}.pth") if root else None
-        if path and os.path.exists(path):
-            sd = torch.load(path, map_location="cpu")
-            sd = {k: v for k, v in sd.items() if not k.startswith(self._classifier)}
-            self.model.load_state_dict(sd, strict=True)
-        else:
-            warnings.warn(f"pretrained weights for '{model_name}' not found (set VDK_PRETRAINED_DIR); using random init")

@@ -10,10 +10,10 @@ NotImplementedError.
 """
 from __future__ import annotations
 
-import torch
 import torch.nn as nn
 
-from .resnet import STEM_POOL_CEIL, BottleneckNetC, ResNetWrapper, fold_bn, pack_grouped
+from .resnet import STEM_POOL_CEIL, BottleneckNetC, pack_grouped
+from .wrapper import BackboneWrapper, cnn_neck, fold_bn
 
 # timm 0.9.16 senet.py model_args (reduction 16; SE-ResNet: stride on the 1x1 conv1, SE-ResNeXt: on the 3x3 conv2)
 SENET_ARCHS = {
@@ -83,14 +83,12 @@ class SENetParams(nn.Module):
         return [b for i in range(4) for b in getattr(self, f"layer{i + 1}")]
 
 
-class SENetWrapper(ResNetWrapper):
-    """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm legacy SENet backbone (eval / extract only);
-    embed / forward / the train-mode refusal are ResNetWrapper's."""
+class SENetWrapper(BackboneWrapper):
+    """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm legacy SENet backbone (eval / extract only)."""
 
-    _classifier = "last_linear."
+    _dropped = ("last_linear.",)
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, **kwargs):
-        nn.Module.__init__(self)
         if model_name not in SENET_ARCHS:
             raise ValueError(f"backbone '{model_name}' is not built for H100 yet; legacy SENets available: {sorted(SENET_ARCHS)}")
         if image_size % 32 != 0:
@@ -98,36 +96,13 @@ class SENetWrapper(ResNetWrapper):
         args = dict(SENET_ARCHS[model_name])
         if depths is not None:
             args["depths"] = tuple(depths)
-        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = SENetParams(**args)
         hw = image_size // 32
-        self.output_layer = nn.Sequential(nn.BatchNorm2d(2048), nn.Flatten(1), nn.Linear(2048 * hw * hw, feat_dim),
-                                          nn.BatchNorm1d(feat_dim))
-        self._packed = None
-        self._packed_key = None
-        self._ws = None
-        if pretrained:
-            self._load_pretrained(model_name)
+        super().__init__(model_name, feat_dim, image_size, SENetParams(**args), cnn_neck(2048, 2048 * hw * hw, feat_dim),
+                         pretrained)
 
-    def _pack(self, device) -> BottleneckNetC:
+    def _build(self, p) -> BottleneckNetC:
         """vdk_bottleneck_net: BatchNorms folded once per weight version, bf16 conv weights [Cout, kh, kw, Cin] (grouped ones
         block-diagonal), the stem as zero-padded (kh, kw, c) patch rows, fp32 SE weights, the folded neck in (h, w, c) order."""
-        key = self._version_key(device)
-        if self._packed is not None and self._packed_key == key:
-            return self._packed["net"]
-        from .backbone import fold_cnn_neck
-        keep = []
-
-        def f32(t):
-            t = t.detach().to(device, torch.float32).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def bf16(t):
-            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
-            keep.append(t)
-            return t.data_ptr()
-
         m, net = self.model, BottleneckNetC()
         net.image_size, net.feat_dim = self.image_size, self.feat_dim
         for i in range(4):
@@ -136,22 +111,18 @@ class SENetWrapper(ResNetWrapper):
         net.width = (64 * 4 // 64) * m.groups if resnext else 64
         net.cardinality, net.stride_on_conv1, net.stem_pool = m.groups, int(not resnext), STEM_POOL_CEIL
         net.deep_stem, net.avg_down, net.se_reduction = 0, 0, SE_REDUCTION
-        w, b = fold_bn(m.layer0.conv1, m.layer0.bn1)
-        rows = w.permute(0, 2, 3, 1).reshape(64, 147)
-        net.stem[0].w, net.stem[0].b = bf16(torch.cat([rows, rows.new_zeros(64, 192 - 147)], dim=1)), f32(b)
+        net.stem[0].w, net.stem[0].b = p.stem_rows(*fold_bn(m.layer0.conv1, m.layer0.bn1), 64)
         for i, blk in enumerate(m.blocks()):
             c = net.blocks[i]
             for dst, cv, bn in ((c.conv1, blk.conv1, blk.bn1), (c.conv2, blk.conv2, blk.bn2), (c.conv3, blk.conv3, blk.bn3)):
                 w, b = fold_bn(cv, bn)
                 w = pack_grouped(w) if cv.groups > 1 else w.permute(0, 2, 3, 1)
-                dst.w, dst.b = bf16(w), f32(b)
+                dst.w, dst.b = p.bf16(w), p.f32(b)
             if blk.downsample is not None:
                 w, b = fold_bn(blk.downsample[0], blk.downsample[1])
-                c.down.w, c.down.b = bf16(w.permute(0, 2, 3, 1)), f32(b)
+                c.down.w, c.down.b = p.bf16(w.permute(0, 2, 3, 1)), p.f32(b)
             se = blk.se_module
-            c.se_fc1_w, c.se_fc1_b = f32(se.fc1.weight.flatten(1)), f32(se.fc1.bias)
-            c.se_fc2_w, c.se_fc2_b = f32(se.fc2.weight.flatten(1)), f32(se.fc2.bias)
-        w, bias = fold_cnn_neck(self.output_layer, 2048, self.image_size // 32, self.feat_dim, device)
-        net.neck_w, net.neck_b = bf16(w), f32(bias)
-        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+            c.se_fc1_w, c.se_fc1_b = p.f32(se.fc1.weight.flatten(1)), p.f32(se.fc1.bias)
+            c.se_fc2_w, c.se_fc2_b = p.f32(se.fc2.weight.flatten(1)), p.f32(se.fc2.bias)
+        net.neck_w, net.neck_b = self._pack_cnn_neck(p)
         return net

@@ -12,14 +12,11 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
-import warnings
-from typing import Dict, Optional
 
 import torch
 import torch.nn as nn
 
-from . import _lib
+from .wrapper import BackboneWrapper, cnn_neck, fold_neck
 
 IMAGE_SIZE = 256  # both towers' default img_size; timm_wrapper.py passes none to create_model
 HEAD_DIM = 32
@@ -135,6 +132,7 @@ MAX_BLOCKS = 24
 
 class SwinV2NetC(C.Structure):
     """vdk_swinv2_net (include/vdk_b200.h)."""
+    api = "vdk_swinv2"
     _fields_ = [
         ("image_size", C.c_int), ("feat_dim", C.c_int), ("embed_dim", C.c_int), ("depths", C.c_int * 4), ("window", C.c_int * 4),
         ("shift", C.c_int * 4), ("stem_w", C.c_void_p), ("stem_b", C.c_void_p), ("stem_ln_w", C.c_void_p),
@@ -151,28 +149,20 @@ def merge_weight_khkw(w: torch.Tensor) -> torch.Tensor:
     return w.reshape(cout, 2, 2, c).permute(0, 2, 1, 3)
 
 
-@torch.no_grad()
 def fold_nhwc_neck(output_layer: nn.Sequential, h: int, wc: int, feat_dim: int, device):
     """The neck BatchNorm2d(h) over the h axis of an NHWC map -> Flatten in (h, w, c) order -> Linear -> BatchNorm1d (eval
     statistics) as one Linear over the (h, w, c) features: (weight [feat_dim, h * wc], bias [feat_dim]) in fp64."""
-    bn2, lin, bn1 = output_layer[0], output_layer[2], output_layer[3]
-    s2 = (bn2.weight.double() / torch.sqrt(bn2.running_var.double() + bn2.eps)).to(device)
-    t2 = bn2.bias.double().to(device) - bn2.running_mean.double().to(device) * s2
-    s1 = (bn1.weight.double() / torch.sqrt(bn1.running_var.double() + bn1.eps)).to(device)
-    w = lin.weight.detach().double().to(device).reshape(feat_dim, h, wc)
-    bias = lin.bias.detach().double().to(device) + (w * t2.view(1, -1, 1)).sum(dim=(1, 2))
-    bias = s1 * (bias - bn1.running_mean.double().to(device)) + bn1.bias.double().to(device)
-    return (w * s2.view(1, -1, 1) * s1.view(-1, 1, 1)).reshape(feat_dim, h * wc), bias
+    w, bias = fold_neck(output_layer, device)
+    return w.reshape(feat_dim, h * wc), bias
 
 
-class SwinV2Wrapper(nn.Module):
+class SwinV2Wrapper(BackboneWrapper):
     """Drop-in for models/faceX/backbone/timm_wrapper.py::TimmWrapper with a timm Swin V2 backbone (eval / extract only)."""
 
-    _dropped = ("head.fc.",)  # timm's classifier keys, dropped from a checkpoint (num_classes=0)
-    _buffers_in_checkpoints = ("relative_position_index", "relative_coords_table", "attn_mask")  # rebuilt, not loaded
+    _dropped = ("head.fc.",)
+    _rebuilt = ("relative_position_index", "relative_coords_table", "attn_mask")  # as timm's own checkpoint filter does
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, depths=None, **kwargs):
-        super().__init__()
         if model_name not in SWINV2_ARCHS:
             raise ValueError(f"backbone '{model_name}' is not built for H100 yet; Swin V2 towers available: {sorted(SWINV2_ARCHS)}")
         if image_size != IMAGE_SIZE:
@@ -181,67 +171,14 @@ class SwinV2Wrapper(nn.Module):
         args = dict(SWINV2_ARCHS[model_name])
         if depths is not None:
             args["depths"] = tuple(depths)
-        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = SwinV2Params(**args)
         c_last, hw = args["embed_dim"] * 8, image_size // 32
-        self.output_layer = nn.Sequential(nn.BatchNorm2d(hw), nn.Flatten(1), nn.Linear(hw * hw * c_last, feat_dim),
-                                          nn.BatchNorm1d(feat_dim))
-        self._packed: Optional[Dict] = None
-        self._packed_key = None
-        self._ws = None
-        if pretrained:
-            self._load_pretrained(model_name)
+        super().__init__(model_name, feat_dim, image_size, SwinV2Params(**args), cnn_neck(hw, hw * hw * c_last, feat_dim),
+                         pretrained)
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.training:
-            raise NotImplementedError(f"{self.model_name}: Swin V2 backbones are extraction-only on H100 (call .eval() first)")
-        return self.embed(x, l2_normalize=False)
-
-    @torch.no_grad()
-    def embed(self, x: torch.Tensor, l2_normalize: bool = False) -> torch.Tensor:
-        """[B,3,256,256] fp32 NCHW -> fp32 [B, feat_dim] (TimmWrapper.forward in eval mode; optionally F.normalize fused)."""
-        lib = _lib.load()
-        if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.SwinV2Wrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
-        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
-            raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
-        x = x.contiguous().float()
-        net = self._pack(x.device)
-        B = x.shape[0]
-        out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
-        need = lib.vdk_swinv2_workspace_bytes(C.byref(net), B)
-        if need == 0:
-            raise RuntimeError("vdk_swinv2_workspace_bytes: invalid network")
-        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
-            self._ws = torch.empty((need,), dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(lib.vdk_swinv2_forward(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(), self._ws.data_ptr(),
-                                              self._ws.numel(), _lib.stream_ptr()), "vdk_swinv2_forward")
-        return out
-
-    def _version_key(self, device):
-        return (str(device),) + tuple(int(t._version) for t in list(self.parameters()) + list(self.buffers()))
-
-    @torch.no_grad()
-    def _pack(self, device) -> SwinV2NetC:
+    def _build(self, p) -> SwinV2NetC:
         """Kernel-side layouts (include/vdk_b200.h), once per weight version: bf16 Linear weights, the qkv bias
         cat(q_bias, 0, v_bias), the clamped logit scales and 16 sigmoid(cpb_mlp(table)) bias tables in fp32, the merge weights
         in (kh, kw, c) order, the folded neck."""
-        key = self._version_key(device)
-        if self._packed is not None and self._packed_key == key:
-            return self._packed["net"]
-        keep = []
-
-        def f32(t):
-            t = t.detach().to(device, torch.float32).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def bf16(t):
-            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
-            keep.append(t)
-            return t.data_ptr()
-
         m = self.model
         if sum(m.depths) > MAX_BLOCKS:
             raise ValueError(f"{self.model_name}: at most {MAX_BLOCKS} blocks")
@@ -249,46 +186,31 @@ class SwinV2Wrapper(nn.Module):
         net.image_size, net.feat_dim, net.embed_dim = self.image_size, self.feat_dim, m.embed_dim
         windows = stage_windows(m.window_size, self.image_size)
         pe = m.patch_embed
-        net.stem_w, net.stem_b = bf16(pe.proj.weight.reshape(m.embed_dim, 48)), f32(pe.proj.bias)
-        net.stem_ln_w, net.stem_ln_b = f32(pe.norm.weight), f32(pe.norm.bias)
+        net.stem_w, net.stem_b = p.bf16(pe.proj.weight.reshape(m.embed_dim, 48)), p.f32(pe.proj.bias)
+        net.stem_ln_w, net.stem_ln_b = p.f32(pe.norm.weight), p.f32(pe.norm.bias)
         blk = 0
         for i, stage in enumerate(m.layers):
             w, shift = windows[i]
             net.depths[i], net.window[i], net.shift[i] = m.depths[i], w, shift
             if i > 0:
                 ds = stage.downsample
-                net.merge_w[i] = bf16(merge_weight_khkw(ds.reduction.weight))
-                net.merge_ln_w[i], net.merge_ln_b[i] = f32(ds.norm.weight), f32(ds.norm.bias)
+                net.merge_w[i] = p.bf16(merge_weight_khkw(ds.reduction.weight))
+                net.merge_ln_w[i], net.merge_ln_b[i] = p.f32(ds.norm.weight), p.f32(ds.norm.bias)
             table = relative_coords_table(w, m.pretrained_window_sizes[i])
             for b in stage.blocks:
                 dst, a = net.blocks[blk], b.attn
                 blk += 1
-                dst.qkv_w = bf16(a.qkv.weight)
-                dst.qkv_b = f32(torch.cat([a.q_bias, torch.zeros_like(a.q_bias), a.v_bias]))
-                dst.attn_scale = f32(torch.clamp(a.logit_scale, max=math.log(100.0)).exp().reshape(-1))
-                dst.attn_bias = f32((16 * torch.sigmoid(a.cpb_mlp(table.to(a.logit_scale.device)))).t())
-                dst.proj_w, dst.proj_b = bf16(a.proj.weight), f32(a.proj.bias)
-                dst.norm1_w, dst.norm1_b = f32(b.norm1.weight), f32(b.norm1.bias)
-                dst.fc1_w, dst.fc1_b = bf16(b.mlp.fc1.weight), f32(b.mlp.fc1.bias)
-                dst.fc2_w, dst.fc2_b = bf16(b.mlp.fc2.weight), f32(b.mlp.fc2.bias)
-                dst.norm2_w, dst.norm2_b = f32(b.norm2.weight), f32(b.norm2.bias)
-        net.norm_w, net.norm_b = f32(m.norm.weight), f32(m.norm.bias)
+                dst.qkv_w = p.bf16(a.qkv.weight)
+                dst.qkv_b = p.f32(torch.cat([a.q_bias, torch.zeros_like(a.q_bias), a.v_bias]))
+                dst.attn_scale = p.f32(torch.clamp(a.logit_scale, max=math.log(100.0)).exp().reshape(-1))
+                dst.attn_bias = p.f32((16 * torch.sigmoid(a.cpb_mlp(table.to(a.logit_scale.device)))).t())
+                dst.proj_w, dst.proj_b = p.bf16(a.proj.weight), p.f32(a.proj.bias)
+                dst.norm1_w, dst.norm1_b = p.f32(b.norm1.weight), p.f32(b.norm1.bias)
+                dst.fc1_w, dst.fc1_b = p.bf16(b.mlp.fc1.weight), p.f32(b.mlp.fc1.bias)
+                dst.fc2_w, dst.fc2_b = p.bf16(b.mlp.fc2.weight), p.f32(b.mlp.fc2.bias)
+                dst.norm2_w, dst.norm2_b = p.f32(b.norm2.weight), p.f32(b.norm2.bias)
+        net.norm_w, net.norm_b = p.f32(m.norm.weight), p.f32(m.norm.bias)
         hw, c_last = self.image_size // 32, m.embed_dim * 8
-        w, bias = fold_nhwc_neck(self.output_layer, hw, hw * c_last, self.feat_dim, device)
-        net.neck_w, net.neck_b = bf16(w), f32(bias)
-        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+        w, bias = fold_nhwc_neck(self.output_layer, hw, hw * c_last, self.feat_dim, p.device)
+        net.neck_w, net.neck_b = p.bf16(w), p.f32(bias)
         return net
-
-    def _load_pretrained(self, model_name: str) -> None:
-        """Like TimmWrapper._load_pretrained: a timm state_dict from $VDK_PRETRAINED_DIR/<model_name>.pth (no network here);
-        the classifier (head.fc.*) and the buffers timm rebuilds (relative_position_index, relative_coords_table, attn_mask)
-        are dropped, as timm's own checkpoint filter does."""
-        root = os.environ.get("VDK_PRETRAINED_DIR")
-        path = os.path.join(root, f"{model_name}.pth") if root else None
-        if path and os.path.exists(path):
-            sd = torch.load(path, map_location="cpu")
-            sd = {k: v for k, v in sd.items()
-                  if not k.startswith(self._dropped) and not k.endswith(self._buffers_in_checkpoints)}
-            self.model.load_state_dict(sd, strict=True)
-        else:
-            warnings.warn(f"pretrained weights for '{model_name}' not found (set VDK_PRETRAINED_DIR); using random init")

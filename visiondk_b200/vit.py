@@ -15,12 +15,12 @@ head dims 72 and 80, a model without a class token (`model.cls_token` absent, po
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional
 
 import torch
 import torch.nn as nn
 
 from . import _lib
+from .wrapper import BackboneWrapper, fold_bn1d
 
 VIT_ARCHS = {
     # timm name -> (patch, embed_dim, depth, heads)
@@ -154,6 +154,7 @@ class VitTensorsC(C.Structure):
 
 class VitNetC(C.Structure):
     """vdk_vit_net (include/vdk_b200.h)."""
+    api = "vdk_vit"
     _fields_ = [("image_size", C.c_int), ("patch", C.c_int), ("dim", C.c_int), ("depth", C.c_int), ("heads", C.c_int),
                 ("feat_dim", C.c_int),
                 ("patch_w", C.c_void_p), ("patch_b", C.c_void_p), ("cls_token", C.c_void_p), ("pos_embed", C.c_void_p),
@@ -163,12 +164,11 @@ class VitNetC(C.Structure):
                 ("norm_pre_w", C.c_void_p), ("norm_pre_b", C.c_void_p), ("ln_eps", C.c_float), ("mlp_dim", C.c_int)]
 
 
-class ViTWrapper(nn.Module):
+class ViTWrapper(BackboneWrapper):
     """Drop-in for the reference's TimmWrapper when the timm model is a VisionTransformer (eval / extract path)."""
 
     def __init__(self, model_name: str, feat_dim: int, image_size: int, pretrained: bool = True, patch=None, dim=None, depth=None,
                  heads=None, pre_norm=None, mlp_dim=None, class_token=None, layer_scale=None, **kwargs):
-        super().__init__()
         if dim is None:
             if model_name not in VIT_ARCHS:
                 raise ValueError(f"backbone '{model_name}' is not built for H100 yet; available: {sorted(VIT_ARCHS)}")
@@ -185,27 +185,18 @@ class ViTWrapper(nn.Module):
                 mlp_dim % 8 != 0):
             raise ValueError("ViT on H100: image_size must be a multiple of patch, head_dim 64, 72 or 80, depth <= 48, mlp_dim a "
                              "multiple of 8")
-        self.model_name, self.feat_dim, self.image_size = model_name, int(feat_dim), int(image_size)
-        self.model = ViTParams(image_size, patch, dim, depth, heads, pre_norm=pre_norm, mlp_dim=mlp_dim, class_token=class_token,
-                               layer_scale=layer_scale)
-        tokens = self.model.tokens
-        self.output_layer = nn.Sequential(nn.LayerNorm(dim), nn.Flatten(1), nn.Linear(tokens * dim, feat_dim),
-                                          nn.BatchNorm1d(feat_dim))
-        self._packed: Optional[Dict] = None
-        self._packed_key = None
-        self._ws = None
-        self._train = None
         if pretrained:
             raise RuntimeError("pretrained timm weights cannot be downloaded here (no network): pass pretrained=False and "
                                "load a checkpoint with load_state_dict (keys are timm's)")
+        model = ViTParams(image_size, patch, dim, depth, heads, pre_norm=pre_norm, mlp_dim=mlp_dim, class_token=class_token,
+                          layer_scale=layer_scale)
+        output_layer = nn.Sequential(nn.LayerNorm(dim), nn.Flatten(1), nn.Linear(model.tokens * dim, feat_dim),
+                                     nn.BatchNorm1d(feat_dim))
+        super().__init__(model_name, feat_dim, image_size, model, output_layer, pretrained=False)
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if self.training and self.model.inference_only_features():
-            raise NotImplementedError(f"{self.model_name}: {', '.join(self.model.inference_only_features())}: built for inference / "
-                                      "extraction only")
-        if self.training:
-            return _ViTTrainFn.apply(self, x, *[p for _, p in self.named_parameters()])
-        return self.embed(x, l2_normalize=False)
+    def _train_refusal(self) -> str:
+        features = self.model.inference_only_features()
+        return f"{', '.join(features)}: built for inference / extraction only" if features else ""
 
     # ---- training path (csrc/vit.cu: vdk_vit_train_forward / vdk_vit_train_backward) -------------------------------------
     def _tensors_struct(self, get) -> VitTensorsC:
@@ -261,12 +252,7 @@ class ViTWrapper(nn.Module):
                            "neck_w": buf(self.feat_dim, tokens * m.dim),
                            "ones": torch.ones(m.dim, dtype=torch.float32, device=device)}
         st = self._train
-        named = dict(self.named_parameters())
-        named.update(dict(self.named_buffers()))
-        for n, t in named.items():
-            if t.is_floating_point() and (t.device != device or t.dtype != torch.float32 or not t.is_contiguous()):
-                raise RuntimeError(f"{n}: training needs contiguous fp32 parameters on {device}")
-        params = self._tensors_struct(lambda n: named[n].data_ptr())
+        params = self._master_tensors(device)
         net = VitNetC()
         net.image_size, net.patch, net.dim, net.depth, net.heads, net.feat_dim = (m.image_size, m.patch, m.dim, m.depth, m.heads,
                                                                                  self.feat_dim)
@@ -305,65 +291,7 @@ class ViTWrapper(nn.Module):
         st["last"] = (net, params, B)
         return out
 
-    def _train_backward(self, dout: torch.Tensor):
-        """Gradients of every parameter: accumulated straight into pre-allocated fp32 `.grad` buffers when every parameter owns
-        one (the fused optimizer's flat buffer), else produced in a scratch buffer and returned to autograd."""
-        lib = _lib.load()
-        st = self._train
-        net, params, B = st["last"]
-        plist = list(self.named_parameters())
-        direct = all(p.grad is not None and p.grad.dtype == torch.float32 and p.grad.is_contiguous() and
-                     p.grad.device == dout.device for _, p in plist)
-        if direct:
-            ptrs = {n: p.grad.data_ptr() for n, p in plist}
-        else:
-            total = sum(p.numel() for _, p in plist)
-            if st["gflat"] is None or st["gflat"].numel() != total:
-                st["gflat"] = torch.empty((total,), dtype=torch.float32, device=dout.device)
-            gflat = st["gflat"]
-            gflat.zero_()
-            offs, off = {}, 0
-            for n, p in plist:
-                offs[n] = off
-                off += p.numel()
-            ptrs = {n: gflat.data_ptr() + 4 * offs[n] for n, _ in plist}
-        grads = self._tensors_struct(lambda n: ptrs.get(n, 0))
-        dout = dout.contiguous().float()
-        hook = getattr(self, "grad_section_hook", None)
-        with torch.cuda.device(dout.device):
-            if hook is not None and direct:  # DDP overlap: reduce the gradients a unit range completed while the next one runs
-                for (u0, u1), names in self.backward_sections():
-                    _lib.check(lib.vdk_vit_train_backward_range(C.byref(net), C.byref(params), C.byref(grads), dout.data_ptr(), B,
-                                                                st["ws"].data_ptr(), st["ws"].numel(), _lib.stream_ptr(), u0, u1),
-                               "vdk_vit_train_backward_range")
-                    hook(names)
-            else:
-                _lib.check(lib.vdk_vit_train_backward(C.byref(net), C.byref(params), C.byref(grads), dout.data_ptr(), B,
-                                                      st["ws"].data_ptr(), st["ws"].numel(), _lib.stream_ptr()),
-                           "vdk_vit_train_backward")
-        if direct:
-            return [None] * len(plist)
-        return [gflat[offs[n]:offs[n] + p.numel()].view_as(p) for n, p in plist]
-
-    def _version_key(self, device):
-        return (str(device),) + tuple(int(t._version) for t in list(self.parameters()) + list(self.buffers()))
-
-    def _pack(self, device) -> VitNetC:
-        key = self._version_key(device)
-        if self._packed is not None and self._packed_key == key:
-            return self._packed["net"]
-        keep = []
-
-        def f32(t):
-            t = t.detach().to(device, torch.float32).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        def bf16(t):
-            t = t.detach().to(device, torch.float32).contiguous().to(torch.bfloat16)
-            keep.append(t)
-            return t.data_ptr()
-
+    def _build(self, p) -> VitNetC:
         m, net = self.model, VitNetC()
         net.image_size, net.patch, net.dim, net.depth, net.heads, net.feat_dim = (m.image_size, m.patch, m.dim, m.depth, m.heads,
                                                                                  self.feat_dim)
@@ -372,69 +300,28 @@ class ViTWrapper(nn.Module):
         w = m.patch_embed.proj.weight.detach().reshape(m.dim, k)  # (c, kh, kw) order
         if kp != k:
             w = torch.cat([w, torch.zeros(m.dim, kp - k, dtype=w.dtype, device=w.device)], dim=1)
-        net.patch_w = bf16(w)
-        net.patch_b = f32(m.patch_embed.proj.bias) if m.patch_embed.proj.bias is not None else 0
+        net.patch_w = p.bf16(w)
+        net.patch_b = p.f32(m.patch_embed.proj.bias) if m.patch_embed.proj.bias is not None else 0
         if m.pre_norm:
-            net.norm_pre_w, net.norm_pre_b = f32(m.norm_pre.weight), f32(m.norm_pre.bias)
+            net.norm_pre_w, net.norm_pre_b = p.f32(m.norm_pre.weight), p.f32(m.norm_pre.bias)
         net.ln_eps = float(m.ln_eps)
         net.mlp_dim = m.mlp_dim
-        net.cls_token = f32(m.cls_token.reshape(-1)) if m.class_token else 0
-        net.pos_embed = f32(m.pos_embed.reshape(-1, m.dim))
-        net.ones = f32(torch.ones(m.dim))
+        net.cls_token = p.f32(m.cls_token.reshape(-1)) if m.class_token else 0
+        net.pos_embed = p.f32(m.pos_embed.reshape(-1, m.dim))
+        net.ones = p.f32(torch.ones(m.dim))
         for i, blk in enumerate(m.blocks):
             b = net.blocks[i]
-            b.ln1_w, b.ln1_b = f32(blk.norm1.weight), f32(blk.norm1.bias)
-            b.qkv_w, b.qkv_b = bf16(blk.attn.qkv.weight), f32(blk.attn.qkv.bias)
-            b.proj_w, b.proj_b = bf16(blk.attn.proj.weight), f32(blk.attn.proj.bias)
-            b.ln2_w, b.ln2_b = f32(blk.norm2.weight), f32(blk.norm2.bias)
-            b.fc1_w, b.fc1_b = bf16(blk.mlp.fc1.weight), f32(blk.mlp.fc1.bias)
-            b.fc2_w, b.fc2_b = bf16(blk.mlp.fc2.weight), f32(blk.mlp.fc2.bias)
+            b.ln1_w, b.ln1_b = p.f32(blk.norm1.weight), p.f32(blk.norm1.bias)
+            b.qkv_w, b.qkv_b = p.bf16(blk.attn.qkv.weight), p.f32(blk.attn.qkv.bias)
+            b.proj_w, b.proj_b = p.bf16(blk.attn.proj.weight), p.f32(blk.attn.proj.bias)
+            b.ln2_w, b.ln2_b = p.f32(blk.norm2.weight), p.f32(blk.norm2.bias)
+            b.fc1_w, b.fc1_b = p.bf16(blk.mlp.fc1.weight), p.f32(blk.mlp.fc1.bias)
+            b.fc2_w, b.fc2_b = p.bf16(blk.mlp.fc2.weight), p.f32(blk.mlp.fc2.bias)
             if m.layer_scale:
-                b.ls1, b.ls2 = f32(blk.ls1.gamma), f32(blk.ls2.gamma)
-        net.norm_w, net.norm_b = f32(m.norm.weight), f32(m.norm.bias)
-        ln, lin, bn = self.output_layer[0], self.output_layer[2], self.output_layer[3]
-        net.neck_ln_w, net.neck_ln_b = f32(ln.weight), f32(ln.bias)
-        # BatchNorm1d (eval statistics) folded into the Linear: y = s * (W x + b - mean) + beta, s = gamma / sqrt(var + eps)
-        s = (bn.weight.detach().double() / torch.sqrt(bn.running_var.detach().double() + bn.eps))
-        wn = lin.weight.detach().double() * s[:, None]
-        bnb = (lin.bias.detach().double() - bn.running_mean.detach().double()) * s + bn.bias.detach().double()
-        net.neck_w, net.neck_b = bf16(wn.float()), f32(bnb.float())
-        self._packed, self._packed_key = {"net": net, "keep": keep}, key
+                b.ls1, b.ls2 = p.f32(blk.ls1.gamma), p.f32(blk.ls2.gamma)
+        net.norm_w, net.norm_b = p.f32(m.norm.weight), p.f32(m.norm.bias)
+        ln, lin = self.output_layer[0], self.output_layer[2]
+        net.neck_ln_w, net.neck_ln_b = p.f32(ln.weight), p.f32(ln.bias)
+        w, bias = fold_bn1d(lin.weight.detach().double(), lin.bias.detach().double(), self.output_layer[3])
+        net.neck_w, net.neck_b = p.bf16(w), p.f32(bias)
         return net
-
-    @torch.no_grad()
-    def embed(self, x: torch.Tensor, l2_normalize: bool = False) -> torch.Tensor:
-        """[B,3,S,S] fp32 NCHW -> fp32 [B, feat_dim] (TimmWrapper.forward in eval mode; optionally F.normalize fused)."""
-        lib = _lib.load()
-        if x.device.type != "cuda":
-            raise RuntimeError("visiondk_b200.ViTWrapper runs on CUDA (sm_90a) only; there is no CPU fallback")
-        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
-            raise ValueError(f"expected [B,3,{self.image_size},{self.image_size}], got {tuple(x.shape)}")
-        x = x.contiguous().float()
-        net = self._pack(x.device)
-        B = x.shape[0]
-        out = torch.empty((B, self.feat_dim), dtype=torch.float32, device=x.device)
-        need = lib.vdk_vit_workspace_bytes(C.byref(net), B)
-        if need == 0:
-            raise RuntimeError("vdk_vit_workspace_bytes: " + _lib.last_error())
-        if self._ws is None or self._ws.numel() < need or self._ws.device != x.device:
-            self._ws = torch.empty((need,), dtype=torch.uint8, device=x.device)
-        with torch.cuda.device(x.device):
-            _lib.check(lib.vdk_vit_forward(C.byref(net), x.data_ptr(), B, int(l2_normalize), out.data_ptr(), self._ws.data_ptr(),
-                                           self._ws.numel(), _lib.stream_ptr()), "vdk_vit_forward")
-        return out
-
-
-class _ViTTrainFn(torch.autograd.Function):
-    """Train-mode forward/backward of the whole ViT + neck as one autograd node (csrc/vit.cu)."""
-
-    @staticmethod
-    def forward(ctx, module, x, *params):
-        ctx.module = module
-        return module._train_forward(x)
-
-    @staticmethod
-    def backward(ctx, dout):
-        grads = ctx.module._train_backward(dout)
-        return (None, None, *grads)
-
