@@ -56,6 +56,7 @@ int vdk_device_check(void);
  * relative error <= 1e-6 for |x| <= 64 before the output rounding. */
 #define VDK_EPI_SILU 7           /* D = silu(acc + bias[n])  (conv + folded BatchNorm + SiLU) */
 #define VDK_EPI_SILU_RESIDUAL 8  /* D = residual[m,n] + silu(acc + bias[n])  (timm's ConvBnAct with skip: the activation first) */
+#define VDK_EPI_HARDSWISH 9      /* D = v relu6(v + 3) / 6 with v = acc + bias[n]  (MobileNetV3's hard-swish, nn.Hardswish) */
 
 typedef struct vdk_gemm_desc {
   const void* A; /* [M,K] 16-bit, pitch lda */
@@ -135,8 +136,9 @@ int vdk_conv2d_grouped(const vdk_conv_desc* desc, int groups, void* stream);
  * kernel, stride and pad as vdk_conv2d.  groups = 1 takes a 1x1 / stride-1 kernel only and runs as vdk_conv2d's plain GEMM
  * with K = Cin (w [Cout, Cin]), so that Cin need not be a multiple of 64 (ResNeSt's conv3). */
 int vdk_conv2d_grouped_ex(const vdk_conv_desc* desc, int groups, void* stream);
-/* Extended form for TensorFlow-"same" padded MBConv networks (timm's tf_efficientnetv2_*, timm/models/_efficientnet_blocks.py
- * with Conv2dSame): separate low and high zero padding per axis, the SiLU epilogues, and Cin any multiple of 8.
+/* Extended form for TensorFlow-"same" padded MBConv networks (timm's tf_efficientnetv2_* and *mobilenetv3_*,
+ * timm/models/_efficientnet_blocks.py with Conv2dSame): separate low and high zero padding per axis, the SiLU and hard-swish
+ * epilogues, and Cin any multiple of 8.
  * Ho = (H + pad_h_lo + pad_h_hi - kernel) / stride + 1, likewise Wo.  1x1 / stride-1 / unpadded convolutions run as a plain
  * GEMM over [B*H*W, Cin] with w [Cout, Cin]; every other shape is an implicit GEMM whose K blocks are 64 channels of one
  * tap, so w is [Cout, kernel, kernel, Cinp] with Cinp = Cin rounded up to a multiple of 64 and zero columns from Cin on
@@ -150,7 +152,7 @@ typedef struct vdk_conv_ex_desc {
   int B, H, W, Cin, Cout;
   int kernel, stride;
   int pad_h_lo, pad_h_hi, pad_w_lo, pad_w_hi; /* each in [0, kernel) */
-  int epilogue; /* VDK_EPI_NONE, VDK_EPI_SILU or VDK_EPI_SILU_RESIDUAL */
+  int epilogue; /* VDK_EPI_NONE, VDK_EPI_SILU, VDK_EPI_SILU_RESIDUAL or VDK_EPI_HARDSWISH */
 } vdk_conv_ex_desc;
 /* Cin and Cout multiples of 8, 1 <= kernel <= 16, 1 <= stride <= 8. */
 int vdk_conv2d_ex(const vdk_conv_ex_desc* desc, void* stream);
@@ -296,6 +298,73 @@ int vdk_dwconv3_silu(const void* x, int B, int H, int W, int C, int stride, cons
  * <= 4096): gate [B, C] fp32 = sigmoid(w2 silu(w1 mean + b1) + b2) (w1 [rd, C], w2 [C, rd]), then d = d * gate in place. */
 int vdk_effnet_se(void* d, const float* mean, int B, int HW, int C, int rd, const float* w1, const float* b1, const float* w2,
                   const float* b2, float* gate, void* stream);
+
+/* ---- MobileNetV3 embedding forward (eval) -------------------------------------------------------- */
+/* Replaces TimmWrapper.forward for timm's MobileNetV3s at width 1.0 (tf_mobilenetv3_large_minimal_100, tf_mobilenetv3_large_100,
+ * tf_mobilenetv3_small_100, tf_mobilenetv3_small_minimal_100, mobilenetv3_large_100, mobilenetv3_small_100;
+ * timm/models/mobilenetv3.py, _efficientnet_blocks.py; models/faceX/backbone/timm_wrapper.py:16-21, 30-38, 51-54) followed
+ * by F.normalize (face_model.py:139).  Every eval BatchNorm folded into its conv; NHWC bf16 activations in `workspace`.
+ * act is ReLU or hard-swish per conv; padding is TF-"same" (tf_*) or symmetric k / 2.  Blocks, with a shortcut when
+ * stride == 1 and cin == cout:
+ *   DS (DepthwiseSeparable)  d = act(dwconv_k/s(x)); [d = d * hsig(W2 relu(W1 mean_hw(d) + b1) + b2)]; out = conv_pw(d) [+ x]
+ *   IR (InvertedResidual)    e = act(conv_pw(x)); d = act(dwconv_k/s(e)); [SE as DS]; out = conv_pwl(d) [+ x]
+ *   CN (ConvBnAct 1x1)       out = act(conv(x))
+ * with hsig(v) = relu6(v + 3) / 6; then conv_head 1x1 (with bias) + act on the unpooled map and the folded CNN neck. */
+#define VDK_MOBILENETV3_MAX_BLOCKS 24
+#define VDK_MNV3_DS 0
+#define VDK_MNV3_IR 1
+#define VDK_MNV3_CN 2
+#define VDK_ACT_RELU 0
+#define VDK_ACT_HARDSWISH 1
+#define VDK_PAD_SAME 0      /* TensorFlow "same": per axis total = max((ceil(H / s) - 1) s + k - H, 0), lo = total / 2 */
+#define VDK_PAD_SYMMETRIC 1 /* k / 2 on every side */
+typedef struct vdk_mobilenetv3_block {
+  int kind;   /* VDK_MNV3_DS, _IR or _CN */
+  int kernel; /* depthwise k: 3 or 5 (CN: 1) */
+  int stride; /* 1 or 2 (CN: 1) */
+  int cin, mid, cout; /* mid: the depthwise width (DS: cin; CN: cout), a multiple of 8 */
+  int act;    /* VDK_ACT_RELU or VDK_ACT_HARDSWISH */
+  int se_rd;  /* the SE bottleneck width; 0: no SE */
+  vdk_resnet_conv conv;     /* IR conv_pw [mid, cin] / CN conv [cout, cin]; unused for DS */
+  const float* dw_w;        /* DS, IR: fp32 [k*k, mid] taps in (dy, dx) order */
+  const float* dw_b;        /* [mid] */
+  const float* se_w1;       /* fp32 [se_rd, mid] conv_reduce */
+  const float* se_b1;       /* [se_rd] */
+  const float* se_w2;       /* [mid, se_rd] conv_expand */
+  const float* se_b2;       /* [mid] */
+  vdk_resnet_conv conv_pwl; /* DS conv_pw / IR conv_pwl: [cout, mid] */
+} vdk_mobilenetv3_block;
+typedef struct vdk_mobilenetv3_net {
+  int image_size; /* square input side, multiple of 32 */
+  int feat_dim;   /* embedding width, multiple of 8 */
+  int num_blocks;
+  int pad;        /* VDK_PAD_SAME or VDK_PAD_SYMMETRIC */
+  int stem_ch;    /* conv_stem 3x3/s2 3 -> stem_ch, as a GEMM over zero-padded (kh, kw, c) rows: stem.w [stem_ch, 64] */
+  int stem_act;   /* VDK_ACT_* */
+  int head_ch;    /* conv_head 1x1 width (1280 large, 1024 small) */
+  int head_act;   /* VDK_ACT_* */
+  vdk_resnet_conv stem;
+  vdk_mobilenetv3_block blocks[VDK_MOBILENETV3_MAX_BLOCKS];
+  vdk_resnet_conv head; /* [head_ch, cout of the last block], conv_head's own bias */
+  const void* neck_w;   /* [feat_dim, h*w*head_ch] bf16, K order (h, w, c), BN2d/BN1d eval statistics folded in */
+  const float* neck_b;  /* [feat_dim] */
+} vdk_mobilenetv3_net;
+size_t vdk_mobilenetv3_workspace_bytes(const vdk_mobilenetv3_net* net, int batch);
+/* images: fp32 NCHW [batch,3,S,S]; embeddings: fp32 [batch, feat_dim], L2-normalised when l2_normalize != 0. */
+int vdk_mobilenetv3_forward(const vdk_mobilenetv3_net* net, const float* images, int batch, int l2_normalize, float* embeddings,
+                            void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_mobilenetv3_net. */
+int vdk_mobilenetv3_struct_sizes(size_t* out, int n);
+/* The DS / IR block's depthwise conv alone: y [B, Ho, Wo, C] bf16 = act(dwconv_k(x) + b) over x [B, H, W, C] bf16 (C a multiple
+ * of 8, <= 4096), k 3 or 5, stride 1 or 2, padding VDK_PAD_SAME or VDK_PAD_SYMMETRIC (Ho = ceil(H / stride) either way for
+ * the even maps of the models; in general Ho = (H + lo + hi - k) / stride + 1), w fp32 [k*k, C], fp32 FMAs in (bias, dy, dx)
+ * order.  mean [B, C] fp32 (may be NULL) = the spatial mean of the bf16 y, summed in a fixed order (bit-reproducible). */
+int vdk_dwconv_mnv3(const void* x, int B, int H, int W, int C, int kernel, int stride, int pad, int act, const float* w,
+                    const float* b, void* y, float* mean, void* stream);
+/* The SE gate alone, on the depthwise output d [B, HW, C] bf16 and its mean [B, C] fp32 (C a multiple of 8, <= 4096):
+ * gate [B, C] fp32 = relu6(w2 relu(w1 mean + b1) + b2 + 3) / 6 (w1 [rd, C], w2 [C, rd]), then d = d * gate in place. */
+int vdk_mnv3_se(void* d, const float* mean, int B, int HW, int C, int rd, const float* w1, const float* b1, const float* w2,
+                const float* b2, float* gate, void* stream);
 
 /* ---- ResNeSt embedding forward (eval) ------------------------------------------------------------ */
 /* Replaces TimmWrapper.forward for timm's ResNeSts with the width-32 deep stem (resnest14d, 26d, 50d, 50d_1s4x24d,

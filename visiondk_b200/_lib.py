@@ -17,6 +17,7 @@ DTYPE_BF16, DTYPE_FP16, DTYPE_FP32 = 0, 1, 2
 EPI_NONE, EPI_GELU, EPI_SCALE_RESIDUAL, EPI_LAYERNORM, EPI_MUL_GELU_GRAD = 0, 1, 2, 3, 4
 EPI_RELU, EPI_RESIDUAL_RELU = 5, 6  # vdk_conv2d only
 EPI_SILU, EPI_SILU_RESIDUAL = 7, 8  # vdk_conv2d_ex only
+EPI_HARDSWISH = 9  # vdk_conv2d_ex only
 
 
 class HeadDesc(C.Structure):
@@ -108,6 +109,11 @@ SIGNATURES = {
     "vdk_effnetv2_struct_sizes": (_i, [_p, _i]),
     "vdk_dwconv3_silu": (_i, [_p, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),
     "vdk_effnet_se": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
+    "vdk_mobilenetv3_workspace_bytes": (_sz, [_p, _i]),
+    "vdk_mobilenetv3_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
+    "vdk_mobilenetv3_struct_sizes": (_i, [_p, _i]),
+    "vdk_dwconv_mnv3": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "vdk_mnv3_se": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
     "vdk_swinv2_workspace_bytes": (_sz, [_p, _i]),
     "vdk_swinv2_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),
     "vdk_swinv2_struct_sizes": (_i, [_p, _i]),

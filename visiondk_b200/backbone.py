@@ -335,4 +335,7 @@ class BackboneFactory:
         if model_name.startswith("tf_efficientnetv2_"):  # EfficientNetV2: eval / extract path (visiondk_b200/efficientnet.py)
             from .efficientnet import EfficientNetV2Wrapper
             return EfficientNetV2Wrapper(model_name=model_name, **self.backbone_param)
+        if model_name.startswith(("mobilenetv3_", "tf_mobilenetv3_")):  # MobileNetV3: eval / extract path
+            from .mobilenetv3 import MobileNetV3Wrapper  # (visiondk_b200/mobilenetv3.py); other widths / variants refused
+            return MobileNetV3Wrapper(model_name=model_name, **self.backbone_param)
         return TimmWrapper(model_name=model_name, **self.backbone_param)

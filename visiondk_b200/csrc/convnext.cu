@@ -848,8 +848,6 @@ int launch_neck_finalize(const float* slabs, int n_slabs, size_t slab_stride, in
   return VDK_OK;
 }
 
-static size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-
 int launch_neck(const __nv_bfloat16* feats, int batch, int Kn, int F, const void* neck_w, const float* neck_b, int l2_normalize,
                 float* scratch, size_t scratch_bytes, float* embeddings, cudaStream_t s) {
   const int tiles = ((batch + 127) / 128) * ((F + 255) / 256);

@@ -29,11 +29,11 @@ int launch_neck(const __nv_bfloat16* feats, int batch, int Kn, int F, const void
 int launch_neck_finalize(const float* slabs, int n_slabs, size_t slab_stride, int B, int F, const float* bias, int l2norm,
                          float* out, cudaStream_t s);
 
-// ---- CNN pieces of resnet.cu shared with effnet.cu ----
-// gate[b, :] = sigmoid(w2 act(w1 mean[b, :] + b1) + b2) in fp32, act = ReLU (silu_hidden 0) or SiLU (1); C + rd floats of
-// shared memory
-int launch_se_excite(const float* mean, int batch, int C, int rd, int silu_hidden, const float* w1, const float* b1,
-                     const float* w2, const float* b2, float* gate, cudaStream_t s);
+// ---- CNN pieces of resnet.cu shared with effnet.cu and mobilenetv3.cu ----
+// gate[b, :] = g(w2 act(w1 mean[b, :] + b1) + b2) in fp32, act = ReLU (silu_hidden 0) or SiLU (1), g = sigmoid (hard_gate 0)
+// or relu6(v + 3) / 6 (1); C + rd floats of shared memory
+int launch_se_excite(const float* mean, int batch, int C, int rd, int silu_hidden, int hard_gate, const float* w1,
+                     const float* b1, const float* w2, const float* b2, float* gate, cudaStream_t s);
 // explicit im2col rows of fp32 NCHW images: out[m][(dy k + dx) C + c] bf16, zero outside the image and from k*k*C to Kp
 int launch_patch_rows_nchw(const float* x, int B, int H, int W, int C, int k, int stride, int pad, int Ho, int Wo, int Kp,
                            __nv_bfloat16* out, cudaStream_t s);
@@ -42,6 +42,23 @@ int launch_patch_rows_nhwc(const __nv_bfloat16* x, int B, int H, int W, int C, i
                            __nv_bfloat16* out, cudaStream_t s);
 // timm's ResNet stem pool MaxPool2d(3, 2, padding 1) over NHWC bf16 (C a multiple of 8)
 int launch_stem_maxpool(const __nv_bfloat16* x, int B, int H, int W, int C, __nv_bfloat16* y, cudaStream_t s);
+
+// ---- MBConv pieces of effnet.cu shared with mobilenetv3.cu ----
+// d[m, c] = bf16(d[m, c] * gate[m / HW, c]) in place over d [M, C] bf16 (C a multiple of 8)
+int launch_se_apply(__nv_bfloat16* d, const float* gate, int64_t M, int HW, int C, cudaStream_t s);
+// p[0 .. n) = v
+int launch_fill(float* p, int n, float v, cudaStream_t s);
+
+inline size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
+// a grid-stride launch over `threads` threads: at most 16 CTAs of 256 per SM of the H100's 132
+inline int grid_for(int64_t threads) { return static_cast<int>((threads + 255) / 256 < 132 * 16 ? (threads + 255) / 256 : 132 * 16); }
+// TensorFlow "same" padding of one axis: the output has ceil(H / s) positions
+inline void same_pad(int H, int k, int s, int& lo, int& hi) {
+  const int out = (H + s - 1) / s;
+  const int total = (out - 1) * s + k - H > 0 ? (out - 1) * s + k - H : 0;
+  lo = total / 2;
+  hi = total - lo;
+}
 
 }  // namespace vdk
 

@@ -133,15 +133,16 @@ __global__ void fill_kernel(float* p, int n, float v) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = v;
 }
 
-static size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-static int grid_for(int64_t threads) { return static_cast<int>(std::min<int64_t>((threads + 255) / 256, 132 * 16)); }
+int launch_se_apply(__nv_bfloat16* d, const float* gate, int64_t M, int HW, int C, cudaStream_t s) {
+  se_apply_kernel<<<grid_for(M * (C / 8)), 256, 0, s>>>(d, gate, M, HW, C);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
 
-// TensorFlow "same" padding of one axis: the output has ceil(H / s) positions
-static void same_pad(int H, int k, int s, int& lo, int& hi) {
-  const int out = (H + s - 1) / s;
-  const int total = std::max((out - 1) * s + k - H, 0);
-  lo = total / 2;
-  hi = total - lo;
+int launch_fill(float* p, int n, float v, cudaStream_t s) {
+  fill_kernel<<<1, 256, 0, s>>>(p, n, v);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
 }
 
 static int dw_run(const __nv_bfloat16* x, int B, int H, int W, int C, int stride, const float* w, const float* b,
@@ -161,12 +162,9 @@ static int dw_run(const __nv_bfloat16* x, int B, int H, int W, int C, int stride
 static int se_run(__nv_bfloat16* d, const float* mean, int B, int HW, int C, int rd, const float* w1, const float* b1,
                   const float* w2, const float* b2, float* gate, cudaStream_t s) {
   ProfScope prof(kProfOther, 4.0 * B * C * rd + static_cast<double>(B) * HW * C, 4.0 * B * static_cast<double>(HW) * C, s);
-  int rc = launch_se_excite(mean, B, C, rd, 1, w1, b1, w2, b2, gate, s);
+  int rc = launch_se_excite(mean, B, C, rd, 1, 0, w1, b1, w2, b2, gate, s);
   if (rc != VDK_OK) return rc;
-  const int64_t M = static_cast<int64_t>(B) * HW;
-  se_apply_kernel<<<grid_for(M * (C / 8)), 256, 0, s>>>(d, gate, M, HW, C);
-  VDK_CUDA_OK(cudaGetLastError());
-  return VDK_OK;
+  return launch_se_apply(d, gate, static_cast<int64_t>(B) * HW, HW, C, s);
 }
 
 static int check_effnet(const vdk_effnetv2_net* n) {
@@ -266,8 +264,7 @@ extern "C" int vdk_effnetv2_forward(const vdk_effnetv2_net* net, const float* im
   ws += up256(static_cast<size_t>(batch) * z.max_mid * 4);
   float* ones = reinterpret_cast<float*>(ws);
   __nv_bfloat16 *x = buf[0], *y = buf[1], *e = buf[2], *d = buf[3];
-  fill_kernel<<<1, 256, 0, s>>>(ones, z.max_cout, 1.f);
-  VDK_CUDA_OK(cudaGetLastError());
+  if ((rc = launch_fill(ones, z.max_cout, 1.f, s)) != VDK_OK) return rc;
 
   // TF-"same" k x k convolution on vdk_conv2d_ex
   auto conv = [&](const void* in, int H, int Cin, const vdk_resnet_conv& c, int Cout, int k, int stride, int epi, const void* res,

@@ -34,7 +34,8 @@ constexpr int kConvIm2col = 2;  // k x k / stride-s convolution: A tiles gathere
 // grouped k x k convolution (vdk_conv2d_grouped, BN = 128): the N tile at n0 contracts over input channels n0 .. n0 + 127
 // only (whole groups, block-diagonal B), so its K block kb = (tap kb / 2, channels n0 + (kb % 2) * 64)
 constexpr int kConvGrouped = 3;
-// vdk_conv2d_ex (TF-"same" padded MBConv convolutions): as kConvDense / kConvIm2col, plus the SiLU epilogues.  cv_pad holds
+// vdk_conv2d_ex (TF-"same" padded MBConv convolutions): as kConvDense / kConvIm2col, plus the SiLU and hard-swish
+// epilogues.  cv_pad holds
 // the low padding of both axes (h | w << 8); the high padding only shapes the im2col map.  Cin a multiple of 8: a K block
 // still loads 64 channels of one tap, the channels past Cin arrive as TMA zero fill and meet zero weight columns.
 constexpr int kConvExDense = 4;
@@ -230,6 +231,9 @@ __device__ __forceinline__ void epi_pair(const GemmParams& p, float& x0, float& 
     } else if (p.epilogue == VDK_EPI_SILU_RESIDUAL) {
       x0 = silu_fast(x0) + r.x;
       x1 = silu_fast(x1) + r.y;
+    } else if (p.epilogue == VDK_EPI_HARDSWISH) {
+      x0 = hardswish(x0);
+      x1 = hardswish(x1);
     }
   }
 }
@@ -881,7 +885,7 @@ int conv_run(const vdk_conv_desc& c, cudaStream_t s) {
                      s);
 }
 
-int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t s) {
+int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t s, bool allow_relu) {
   VDK_REQUIRE(c.x && c.w && c.y, "vdk_conv2d_ex: null operand");
   VDK_REQUIRE(c.B > 0 && c.H > 0 && c.W > 0, "vdk_conv2d_ex: empty input B=%d H=%d W=%d", c.B, c.H, c.W);
   VDK_REQUIRE(c.Cin > 0 && c.Cin % 8 == 0, "vdk_conv2d_ex: Cin must be a positive multiple of 8 (Cin=%d)", c.Cin);
@@ -894,8 +898,9 @@ int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t s) {
               "vdk_conv2d_ex: pads (%d, %d, %d, %d) must lie in [0, kernel)", c.pad_h_lo, c.pad_h_hi, c.pad_w_lo, c.pad_w_hi);
   VDK_REQUIRE(c.H + c.pad_h_lo + c.pad_h_hi >= c.kernel && c.W + c.pad_w_lo + c.pad_w_hi >= c.kernel,
               "vdk_conv2d_ex: kernel larger than the padded input");
-  VDK_REQUIRE(c.epilogue == VDK_EPI_NONE || c.epilogue == VDK_EPI_SILU || c.epilogue == VDK_EPI_SILU_RESIDUAL,
-              "vdk_conv2d_ex: epilogue must be NONE, SILU or SILU_RESIDUAL (got %d)", c.epilogue);
+  VDK_REQUIRE(c.epilogue == VDK_EPI_NONE || c.epilogue == VDK_EPI_SILU || c.epilogue == VDK_EPI_SILU_RESIDUAL ||
+                  c.epilogue == VDK_EPI_HARDSWISH || (allow_relu && c.epilogue == VDK_EPI_RELU),
+              "vdk_conv2d_ex: epilogue must be NONE, SILU, SILU_RESIDUAL or HARDSWISH (got %d)", c.epilogue);
   VDK_REQUIRE((c.epilogue == VDK_EPI_SILU_RESIDUAL) == (c.residual != nullptr),
               "vdk_conv2d_ex: a residual is given exactly with the SILU_RESIDUAL epilogue");
   VDK_REQUIRE((reinterpret_cast<uintptr_t>(c.x) & 15) == 0 && (reinterpret_cast<uintptr_t>(c.w) & 15) == 0 &&

@@ -24,9 +24,6 @@ constexpr int kExciteImgs = 8;        // images per attn_excite CTA: each weight
 constexpr int kExciteChannels = 256;  // output channels c (all R radix rows of each) per attn_excite CTA
 constexpr int kMaxRadix = 4;
 
-size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-int grid_for(int64_t threads) { return static_cast<int>(std::min<int64_t>((threads + 255) / 256, 132 * 16)); }
-
 __device__ __forceinline__ void load8(const __nv_bfloat16* p, float* f) {
   const uint4 u = *reinterpret_cast<const uint4*>(p);
   const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);

@@ -146,13 +146,14 @@ __global__ void __launch_bounds__(256) se_mean_kernel(const __nv_bfloat16* __res
   }
 }
 
-// se_excite: s[b, :] = sigmoid(fc2(act(fc1(mean[b, :]) + b1)) + b2) in fp32, one block of 256 threads per image; act is
-// ReLU (the legacy SENets) or SiLU (EfficientNetV2, silu_hidden).  fc1: one warp per hidden unit, lanes over C, a fixed
-// shuffle tree; fc2: one thread per channel, sequential over rd.
+// se_excite: s[b, :] = gate(fc2(act(fc1(mean[b, :]) + b1)) + b2) in fp32, one block of 256 threads per image; act is
+// ReLU (the legacy SENets, MobileNetV3) or SiLU (EfficientNetV2, silu_hidden); gate is sigmoid, or MobileNetV3's hard
+// sigmoid relu6(v + 3) / 6 (hard_gate).  fc1: one warp per hidden unit, lanes over C, a fixed shuffle tree; fc2: one thread
+// per channel, sequential over rd.
 __global__ void __launch_bounds__(256) se_excite_kernel(const float* __restrict__ mean, int C, int rd,
                                                         const float* __restrict__ w1, const float* __restrict__ b1,
                                                         const float* __restrict__ w2, const float* __restrict__ b2,
-                                                        float* __restrict__ s, int silu_hidden) {
+                                                        float* __restrict__ s, int silu_hidden, int hard_gate) {
   extern __shared__ float se_smem[];
   float* m = se_smem;       // [C]
   float* hid = se_smem + C;  // [rd]
@@ -175,7 +176,8 @@ __global__ void __launch_bounds__(256) se_excite_kernel(const float* __restrict_
     const float* wr = w2 + static_cast<int64_t>(c) * rd;
     float a = 0.f;
     for (int j = 0; j < rd; ++j) a = fmaf(wr[j], hid[j], a);
-    s[static_cast<int64_t>(b) * C + c] = 1.f / (1.f + expf(-(a + b2[c])));
+    const float v = a + b2[c];
+    s[static_cast<int64_t>(b) * C + c] = hard_gate ? fminf(fmaxf(v + 3.f, 0.f), 6.f) / 6.f : 1.f / (1.f + expf(-v));
   }
 }
 
@@ -209,13 +211,9 @@ __global__ void __launch_bounds__(256) se_scale_kernel(const __nv_bfloat16* __re
   }
 }
 
-static size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-
-static int grid_for(int64_t threads) { return static_cast<int>(std::min<int64_t>((threads + 255) / 256, 132 * 16)); }
-
-int launch_se_excite(const float* mean, int batch, int C, int rd, int silu_hidden, const float* w1, const float* b1,
-                     const float* w2, const float* b2, float* gate, cudaStream_t s) {
-  se_excite_kernel<<<batch, 256, (C + rd) * sizeof(float), s>>>(mean, C, rd, w1, b1, w2, b2, gate, silu_hidden);
+int launch_se_excite(const float* mean, int batch, int C, int rd, int silu_hidden, int hard_gate, const float* w1,
+                     const float* b1, const float* w2, const float* b2, float* gate, cudaStream_t s) {
+  se_excite_kernel<<<batch, 256, (C + rd) * sizeof(float), s>>>(mean, C, rd, w1, b1, w2, b2, gate, silu_hidden, hard_gate);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }
@@ -378,7 +376,7 @@ static int se_gate(const __nv_bfloat16* y, int batch, int HW, int C, int rd, con
   int rc;
   se_mean_kernel<<<dim3(C / 64, batch), 256, 0, s>>>(y, HW, C, mean);
   VDK_CUDA_OK(cudaGetLastError());
-  if ((rc = launch_se_excite(mean, batch, C, rd, 0, w1, b1, w2, b2, sc, s)) != VDK_OK) return rc;
+  if ((rc = launch_se_excite(mean, batch, C, rd, 0, 0, w1, b1, w2, b2, sc, s)) != VDK_OK) return rc;
   const int64_t M = static_cast<int64_t>(batch) * HW;
   se_scale_kernel<<<grid_for(M * (C / 8)), 256, 0, s>>>(y, sc, M, HW, C, res);
   VDK_CUDA_OK(cudaGetLastError());

@@ -331,8 +331,6 @@ static int launch_postnorm_residual(__nv_bfloat16* x, const __nv_bfloat16* y, in
   return VDK_OK;
 }
 
-static size_t up256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-
 static int check_swinv2(const vdk_swinv2_net* n) {
   VDK_REQUIRE(n, "vdk_swinv2: null network");
   VDK_REQUIRE(n->image_size == 256, "vdk_swinv2: image_size must be 256, the towers' size (got %d)", n->image_size);

@@ -82,7 +82,8 @@ int conv_run(const vdk_conv_desc& c, cudaStream_t stream);
 // Internal form of vdk_conv2d_grouped (the ResNeXt / SE-ResNeXt forward).
 int conv_grouped_run(const vdk_conv_desc& c, int groups, cudaStream_t stream);
 // Internal form of vdk_conv2d_ex (the EfficientNetV2 forward).
-int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t stream);
+// allow_relu: also take VDK_EPI_RELU, which the public vdk_conv2d_ex keeps refusing (the MobileNetV3 forward's 1x1s use it)
+int conv_ex_run(const vdk_conv_ex_desc& c, cudaStream_t stream, bool allow_relu = false);
 // Internal form of vdk_conv2d_grouped_ex (the ResNeSt forward), and the 64-channel blocks per tap its packed weight holds.
 int conv_grouped_ex_run(const vdk_conv_desc& c, int groups, cudaStream_t stream);
 int conv_grouped_ex_cpb(int Cin, int Cout, int groups);

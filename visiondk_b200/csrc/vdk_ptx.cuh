@@ -13,6 +13,9 @@
 
 namespace vdk {
 
+// nn.Hardswish in fp32: x relu6(x + 3) / 6, the 1/6 as a multiply (within 2^-21 |y| of the exact value)
+__device__ __forceinline__ float hardswish(float x) { return x * fminf(fmaxf(x + 3.f, 0.f), 6.f) * (1.f / 6.f); }
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

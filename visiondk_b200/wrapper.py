@@ -1,4 +1,5 @@
-"""What every extraction backbone wrapper shares (ConvNeXt, ViT, ResNet / ResNeXt, SENet, ResNeSt, EfficientNetV2, Swin V2).
+"""What every extraction backbone wrapper shares (ConvNeXt, ViT, ResNet / ResNeXt, SENet, ResNeSt, EfficientNetV2, MobileNetV3,
+Swin V2).
 
 `BackboneWrapper` keeps the reference TimmWrapper's surface (`model.` / `output_layer.` parameters, `forward(x) -> [B,
 feat_dim]`) and owns the host side around the family's kernels: the weight-pack cache, `embed`, the checkpoint load and, for
