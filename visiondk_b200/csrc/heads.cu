@@ -8,9 +8,14 @@
 //
 // The reference runs this path in fp32 (no autocast, train.py:227).  The class-logit contraction cos = f~ . W~ and the
 // two gradient contractions run on the wgmma GEMM with a 3-way bf16 split of every fp32 operand
-// (x = p0 + p1 + p2, 8 mantissa bits each; the six products with i + j <= 2 are laid side by side along K), which
-// reproduces fp32 accuracy (~2^-22 relative) on 16-bit tensor cores.  Everything else (row/column normalisation,
-// margins, online softmax, the normalisation backward) is fused into a few HBM-bound kernels.
+// (x = p0 + p1 + p2, 8 mantissa bits each; the six products with i + j <= 2 are laid side by side along K).  Verified
+// against fp64 (tests/test_heads_fp64_gpu.py): every output within its fp32 rounding bound; the cos RMS error, in units of
+// 2^-24 sum|f~_k w~_k|, is 1.0 at D = 16, 3.0 at D = 128 and 6.2 at D = 512 on an H100 SXM, growing like sqrt(D) because
+// the wgmma fp32 accumulator does not round to nearest (torch's fp32 matmul: 0.3-0.4; a 2-part split: 4-8 at D = 128).
+// The same drift over dF~'s K = 6 Cp (3.5e5 at C = 58 671) gave an RMS of 31; dF~ therefore runs as fixed-order split-K
+// slabs (dfn_splits), which measure 0.09.  Everything else (row/column normalisation, margins, online softmax, the normalisation backward) is fused into a few
+// HBM-bound kernels.
+#include "train_gemm.h"
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
 
@@ -168,32 +173,36 @@ __device__ __forceinline__ void head_logit(const HeadCfg& h, const MvRow& mv, fl
     return;
   }
   const float c = fminf(fmaxf(cos_raw, -1.f), 1.f);
-  const float clamp_pass = (cos_raw >= -1.f && cos_raw <= 1.f) ? 1.f : 0.f;  // torch.clamp backward
+  // torch.clamp's backward is a select, not a product: past the clamp the derivative is 0 even where the unclamped
+  // expression is not finite (the label's c / s at c = 1, s = 0)
+  const bool clamp_pass = cos_raw >= -1.f && cos_raw <= 1.f;
+  float d;
   if (h.kind == VDK_HEAD_ARCFACE) {
     if (is_label) {
       if (c > h.min_cos) {
         const float s = sqrtf(1.0f - c * c);
         z = (c * h.cos_m - s * h.sin_m) * h.scale;
-        dz_dcos = (h.cos_m + (c / s) * h.sin_m) * h.scale * clamp_pass;
+        d = (h.cos_m + (c / s) * h.sin_m) * h.scale;
       } else {
         z = (c - h.margin_am) * h.scale;
-        dz_dcos = h.scale * clamp_pass;
+        d = h.scale;
       }
     } else {
       z = c * h.scale;
-      dz_dcos = h.scale * clamp_pass;
+      d = h.scale;
     }
   } else {
     if (is_label) {
       const float ap = fmaxf((1.f + h.margin) - c, 0.f);  // detached
       z = ap * (c - (1.f - h.margin)) * h.gamma;
-      dz_dcos = ap * h.gamma * clamp_pass;
+      d = ap * h.gamma;
     } else {
       const float an = fmaxf(c + h.margin, 0.f);  // detached
       z = an * (c - h.margin) * h.gamma;
-      dz_dcos = an * h.gamma * clamp_pass;
+      d = an * h.gamma;
     }
   }
+  dz_dcos = clamp_pass ? d : 0.f;
 }
 
 // forward: one CTA per row; online softmax over the classes; optional logits output
@@ -354,10 +363,18 @@ static int make_cfg(const vdk_head_desc* d, HeadCfg* h) {
 }
 
 struct HeadWs {
-  float *inv_f, *inv_w, *fn, *cosm, *row_loss, *dcos_plain, *dcos_scaled, *dfn, *dwn;
+  float *inv_f, *inv_w, *fn, *cosm, *row_loss, *dcos_plain, *dcos_scaled, *dfn, *dwn, *dfn_slabs;
   __nv_bfloat16 *a_split, *b_split;
-  int Cp, Bp, Dp;
+  int Cp, Bp, Dp, dfn_splits;
 };
+
+// dF~ = dcos' . W^T contracts over K = 6 Cp (3.5e5 at C = 58 671).  The wgmma fp32 accumulator does not round to nearest, so
+// one chain over K drifts with the number of k16 steps; the contraction is cut into split-K slabs of at most ~16 K-blocks
+// (64 k16 steps, at most 256 slabs), each stored to its own fp32 slab and summed in a fixed order (deterministic).
+static int dfn_splits(int Cp) {
+  const int kbt = (6 * Cp + 63) / 64;
+  return vdk_gemm_effective_splits(6 * Cp, std::min(256, (kbt + 15) / 16));
+}
 static size_t head_ws_layout(const vdk_head_desc* d, void* base, HeadWs* w) {
   const size_t B = d->batch, D = d->feat_dim, Cn = d->num_class;
   const size_t Cp = pad8(d->num_class), Bp = pad8(d->batch), Dp = pad8(d->feat_dim);
@@ -373,13 +390,15 @@ static size_t head_ws_layout(const vdk_head_desc* d, void* base, HeadWs* w) {
   float* dcos_scaled = reinterpret_cast<float*>(take(B * Cp * 4));
   float* dfn = reinterpret_cast<float*>(take(B * D * 4));
   float* dwn = reinterpret_cast<float*>(take(D * Cp * 4));
+  const int splits = dfn_splits(static_cast<int>(Cp));
+  float* dfn_slabs = splits > 1 ? reinterpret_cast<float*>(take(static_cast<size_t>(splits) * B * D * 4)) : nullptr;
   // split operands: the largest A side is max(B*6Dp, B*6Cp, D*6Bp), the largest B side max(Cp*6Dp, D*6Cp, Cp*6Bp)
   const size_t a_elems = std::max(std::max(B * 6 * Dp, B * 6 * Cp), D * 6 * Bp);
   const size_t b_elems = std::max(std::max(Cp * 6 * Dp, D * 6 * Cp), Cp * 6 * Bp);
   __nv_bfloat16* a_split = reinterpret_cast<__nv_bfloat16*>(take(a_elems * 2));
   __nv_bfloat16* b_split = reinterpret_cast<__nv_bfloat16*>(take(b_elems * 2));
-  if (w) *w = HeadWs{inv_f, inv_w, fn, cosm, row_loss, dcos_plain, dcos_scaled, dfn, dwn, a_split, b_split,
-                     static_cast<int>(Cp), static_cast<int>(Bp), static_cast<int>(Dp)};
+  if (w) *w = HeadWs{inv_f, inv_w, fn, cosm, row_loss, dcos_plain, dcos_scaled, dfn, dwn, dfn_slabs, a_split, b_split,
+                     static_cast<int>(Cp), static_cast<int>(Bp), static_cast<int>(Dp), splits};
   return off + 256;
 }
 
@@ -456,6 +475,7 @@ extern "C" int vdk_head_backward(const vdk_head_desc* d, const float* feats, con
   HeadWs w;
   head_ws_layout(d, workspace, &w);
   const int B = d->batch, D = d->feat_dim, Cn = d->num_class;
+  VDK_REQUIRE(D % 8 == 0, "vdk_head_backward: feat_dim must be a multiple of 8 (it is the N of the dF~ GEMM)");
   // recompute cos (cheaper than keeping [B,C] alive between forward and backward at face-scale C)
   rc = head_cos(d, feats, weight, w, s);
   if (rc != VDK_OK) return rc;
@@ -468,8 +488,18 @@ extern "C" int vdk_head_backward(const vdk_head_desc* d, const float* feats, con
   split3_rows_kernel<<<blocks_for(static_cast<int64_t>(D) * w.Cp, 256), 256, 0, s>>>(weight, D, Cn, Cn, w.Cp, nullptr, nullptr, 1,
                                                                                     w.b_split, nullptr);
   VDK_CUDA_OK(cudaGetLastError());
-  VDK_REQUIRE(D % 8 == 0, "vdk_head_backward: feat_dim must be a multiple of 8");
-  rc = split_gemm(w.a_split, w.b_split, w.dfn, B, D, 6 * w.Cp, D, s);
+  if (w.dfn_splits > 1) {
+    vdk_gemm_desc g{};
+    g.A = w.a_split; g.B = w.b_split; g.D = w.dfn_slabs;
+    g.M = B; g.N = D; g.K = 6 * w.Cp; g.lda = 6 * w.Cp; g.ldb = 6 * w.Cp; g.ldd = D;
+    g.in_dtype = VDK_DTYPE_BF16; g.out_dtype = VDK_DTYPE_FP32; g.epilogue = VDK_EPI_NONE;
+    g.split_k = w.dfn_splits; g.split_stride = static_cast<long long>(B) * D;
+    rc = gemm_run(g, s);
+    if (rc != VDK_OK) return rc;
+    rc = launch_slab_reduce(w.dfn_slabs, w.dfn_splits, static_cast<size_t>(B) * D, static_cast<int64_t>(B) * D / 4, w.dfn, 0, s);
+  } else {
+    rc = split_gemm(w.a_split, w.b_split, w.dfn, B, D, 6 * w.Cp, D, s);
+  }
   if (rc != VDK_OK) return rc;
   fgrad_finalize_kernel<<<(B * 32 + 255) / 256, 256, 0, s>>>(w.dfn, w.fn, w.inv_f, B, D, dfeats);
   // dW~ [D,C] = f~^T [D,B] . dcos [B,C]   (A = f~^T over K=B, B = dcos^T [C, B])

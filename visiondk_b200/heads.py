@@ -54,6 +54,12 @@ def _check_inputs(feats, weight, labels):
         raise ValueError("labels must be [B]")
 
 
+def _check_backward(feats):
+    if feats.shape[1] % 8:
+        raise ValueError(f"the head backward needs feat_dim to be a multiple of 8, got {feats.shape[1]} (the forward has no such "
+                         f"restriction)")
+
+
 class _HeadLogits(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feats, weight, labels, head):
@@ -78,6 +84,7 @@ class _HeadLogits(torch.autograd.Function):
     def backward(ctx, dlogits):
         lib = _lib.load()
         feats, weight, labels = ctx.saved_tensors
+        _check_backward(feats)
         desc = _desc(ctx.head, feats.shape[0], 0.0)
         dlogits = dlogits.contiguous().float()
         df, dw = torch.empty_like(feats), torch.empty_like(weight)
@@ -111,6 +118,7 @@ class _HeadCE(torch.autograd.Function):
     def backward(ctx, gout):
         lib = _lib.load()
         feats, weight, labels, lse = ctx.saved_tensors
+        _check_backward(feats)
         desc = _desc(ctx.head, feats.shape[0], ctx.label_smooth)
         gout = gout.contiguous().float()
         df, dw = torch.empty_like(feats), torch.empty_like(weight)
