@@ -191,6 +191,123 @@ def check_attention(lib, qkv, stats=None, with_lse=True):
     return got
 
 
+def crafted_qkv(B, N, H, alphas, beta, seed, dense=False, device="cuda"):
+    """q_i = alphas[i % len] e_0, k_j = beta[j] e_0, so every raw score q_i . k_j = alpha * beta is an exact product of two bf16
+    values: the test chooses each row's score sequence.  Neighbouring rows take different alphas, so the rows of one 16-row
+    warp slice mix rows that rescale with rows that do not.  dense=True adds random q components in dimensions 1-31 and random k
+    components in dimensions 32-63: the scores stay exact (the two sets of dimensions are disjoint), and the backward's dQ = dS K
+    and dK = dS^T Q are dense rows instead of multiples of e_0."""
+    torch.manual_seed(seed)
+    qkv = torch.zeros(B, N, 3, H, 64, device=device)
+    a = torch.tensor(alphas, device=device)[torch.arange(N, device=device) % len(alphas)]
+    qkv[:, :, 0, :, 0] = a[None, :, None]
+    qkv[:, :, 1, :, 0] = beta[None, :, None]
+    qkv[:, :, 2] = torch.randn(B, N, H, 64, device=device).to(torch.bfloat16).float()
+    if dense:
+        qkv[:, :, 0, :, 1:32] = torch.randn(B, N, H, 31, device=device).to(torch.bfloat16).float()
+        qkv[:, :, 1, :, 32:] = torch.randn(B, N, H, 32, device=device).to(torch.bfloat16).float()
+    out = qkv.to(torch.bfloat16)
+    assert torch.equal(out.float(), qkv)  # alphas and betas are bf16 values
+    return out
+
+
+def _store(ref, e32):
+    """Bound after the bf16 store of an fp32 value within e32 of ref; 0 where both are 0 (an exact fp32 zero stores exactly)."""
+    return torch.where(ref.abs() + e32 > 0, bf16_store_bound(ref, e32), torch.zeros_like(e32))
+
+
+def attention_bwd_reference(qkv, out, dout, lse2, out_bound=None, lse2_bound=None):
+    """fp64 dq, dk, dv of softmax(q k^T / 8) v per (image, head), with an elementwise bound of attention_bwd_kernel's result.
+    Returns (dqkv [B, N, 3, H, 64], bound of the same shape), both fp64.
+
+    The reference differentiates with P_ij = 2^(S_ij log2(e) / 8 - lse2_i) and D_i = sum_d dO_id out_id, taking `out`
+    [B, N, H*64] and `lse2` [B, H, N] as given:
+      isolated: out and lse2 are the kernel's own operands (bf16 and fp32 of the fp64 forward), out_bound = lse2_bound = None.
+                This is exactly the kernel's contract, and P is whatever that lse2 makes of the scores.
+      chained:  out and lse2 are the exact fp64 forward (attention_reference), so P is the exact softmax and the result is the
+                exact gradient; out_bound and lse2_bound bound how far the forward kernel's out and lse2, which the backward
+                kernel is then given, lie from them, and enter D's and x's errors below.
+
+    Kernel arithmetic (vit.cu attention_bwd_kernel) and the bound of each step, for query row i, key j, feature d, with
+    u = 2^-24 (fp32 unit roundoff), U = 2^-23 and n = ceil(N / 16) k16 steps over the (zero-padded) token dimension.
+    An fp32 chain of k16 mma.sync steps is within (steps + 17) U of the product of magnitudes (DESIGN.md §3 model).
+      S_ij = q_i . k_j, 4 k16 steps: |dS_ij| <= 21 U A_ij, A_ij = |q_i| . |k_j|
+      x_ij = S_ij c - lse2_i, c = 0.125 fp32(log2 e): c's own rounding u c |S|, the fp32 multiply and subtract (or one fma)
+             u c |S| + u |x|, and the input's error lse2_bound_i (chained):
+             |dx_ij| <= c 21 U A_ij + U c |S_ij| + U |x_ij| + lse2_bound_i   (U, not u, on |x| covers |x~| > |x|)
+      P~_ij = ex2.approx.ftz(x~_ij): 2 ulp (2^-22) relative on top of 2^dx, and an absolute 2^-126 where ftz flushes to 0:
+             |P~ - P| <= P a + 2^-126,  a_ij = (2^|dx_ij| - 1)(1 + 2^-22) + 2^-22
+      P^ = bf16(P~) (0 for padded rows and columns): |P^ - P| <= eP = P (a + 2^-8 (1 + a)) + 2^-126
+      D~_i: two lanes each run a 32-term fp32 fma chain of exact bf16 products, then one add, over the bf16 out (chained: out
+             lies within out_bound of the exact O): |dD_i| <= 33 u sum_d |dO_id| (|out_id| + ob_id) + sum_d |dO_id| ob_id
+      dP~_ij = dO_i . v_j, 4 k16 steps: |ddP_ij| <= 21 U B_ij, B_ij = |dO_i| . |v_j|;  E_ij = 21 U B_ij + |dD_i|
+      dS~_ij = bf16(fp32(0.125 P^_ij) fp32(dP~_ij - D~_i)): 0.125 P^ is exact; with G_ij = |dP_ij - D_i|, |dP~ - D~| <= G + E,
+             so before the store |dS~ - dS| <= 0.125 (eP (G + E) + P E + (P + eP)(G + E)(2u + u^2)) + 2^-149 (an fp32
+             subnormal product), then half a bf16 ulp.  The bound scales with |dP| + |D|, not with |dP - D|: where a peaked
+             row makes dP_ij - D_i cancel, the error of each term does not.
+      dV_j = sum_i P^_ij dO_i (A = P^T), n steps: (n + 17) U sum_i (P + eP)_ij |dO_i| + sum_i eP_ij |dO_i|, then the bf16 store
+      dQ_i = sum_j dS^_ij k_j, n steps: (n + 17) U sum_j (|dS| + eS)_ij |k_j| + sum_j eS_ij |k_j|, then the bf16 store
+      dK_j = sum_i dS^_ij q_i (A = dS^T), n steps: likewise with |q_i|
+    A row of dO that is exactly 0 has D = 0 and dP = 0 exactly, so its dS and dQ rows are exact zeros; their bound is 0 too.
+    The work is chunked over (image, head) slices so that no [slices, N, N] fp64 temporary exceeds 2^24 elements.
+    """
+    B, N, _, H, D = qkv.shape
+    assert D == 64
+    dev = qkv.device
+    n = -(-N // 16)
+    u, c = 2.0 ** -24, float(torch.tensor(LOG2E, dtype=torch.float32)) / 8.0
+    e_chain = (n + 17) * U32
+
+    def heads(t):  # [B, N, H*64] -> [B*H, N, 64]
+        return t.double().reshape(B, N, H, D).transpose(1, 2).reshape(B * H, N, D)
+
+    q, k, v = (t.reshape(B * H, N, D) for t in qkv.double().permute(2, 0, 3, 1, 4).unbind(0))
+    o, do = heads(out), heads(dout)
+    ob = heads(out_bound) if out_bound is not None else torch.zeros_like(o)
+    l = lse2.double().reshape(B * H, N)
+    lb = lse2_bound.double().reshape(B * H, N) if lse2_bound is not None else torch.zeros_like(l)
+    grads = torch.empty(3, B * H, N, D, dtype=torch.float64, device=dev)
+    bounds = torch.empty_like(grads)
+    step = max(1, (1 << 24) // (N * N))
+    for s0 in range(0, B * H, step):
+        sl = slice(s0, min(B * H, s0 + step))
+        qs, ks, vs, os_, dos = q[sl], k[sl], v[sl], o[sl], do[sl]
+        aq, ak, av, ado = qs.abs(), ks.abs(), vs.abs(), dos.abs()
+        S = qs @ ks.transpose(-1, -2)
+        x = S * (LOG2E / 8.0) - l[sl, :, None]
+        P = torch.exp2(x)
+        dx = c * 21 * U32 * (aq @ ak.transpose(-1, -2)) + U32 * c * S.abs() + U32 * x.abs() + lb[sl, :, None]
+        del S, x
+        a = torch.expm1(math.log(2.0) * dx) * (1 + 2.0 ** -22) + 2.0 ** -22
+        del dx
+        eP = P * (a + 2.0 ** -8 * (1 + a)) + 2.0 ** -126
+        del a
+        Dv = (dos * os_).sum(-1)
+        eD = 33 * u * (ado * (os_.abs() + ob[sl])).sum(-1) + (ado * ob[sl]).sum(-1)
+        dP = dos @ vs.transpose(-1, -2)
+        E = 21 * U32 * (ado @ av.transpose(-1, -2)) + eD[..., None]
+        Gm = dP - Dv[..., None]
+        dS = 0.125 * P * Gm
+        G = Gm.abs()
+        del dP, Gm
+        eS32 = 0.125 * (eP * (G + E) + P * E + (P + eP) * (G + E) * (2 * u + u * u))
+        eS = _store(dS, eS32 + (G + E > 0).double() * 2.0 ** -149)
+        del G, E, eS32
+        grads[2, sl] = P.transpose(-1, -2) @ dos
+        bounds[2, sl] = _store(grads[2, sl], (e_chain * (P + eP) + eP).transpose(-1, -2) @ ado)
+        del P, eP
+        W = e_chain * (dS.abs() + eS) + eS
+        grads[0, sl] = dS @ ks
+        bounds[0, sl] = _store(grads[0, sl], W @ ak)
+        grads[1, sl] = dS.transpose(-1, -2) @ qs
+        bounds[1, sl] = _store(grads[1, sl], W.transpose(-1, -2) @ aq)
+        del dS, eS, W
+    # [3, B*H, N, 64] -> [B, N, 3, H, 64]
+    grads = grads.view(3, B, H, N, D).permute(1, 3, 0, 2, 4).contiguous()
+    bounds = bounds.view(3, B, H, N, D).permute(1, 3, 0, 2, 4).contiguous()
+    return grads, bounds
+
+
 # ------------------------------------------------------------------------------------------------------------------------------
 # ConvNeXt HBM-bound kernels (csrc/convnext.cu, csrc/train_ops.cu): launch arithmetic, fp64 references and bounds.
 # Every reference takes the kernel's own bf16 / fp32 inputs and is computed in fp64 on the device.

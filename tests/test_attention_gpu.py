@@ -8,7 +8,7 @@ device's SM count so that CTAs run several items (and one case exactly SM + 1), 
 import pytest
 import torch
 
-from kernel_ref import ATT_KVTILE, attention_items, check_attention
+from kernel_ref import ATT_KVTILE, attention_items, check_attention, crafted_qkv
 
 pytestmark = pytest.mark.gpu
 
@@ -60,21 +60,6 @@ def test_attention_long_sequence_wraps_the_kv_ring(lib):
     torch.manual_seed(2049)
     qkv = (torch.randn(B, N, 3, H, 64, device="cuda") * 1.5).to(torch.bfloat16)
     check_attention(lib, qkv)
-
-
-def crafted_qkv(B, N, H, alphas, beta, seed):
-    """q_i = alphas[i % len] e_0, k_j = beta[j] e_0, so every raw score q_i . k_j = alpha * beta is an exact product of two bf16
-    values: the test chooses each row's score sequence.  Neighbouring rows take different alphas, so the rows of one 16-row
-    warp slice mix rows that rescale with rows that do not."""
-    torch.manual_seed(seed)
-    qkv = torch.zeros(B, N, 3, H, 64, device="cuda")
-    a = torch.tensor(alphas, device="cuda")[torch.arange(N, device="cuda") % len(alphas)]
-    qkv[:, :, 0, :, 0] = a[None, :, None]
-    qkv[:, :, 1, :, 0] = beta[None, :, None]
-    qkv[:, :, 2] = torch.randn(B, N, H, 64, device="cuda").to(torch.bfloat16).float()
-    out = qkv.to(torch.bfloat16)
-    assert torch.equal(out.float(), qkv)  # alphas and betas are bf16 values
-    return out
 
 
 def _tiles(N, fn):

@@ -3,9 +3,8 @@ pinned against HF ViTModel on CPU).  bf16 activations vs the fp32 oracle: tolera
 import pytest
 import torch
 
-from kernel_ref import attention_reference, check_attention, check_within
+from kernel_ref import check_attention
 from oracle.vit import ViTWrapperOracle, randomize_
-from visiondk_b200 import _lib
 from visiondk_b200.backbone import BackboneFactory
 from visiondk_b200.vit import ViTWrapper
 
@@ -92,33 +91,6 @@ def test_vit_large_patch14_clip_336_embeddings_match_oracle(lib):
     assert cos.min().item() >= 0.999
     with pytest.raises(NotImplementedError):
         ours.train()(x.cuda())
-
-
-@pytest.mark.parametrize("B,N,H", [(2, 197, 3), (1, 208, 2), (3, 50, 2), (2, 17, 1)])
-def test_attention_backward_matches_torch_autograd(lib, B, N, H):
-    """dqkv of softmax(q k^T / 8) v against fp32 autograd on the same bf16-rounded inputs (P and dS are rounded to bf16 inside
-    the kernel: rel L2 <= 2e-2 per operand)."""
-    import ctypes as C
-    torch.manual_seed(N + H)
-    qkv = (torch.randn(B, N, 3, H, 64, device="cuda")).to(torch.bfloat16)
-    dout = torch.randn(B, N, H * 64, device="cuda").to(torch.bfloat16)
-    out = torch.empty((B, N, H * 64), dtype=torch.bfloat16, device="cuda")
-    lse = torch.empty((B, H, N), dtype=torch.float32, device="cuda")
-    dqkv = torch.full_like(qkv, float("nan"))
-    s = _lib.stream_ptr()
-    _lib.check(lib.vdk_attention_fwd_lse(qkv.data_ptr(), B, N, H, 64, out.data_ptr(), lse.data_ptr(), s), "attention fwd+lse")
-    _lib.check(lib.vdk_attention_bwd(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), B, N, H, 64, dqkv.data_ptr(), s),
-               "attention bwd")
-    x = qkv.float().requires_grad_(True)
-    q, k, v = x.permute(2, 0, 3, 1, 4).unbind(0)
-    ref = (torch.softmax((q @ k.transpose(-2, -1)) * 0.125, dim=-1) @ v).transpose(1, 2).reshape(B, N, H * 64)
-    ref.backward(dout.float())
-    # the saved log-sum-exp (log2 domain) against the fp64 logsumexp of the scaled scores, within its derived bound
-    _, _, lse_ref, lse_bound = attention_reference(qkv)
-    check_within(lse, lse_ref, lse_bound, "lse2", lambda bad: f"{int(bad.sum())} rows")
-    assert torch.isfinite(dqkv.float()).all()
-    for i, name in enumerate("qkv"):
-        assert rel(dqkv[:, :, i], x.grad[:, :, i]) <= 2e-2, (name, rel(dqkv[:, :, i], x.grad[:, :, i]))
 
 
 def grads_match(ours, oracle, rel_tol, cos_tol, invariant, vec_rel_tol=None, vec_cos_tol=None):
