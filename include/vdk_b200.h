@@ -573,10 +573,9 @@ typedef struct vdk_convnext_tensors {
 
 /* Refreshes the bf16 / permuted kernel-layout weights of `net` (whose pointer fields address caller-allocated
  * buffers) from the fp32 masters: stem_w, down[].conv_w, blocks[].{dw_w, fc1_w, fc2_w, fc2_wg}, neck_w (un-folded,
- * (h,w,c) order).  fp32 vectors (biases, norms, gamma) are used in place: point net's fields at the masters.
- * vdk_convnext_pack_flip then derives blocks[].dw_w_flip. */
+ * (h,w,c) order), and blocks[].dw_w_flip (the reversed taps) where net carries that buffer.  fp32 vectors (biases,
+ * norms, gamma) are used in place: point net's fields at the masters. */
 int vdk_convnext_pack(const vdk_convnext_tensors* params, vdk_convnext_net* net, void* stream);
-int vdk_convnext_pack_flip(const vdk_convnext_net* net, void* stream);
 size_t vdk_convnext_train_workspace_bytes(const vdk_convnext_net* net, int batch);
 /* images fp32 NCHW -> out_feats fp32 [batch, feat_dim] (NOT normalised: the head normalises).  Saves activations in
  * `workspace` for the backward; updates the BatchNorm running statistics in `params` with `bn_momentum`. */
@@ -665,7 +664,7 @@ int vdk_vit_forward(const vdk_vit_net* net, const float* images, int batch, int 
                     void* workspace, size_t workspace_bytes, void* stream);
 /* softmax(Q K^T / sqrt(d)) V on the qkv Linear's output as stored: qkv bf16 [batch, tokens, 3, heads, head_dim] ->
  * out bf16 [batch, tokens, heads*head_dim]  (timm Attention.forward, scores never written to memory).  head_dim 64, 72 or 80
- * (other values: VDK_ERR_INVALID); with VDK_ATT_TC=0 (the earlier mma.sync kernel) 64 only. */
+ * (other values: VDK_ERR_INVALID). */
 int vdk_attention_fwd(const void* qkv, int batch, int tokens, int heads, int head_dim, void* out, void* stream);
 
 /* ---- ViT training forward / backward (BASELINE config 3: ViT-B/16 + CircleLoss) ----------------------------------- */

@@ -301,15 +301,15 @@ def test_bound_from_sketches_matches_the_counting_argument(lib):
         assert np.array_equal(got.cpu().numpy().view(np.uint32), want.view(np.uint32)), (n_shards, ranks, k)
 
 
-@pytest.mark.parametrize("world,clustered,sketch", [(8, False, "1"), (8, True, "1"), (3, False, "1"), (8, False, "0")])
-def test_sharded_protocol_on_local_shards(lib, monkeypatch, world, clustered, sketch):
+@pytest.mark.parametrize("world,clustered,k", [(8, False, 100), (8, True, 100), (3, False, 100), (8, False, 1)])
+def test_sharded_protocol_on_local_shards(lib, world, clustered, k):
     """The W-shard search (range schedule, rank-sketch exchange after every range, bounded re-rank, packed merge) with the
     collectives replaced by barriers between W host threads on one GPU: every shard must return the unsharded answer, bit for
-    bit, and every published sketch entry must be a TRUE lower bound (>= r rows of that shard score at least sketch[r])."""
+    bit, and every published sketch entry must be a TRUE lower bound (>= r rows of that shard score at least sketch[r]).
+    At k = 1 the shards exchange only the element-wise max of their k-th bounds."""
     from visiondk_b200 import sharding
     from visiondk_b200.retrieval import sharded_flat_search, bound_from_sketches, _Exchange
-    monkeypatch.setenv("VDK_SHARD_SKETCH", sketch)
-    nq, ng, dim, k = 256, 120000, 128, 100
+    nq, ng, dim = 256, 120000, 128
     q, g = unit_rows(nq, dim, 41), unit_rows(ng, dim, 42)
     if clustered:  # all near neighbours of query j live in ONE shard (a gallery stored class by class)
         rng = np.random.default_rng(43)
@@ -353,9 +353,11 @@ def test_sharded_protocol_on_local_shards(lib, monkeypatch, world, clustered, sk
         assert torch.equal(i, wi) and torch.equal(s.view(torch.int32), ws.view(torch.int32)), f"shard {r} disagrees"
     for sh in shards:
         sh.check_status()
-    if sketch == "1":
-        ranks = _Exchange(None, group.comm(0), k).ranks
-        assert ranks == R.sketch_ranks(k, world)
+    ranks = _Exchange(None, group.comm(0), k).ranks
+    assert ranks == R.sketch_ranks(k, world)
+    if k == 1:
+        assert ranks == [1] and not gathered  # no sketch is published
+    else:
         assert len(ranks) > 1 and len(gathered) >= 2  # one exchange per gallery range
         g_dev = torch.from_numpy(g).cuda()
         kth_true = ws[:, k - 1]  # the global k-th canonical score

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """A W-way sharded search of the bench's gallery emulated on ONE H100 (W shards, one host thread each, the collectives replaced by
 barriers — visiondk_b200.sharding.LocalShardGroup): checks the protocol against the unsharded search and prints the device time
-of ONE shard's share of the work (total / W) for the exchange variants and range schedules.  What it cannot see: the NCCL
+of ONE shard's share of the work (total / W) and the range schedule.  What it cannot see: the NCCL
 latency of the 2-3 small all-gathers and the 8 MB-per-rank list gather (measured by bench.py --gpus N).
 
     python tools/emulate_shards.py --world 8 [--nq 10000 --ng 1000000 --k 100]
@@ -24,7 +24,6 @@ def main():
     ap.add_argument("--dim", type=int, default=512)
     ap.add_argument("--k", type=int, default=100)
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--variants", default="sketch=1;sketch=0;sketch=1,growth=8;sketch=1,first=8192")
     a = ap.parse_args()
     from visiondk_b200 import _lib, sharding
     from visiondk_b200.retrieval import FlatIPIndex, sharded_flat_search, shard_schedule
@@ -60,34 +59,27 @@ def main():
     ms1 = timed(lambda: whole.search_device(q, a.k))
     print(json.dumps({"variant": "unsharded", "ms": round(ms1, 3)}), flush=True)
     group = sharding.LocalShardGroup(a.world)
-    for var in a.variants.split(";"):
-        opts = dict(kv.split("=") for kv in var.split(",") if kv)
-        for key, env in (("sketch", "VDK_SHARD_SKETCH"), ("growth", "VDK_SHARD_GROWTH"), ("first", "VDK_SHARD_FIRST")):
-            if key in opts:
-                os.environ[env] = opts[key]
-            else:
-                os.environ.pop(env, None)
 
-        def search():
-            return group.run(lambda comm: sharded_flat_search(shards[comm.rank], q, [a.nq], a.k, defer_check=True, comm=comm), device=dev)
+    def search():
+        return group.run(lambda comm: sharded_flat_search(shards[comm.rank], q, [a.nq], a.k, defer_check=True, comm=comm), device=dev)
 
-        res = search()
-        ok = all(torch.equal(i, wi) and torch.equal(s.view(torch.int32), ws.view(torch.int32)) for s, i in res)
-        for sh in shards:
-            sh.check_status()
-        ms = timed(search)
-        with _lib.profile() as prof:
-            search()
-        torch.cuda.synchronize()
-        sf = prof.totals["score_filter"]  # upper bound: another shard's launch can slip between a launch and its closing event
-        sf = {"launches": sf["launches"], "ms_per_shard": round(sf["ms"] / a.world, 3)}
-        print(json.dumps({"variant": var, "world": a.world, "equals_unsharded": ok,
-                          "schedule": shard_schedule(max(sh.ntotal for sh in shards), a.world, a.k),
-                          "ms_all_shards": round(ms, 3), "ms_per_shard": round(ms / a.world, 3),
-                          "score_filter": sf, "max_candidates": int(max(int(sh.last_status[1]) for sh in shards)),
-                          "rerank_rows_max": int(max(int(sh.last_status[2]) for sh in shards))}), flush=True)
-        if not ok:
-            raise SystemExit("sharded result differs from the unsharded search")
+    res = search()
+    ok = all(torch.equal(i, wi) and torch.equal(s.view(torch.int32), ws.view(torch.int32)) for s, i in res)
+    for sh in shards:
+        sh.check_status()
+    ms = timed(search)
+    with _lib.profile() as prof:
+        search()
+    torch.cuda.synchronize()
+    sf = prof.totals["score_filter"]  # upper bound: another shard's launch can slip between a launch and its closing event
+    sf = {"launches": sf["launches"], "ms_per_shard": round(sf["ms"] / a.world, 3)}
+    print(json.dumps({"variant": "sharded", "world": a.world, "equals_unsharded": ok,
+                      "schedule": shard_schedule(max(sh.ntotal for sh in shards), a.world, a.k),
+                      "ms_all_shards": round(ms, 3), "ms_per_shard": round(ms / a.world, 3),
+                      "score_filter": sf, "max_candidates": int(max(int(sh.last_status[1]) for sh in shards)),
+                      "rerank_rows_max": int(max(int(sh.last_status[2]) for sh in shards))}), flush=True)
+    if not ok:
+        raise SystemExit("sharded result differs from the unsharded search")
 
 
 if __name__ == "__main__":

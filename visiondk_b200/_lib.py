@@ -127,7 +127,6 @@ SIGNATURES = {
     "vdk_batchnorm_train_fwd": (_i, [_p, _i, _i, _i, _p, _p, C.c_float, C.c_float, _p, _p, _p, _p, _p, _p]),
     "vdk_batchnorm_train_bwd": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p]),
     "vdk_convnext_pack": (_i, [_p, _p, _p]),
-    "vdk_convnext_pack_flip": (_i, [_p, _p]),
     "vdk_convnext_train_workspace_bytes": (_sz, [_p, _i]),
     "vdk_convnext_train_forward": (_i, [_p, _p, _p, _i, C.c_float, _p, _p, _sz, _p]),
     "vdk_convnext_train_backward": (_i, [_p, _p, _p, _p, _i, _p, _sz, _p]),

@@ -992,10 +992,8 @@ int vdk::launch_dwconv7(int mode, const __nv_bfloat16* x, int batch, int H, int 
     if (C % 128 == 0) chunk = 128;
     else if (C % 96 == 0) chunk = 96;
     else if (C % 64 == 0) chunk = 64;
-    static const bool use_chunked = [] {
-      const char* e = getenv("VDK_DWCONV_CHUNKED");
-      return e ? atoi(e) != 0 : true;
-    }();
+    // VDK_DWCONV_PIPE=0 runs the one-tile-per-CTA chunk kernel below, which otherwise runs only where the persistent grid does
+    // not fit the device: the switch lets the tests reach that fallback
     static const bool use_pipe = [] {
       const char* e = getenv("VDK_DWCONV_PIPE");
       return e ? atoi(e) != 0 : true;
@@ -1004,7 +1002,7 @@ int vdk::launch_dwconv7(int mode, const __nv_bfloat16* x, int batch, int H, int 
       const int rc = launch_dwconv7_pipe(mode, x, batch, H, W, C, chunk, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s);
       if (rc != VDK_ERR_WORKSPACE) return rc;  // VDK_ERR_WORKSPACE: the persistent grid does not fit this device -> fall through
     }
-    if (use_chunked && chunk > 0 && C / chunk <= 16) {
+    if (chunk > 0 && C / chunk <= 16) {
       const int nchunks = C / chunk;
       const int TH = std::min(7, H);
       CUtensorMap mx;

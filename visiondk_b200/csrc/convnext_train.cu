@@ -113,6 +113,12 @@ __global__ void slab_reduce_bias_kernel(const float* __restrict__ slabs, int n_s
   for (int s = 0; s < n_slabs; ++s) v += slabs[s * stride + i];
   out[i] = v;
 }
+int launch_slab_reduce_bias(const float* slabs, int n_slabs, size_t stride, const float* bias, int rows, int cols, float* out,
+                            cudaStream_t s) {
+  slab_reduce_bias_kernel<<<(rows * cols + 255) / 256, 256, 0, s>>>(slabs, n_slabs, stride, bias, rows, cols, out);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
 // dst[i] (+)= sum_s slabs[s * stride + i]: 32 float4 columns x 8 slab groups per block; the groups meet in shared
 // memory and are added in a fixed order
 __global__ void __launch_bounds__(256)
@@ -157,6 +163,11 @@ __global__ void col_sum_f32_small_kernel(const float* __restrict__ x, int rows, 
   float s = 0.f;
   for (int r = 0; r < rows; ++r) s += x[static_cast<size_t>(r) * cols + c];
   out[c] += s;
+}
+int launch_col_sum_f32_small(const float* x, int rows, int cols, float* out, cudaStream_t s) {
+  col_sum_f32_small_kernel<<<(cols + 255) / 256, 256, 0, s>>>(x, rows, cols, out);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
 }
 __global__ void stem_patchify_train_kernel(const float* __restrict__ x, int B, int H, int W, __nv_bfloat16* __restrict__ out) {
   const int PH = H / 4, PW = W / 4;
@@ -306,29 +317,6 @@ extern "C" int vdk_convnext_pack(const vdk_convnext_tensors* p, vdk_convnext_net
   return VDK_OK;
 }
 
-__global__ void flip_taps_kernel(const float* __restrict__ w49, int C, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= 49 * C) return;
-  const int t = i / C, c = i - t * C;
-  out[(48 - t) * C + c] = w49[i];
-}
-
-// Reversed taps from the PACKED taps of `net` (kept for callers that pack by other means; vdk_convnext_pack already
-// writes them when the net carries dw_w_flip buffers).
-extern "C" int vdk_convnext_pack_flip(const vdk_convnext_net* net, void* stream) {
-  VDK_REQUIRE(net, "vdk_convnext_pack_flip: null net");
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  int k = 0;
-  for (int st = 0; st < 4; ++st)
-    for (int j = 0; j < net->depths[st]; ++j, ++k) {
-      const vdk_convnext_block* o = &net->blocks[k];
-      if (!o->dw_w_flip) continue;
-      flip_taps_kernel<<<(49 * net->dims[st] + 255) / 256, 256, 0, s>>>(o->dw_w, net->dims[st], const_cast<float*>(o->dw_w_flip));
-    }
-  VDK_CUDA_OK(cudaGetLastError());
-  return VDK_OK;
-}
-
 extern "C" int vdk_convnext_train_forward(const vdk_convnext_net* net, const vdk_convnext_tensors* p, const float* images,
                                           int batch, float bn_momentum, float* out_feats, void* workspace,
                                           size_t workspace_bytes, void* stream) {
@@ -391,8 +379,7 @@ extern "C" int vdk_convnext_train_forward(const vdk_convnext_net* net, const vdk
     const size_t slab = static_cast<size_t>(batch) * F;
     RC(G.run(B16(L.fn), net->neck_w, F32(L.zslab), batch, F, Kn, Kn, Kn, F, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0,
              VDK_DTYPE_FP32, split, split > 1 ? static_cast<long long>(slab) : 0, 0, 0));
-    slab_reduce_bias_kernel<<<(batch * F + 255) / 256, 256, 0, s>>>(F32(L.zslab), split, slab, p->lin_b, batch, F, F32(L.z));
-    VDK_CUDA_OK(cudaGetLastError());
+    RC(launch_slab_reduce_bias(F32(L.zslab), split, slab, p->lin_b, batch, F, F32(L.z), s));
     RC(launch_bn_fwd_f32(F32(L.z), batch, F, p->bn1_w, p->bn1_b, 1e-5f, bn_momentum, out_feats, F32(L.bn1_mean), F32(L.bn1_rstd),
                          p->bn1_running_mean, p->bn1_running_var, s));
   }
@@ -434,7 +421,7 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
     VDK_CUDA_OK(cudaMemsetAsync(F32(L.sdo), 0, static_cast<size_t>(L.n_blocks) * 2048 * 4, s));
     VDK_CUDA_OK(cudaMemsetAsync(F32(L.dw49), 0, static_cast<size_t>(L.n_blocks) * 49 * 2048 * 4, s));
     RC(launch_bn_bwd_f32(d_feats, F32(L.z), batch, F, p->bn1_w, F32(L.bn1_mean), F32(L.bn1_rstd), F32(L.dz), g->bn1_w, g->bn1_b, s));
-    col_sum_f32_small_kernel<<<(F + 255) / 256, 256, 0, s>>>(F32(L.dz), batch, F, g->lin_b);
+    RC(launch_col_sum_f32_small(F32(L.dz), batch, F, g->lin_b, s));
     RC(launch_cast_bf16(F32(L.dz), static_cast<int64_t>(batch) * F, B16(L.dzb), s));
     // dW[F, (h,w,c)] = dZ^T . FN  (both stored with the batch index slow), then un-permute into timm's (c, h, w) order
     RC(G.run(B16(L.dzb), B16(L.fn), F32(L.gwneck), F, Kn, batch, F, Kn, Kn, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0,

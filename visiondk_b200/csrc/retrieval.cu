@@ -331,7 +331,6 @@ struct SelectParams {
   float* kth_lb;          // [n_query] optional: lower bound of the k-th largest canonical score of this shard
   int stage_cap;          // entries of dynamic shared memory available for staging (<= kSelStage)
   const float* ext_lb;    // [n_query] optional: lower bound of the GLOBAL k-th canonical score known before this range
-  int prefilter;          // dense ranges: drop what cannot reach the top-k before the radix passes (see select_kernel)
 };
 
 // Rows whose lists hold at most kSelStage entries in total (every sparse range in practice: ~110 carried + a few hundred
@@ -340,9 +339,9 @@ struct SelectParams {
 // then run out of shared memory.  Longer rows keep sweeping the lists in place.
 constexpr int kSelStage = 4096;
 
-// kPre: the prefilter of dense ranges, 1 = two sweeps over the entries, 2 = entries held in registers (default).  Its own
-// instantiation: the 64 registers of the entry array would otherwise cut the occupancy of every sparse-range launch.
-template <bool kAgg, int kPre>
+// kPre: the prefilter of dense ranges, entries held in registers.  Its own instantiation: the 64 registers of the entry
+// array would otherwise cut the occupancy of every sparse-range launch.
+template <bool kAgg, bool kPre>
 __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectParams p) {
   extern __shared__ uint2 s_stage[];  // [p.stage_cap]
   __shared__ unsigned hist[256];
@@ -391,9 +390,9 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectParams 
   // entries t, t + 128, ...; >= k threads hold a maximum >= F (the k-th largest of the 128 maxima), so the
   // k-th largest score of the row is >= F and only entries >= F - 2 eps can survive the select.  They (a few hundred) are
   // compacted into shared memory and the radix passes run on them.
-  const bool pre = kPre != 0 && p.dense_n > 0 && staged && n >= 1024u && p.k <= kSelThreads;  // CTA-uniform
-  if constexpr (kPre == 2) {
-    // register form: every entry is read ONCE and kept (64 registers) between the maximum and the compaction
+  const bool pre = kPre && p.dense_n > 0 && staged && n >= 1024u && p.k <= kSelThreads;  // CTA-uniform
+  if constexpr (kPre) {
+    // every entry is read ONCE and kept (64 registers) between the maximum and the compaction
     if (pre) {
       constexpr int kPer = kSelStage / kSelThreads;
       uint2 ent[kPer];
@@ -417,7 +416,7 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectParams 
         gt += y > mx ? 1 : 0;
         ge += y >= mx ? 1 : 0;
       }
-      if (gt < p.k && p.k <= ge) s_floor = mx;
+      if (gt < p.k && p.k <= ge) s_floor = mx;  // the k-th largest maximum (ties write the same value)
       __syncthreads();
       const float keep_from = s_floor - 2.0f * p.eps[row];
 #pragma unroll
@@ -436,46 +435,6 @@ __global__ void __launch_bounds__(kSelThreads) select_kernel(const SelectParams 
       n_lists = 1;
       __syncthreads();
     }
-  } else if constexpr (kPre == 1) {
-   if (pre) {
-    // two sweeps over the row's entries (32 KB: the second one hits L2), nothing held in registers in between
-    const uint2* c0 = list_ptr_g(0);
-    const uint2* d0 = list_ptr_g(1);
-    const unsigned cnt0 = s_cnt[0];
-    float mx = -INFINITY;
-#pragma unroll 8
-    for (unsigned i = tid; i < n; i += kSelThreads) mx = fmaxf(mx, __uint_as_float(i < cnt0 ? c0[i].x : d0[i - cnt0].x));
-    float* s_mx = reinterpret_cast<float*>(hist);  // re-zeroed by every radix pass
-    s_mx[tid] = mx;
-    __syncthreads();
-    int gt = 0, ge = 0;
-    for (int j = 0; j < kSelThreads; ++j) {
-      const float y = s_mx[j];
-      gt += y > mx ? 1 : 0;
-      ge += y >= mx ? 1 : 0;
-    }
-    if (gt < p.k && p.k <= ge) s_floor = mx;  // the k-th largest maximum (ties write the same value)
-    __syncthreads();
-    const float keep_from = s_floor - 2.0f * p.eps[row];
-#pragma unroll 4
-    for (unsigned base = 0; base < n; base += kSelThreads) {
-      const unsigned i = base + tid;
-      uint2 v = make_uint2(0u, 0u);
-      if (i < n) v = i < cnt0 ? c0[i] : d0[i - cnt0];
-      const bool k_ = i < n && __uint_as_float(v.x) >= keep_from;
-      const unsigned m = __ballot_sync(0xffffffffu, k_);
-      if (m != 0u) {  // warp-uniform
-        unsigned base_pos = 0;
-        if (lane == 0) base_pos = atomicAdd(&s_n2, static_cast<unsigned>(__popc(m)));
-        base_pos = __shfl_sync(0xffffffffu, base_pos, 0);
-        if (k_) s_stage[base_pos + __popc(m & ((1u << lane) - 1u))] = v;
-      }
-    }
-    __syncthreads();
-    if (tid == 0) s_cnt[0] = s_n2;  // <= n <= stage_cap
-    n_lists = 1;
-    __syncthreads();
-   }
   }
   if (!pre && staged) {
     for (int l = warp; l < n_lists; l += kSelThreads / 32) {
@@ -743,12 +702,9 @@ __global__ void eps_kernel(const float* __restrict__ q_norm, const float* __rest
 // ------------------------------------------------------------------------------------------------
 // merge of per-shard lists, and brute-force pair scores for verification
 // ------------------------------------------------------------------------------------------------
-// Lists arrive either as separate (scores, ids) arrays or PACKED as one 64-bit word per entry (score bits << 32 | uint32 id,
-// id -1 = 0xffffffff): the packed form is what the ranks exchange in ONE all-gather.
-template <bool kPacked>
-__global__ void topk_merge_kernel(const float* __restrict__ scores, const int64_t* __restrict__ ids,
-                                  const unsigned long long* __restrict__ packed, int n_lists, int64_t n_query, int k,
-                                  float* __restrict__ out_scores, int64_t* __restrict__ out_ids) {
+// Lists as separate (scores, ids) arrays.
+__global__ void topk_merge_kernel(const float* __restrict__ scores, const int64_t* __restrict__ ids, int n_lists, int64_t n_query,
+                                  int k, float* __restrict__ out_scores, int64_t* __restrict__ out_ids) {
   // one warp per query; lists are individually ordered, so a k-step tournament over n_lists heads suffices
   const int lane = threadIdx.x & 31;
   const int64_t row = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
@@ -759,15 +715,8 @@ __global__ void topk_merge_kernel(const float* __restrict__ scores, const int64_
     float sc = -FLT_MAX;
     int64_t id = -1;
     if (lane < n_lists && head < k) {
-      if (kPacked) {
-        const unsigned long long w = packed[lane * list_stride + row * k + head];
-        sc = __uint_as_float(static_cast<uint32_t>(w >> 32));
-        const uint32_t lo = static_cast<uint32_t>(w & 0xffffffffull);
-        id = lo == 0xffffffffu ? -1 : static_cast<int64_t>(lo);
-      } else {
-        sc = scores[lane * list_stride + row * k + head];
-        id = ids[lane * list_stride + row * k + head];
-      }
+      sc = scores[lane * list_stride + row * k + head];
+      id = ids[lane * list_stride + row * k + head];
     }
     // best = max score, then smallest non-negative id
     float bs = sc;
@@ -798,7 +747,8 @@ __global__ void topk_merge_kernel(const float* __restrict__ scores, const int64_
   }
 }
 
-// Packed lists (the sharded search's merge): one query per GROUP of `group` = pow2 >= n_lists lanes (4 queries per warp on 8
+// Lists PACKED as one 64-bit word per entry (score bits << 32 | uint32 id, id -1 = 0xffffffff), the form the ranks of the
+// sharded search exchange in ONE all-gather: one query per GROUP of `group` = pow2 >= n_lists lanes (4 queries per warp on 8
 // shards).  Lane l of a group walks list l and holds its head as ONE 64-bit key (order-preserving score bits << 32 | ~id: larger
 // is better — score desc, id asc; 0 = list exhausted) with the next entry already loaded, so a step is log2(group) 64-bit
 // max-shuffles and the winner's register move: no load on the critical path (the general kernel above re-loads 32 heads and
@@ -1220,10 +1170,9 @@ static int topk_filter(const vdk_topk_plan* plan, const void* qh, const float* q
   }
   static bool sel_attr = false;
   if (!sel_attr) {
-    VDK_CUDA_OK(cudaFuncSetAttribute(select_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelStage * sizeof(uint2)));
-    VDK_CUDA_OK(cudaFuncSetAttribute(select_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelStage * sizeof(uint2)));
-    VDK_CUDA_OK(cudaFuncSetAttribute(select_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelStage * sizeof(uint2)));
-    VDK_CUDA_OK(cudaFuncSetAttribute(select_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelStage * sizeof(uint2)));
+    VDK_CUDA_OK(cudaFuncSetAttribute(select_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelStage * sizeof(uint2)));
+    VDK_CUDA_OK(cudaFuncSetAttribute(select_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelStage * sizeof(uint2)));
+    VDK_CUDA_OK(cudaFuncSetAttribute(select_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSelStage * sizeof(uint2)));
     sel_attr = true;
   }
   int cur = 0;  // carry buffer holding the current survivors
@@ -1268,26 +1217,14 @@ static int topk_filter(const vdk_topk_plan* plan, const void* qh, const float* q
       sp.ext_lb = ext_lb;
       // staging area: the dense first range needs room for every score of the range, a sparse range for a few hundred
       sp.stage_cap = dense ? kSelStage : kSelStage / 2;
-      static const int prefilter = [] {  // VDK_SELECT_PREFILTER: 0 plain staged select on dense ranges too, 1 two sweeps, 2 registers
-        const char* e = getenv("VDK_SELECT_PREFILTER");
-        return e ? atoi(e) : 2;
-      }();
-      sp.prefilter = prefilter;
-      const bool pre = prefilter && dense && k <= kSelThreads;  // what is left after the prefilter needs no aggregation
-      // warp-aggregated histogram atomics pay on the dense range (thousands of keys whose first digit collides); VDK_SELECT_AGG
-      // = 0 never, 1 dense ranges only (default), 2 always
-      static const int agg_mode = [] {
-        const char* e = getenv("VDK_SELECT_AGG");
-        return e ? atoi(e) : 1;
-      }();
-      if (pre && prefilter == 2)
-        select_kernel<false, 2><<<static_cast<unsigned>(nq), kSelThreads, sp.stage_cap * sizeof(uint2), s>>>(sp);
-      else if (pre)
-        select_kernel<false, 1><<<static_cast<unsigned>(nq), kSelThreads, sp.stage_cap * sizeof(uint2), s>>>(sp);
-      else if (agg_mode == 2 || (agg_mode == 1 && dense))
-        select_kernel<true, 0><<<static_cast<unsigned>(nq), kSelThreads, sp.stage_cap * sizeof(uint2), s>>>(sp);
+      // dense ranges: the prefilter where it applies (what is left after it needs no aggregation), else warp-aggregated
+      // histogram atomics, which pay on thousands of keys whose first digit collides; sparse ranges: the plain select
+      if (dense && k <= kSelThreads)
+        select_kernel<false, true><<<static_cast<unsigned>(nq), kSelThreads, sp.stage_cap * sizeof(uint2), s>>>(sp);
+      else if (dense)
+        select_kernel<true, false><<<static_cast<unsigned>(nq), kSelThreads, sp.stage_cap * sizeof(uint2), s>>>(sp);
       else
-        select_kernel<false, 0><<<static_cast<unsigned>(nq), kSelThreads, sp.stage_cap * sizeof(uint2), s>>>(sp);
+        select_kernel<false, false><<<static_cast<unsigned>(nq), kSelThreads, sp.stage_cap * sizeof(uint2), s>>>(sp);
       VDK_CUDA_OK(cudaGetLastError());
       cur ^= 1;
       lo = hi;
@@ -1568,8 +1505,8 @@ extern "C" int vdk_topk_merge(const float* scores, const int64_t* ids, int n_lis
   VDK_REQUIRE(n_lists >= 1 && n_lists <= 32 && k >= 1 && n_query >= 0, "vdk_topk_merge: n_lists must be in [1,32]");
   if (n_query == 0) return VDK_OK;
   const int64_t blocks = (n_query + 7) / 8;
-  topk_merge_kernel<false><<<static_cast<unsigned>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      scores, ids, nullptr, n_lists, n_query, k, out_scores, out_ids);
+  topk_merge_kernel<<<static_cast<unsigned>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      scores, ids, n_lists, n_query, k, out_scores, out_ids);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }
@@ -1588,20 +1525,10 @@ extern "C" int vdk_topk_merge_packed(const void* packed, int n_lists, int64_t n_
   VDK_REQUIRE(packed && out_scores && out_ids, "vdk_topk_merge_packed: null operand");
   VDK_REQUIRE(n_lists >= 1 && n_lists <= 32 && k >= 1 && n_query >= 0, "vdk_topk_merge_packed: n_lists must be in [1,32]");
   if (n_query == 0) return VDK_OK;
-  static const int fast = [] {  // VDK_MERGE_FAST=0: the general tournament kernel
-    const char* e = getenv("VDK_MERGE_FAST");
-    return e ? atoi(e) : 1;
-  }();
-  if (fast) {
-    const int group = pow2_ceil(n_lists);
-    const int64_t warps = (n_query + 32 / group - 1) / (32 / group);
-    topk_merge_packed_kernel<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<const unsigned long long*>(packed), n_lists, group, n_query, k, out_scores, out_ids);
-  } else {
-    const int64_t blocks = (n_query + 7) / 8;
-    topk_merge_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        nullptr, nullptr, reinterpret_cast<const unsigned long long*>(packed), n_lists, n_query, k, out_scores, out_ids);
-  }
+  const int group = pow2_ceil(n_lists);
+  const int64_t warps = (n_query + 32 / group - 1) / (32 / group);
+  topk_merge_packed_kernel<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const unsigned long long*>(packed), n_lists, group, n_query, k, out_scores, out_ids);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }

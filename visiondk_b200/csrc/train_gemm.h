@@ -8,6 +8,11 @@ namespace vdk {
 
 // dst[i] (+)= sum over slabs, fixed order (convnext_train.cu)
 int launch_slab_reduce(const float* slabs, int n_slabs, size_t stride, int64_t n4, float* dst, int accumulate, cudaStream_t s);
+// out[r, c] = bias[c] (0 when bias is null) + sum over slabs, fixed order: the split-K neck Linear (convnext_train.cu)
+int launch_slab_reduce_bias(const float* slabs, int n_slabs, size_t stride, const float* bias, int rows, int cols, float* out,
+                            cudaStream_t s);
+// out[c] += sum_r x[r, c], one thread per column: the neck Linear's bias gradient over a small batch (convnext_train.cu)
+int launch_col_sum_f32_small(const float* x, int rows, int cols, float* out, cudaStream_t s);
 
 // split count for a weight-gradient GEMM (few output tiles, very long contraction): at least two, so that vdk_gemm
 // takes its raw-partials output mode; every split stores its own fp32 slab, which a reduction kernel then adds in a

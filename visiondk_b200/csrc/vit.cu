@@ -11,16 +11,14 @@
 //               y = LN2(x); h = GELU(GEMM(y)+b); x = x + ls2 * (GEMM(h)+b)                  ls = 1 without LayerScale)
 //   y = LN_neck(LN_final(x)); embeddings = split-K GEMM over (token, channel) with BatchNorm1d folded [+ L2 normalise]
 //
-// Attention: one CTA = 64 query rows of one (image, head), 4 warps x 16 rows, K/V streamed in 64-row tiles through
-// swizzled shared memory, mma.sync m16n8k16 (bf16 in, fp32 accumulate) with the online-softmax recurrence in registers
-// (scores never leave the SM).  Attention is 4 % of a ViT-B's FLOPs.
+// Attention: the forward is the wgmma kernel of attention_tc.cu, with the online-softmax recurrence in registers (scores
+// never leave the SM); the training backward below runs on mma.sync m16n8k16.  Attention is 4 % of a ViT-B's FLOPs.
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
 #include "convnext_internal.h"
 #include "train_gemm.h"
 
 #include <algorithm>
-#include <cstdlib>
 
 namespace vdk {
 
@@ -71,7 +69,25 @@ vit_assemble_kernel(const __nv_bfloat16* __restrict__ tok, const float* __restri
 }
 
 // ------------------------------------------------------------------------------------------------
-// attention forward, head_dim 64
+// attention forward: the wgmma kernel of attention_tc.cu, head_dim 64, 72 or 80
+// ------------------------------------------------------------------------------------------------
+int launch_attention_tc(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
+                        cudaStream_t s);  // attention_tc.cu
+
+static int launch_attention(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
+                            cudaStream_t s) {
+  VDK_REQUIRE(head_dim == 64 || head_dim == 72 || head_dim == 80, "attention: head_dim must be 64, 72 or 80 (got %d)", head_dim);
+  const double D = head_dim;
+  ProfScope prof(kProfAttention, 4.0 * static_cast<double>(B) * H * N * N * D, 2.0 * static_cast<double>(B) * N * H * D * 4.0, s);
+  return launch_attention_tc(qkv, B, N, H, head_dim, out, lse2, s);
+}
+
+// ------------------------------------------------------------------------------------------------
+// attention backward for N <= 208 tokens (ViT-*/16 at 224^2: 197): one CTA per (image, head) keeps Q, K, V, dO and the
+// whole probability matrix in shared memory and runs the five products of the backward as in-CTA GEMMs on mma.sync:
+//   P = exp2(scale' Q K^T - lse2)                    (recomputed from the saved log-sum-exp)
+//   dV = P^T dO;  dP = dO V^T;  dS = scale P (dP - D),  D_i = sum_d dO_id O_id;  dQ = dS K;  dK = dS^T Q
+// Warp w owns rows 16w .. 16w+15 of whichever matrix is being produced.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
@@ -84,247 +100,13 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-constexpr int kAttD = 64;        // head dim
-constexpr int kAttBN = 64;       // key/value rows per shared-memory tile
-constexpr int kAttMaxWarps = 16; // query rows per CTA = 16 per warp
+constexpr int kAttD = 64;  // head dim
 
 // [rows] x 64 bf16 tile in shared memory: 128-byte rows, 16-byte chunk index XOR (row & 7) (conflict-free ldmatrix)
 __device__ __forceinline__ uint32_t att_tile_addr(uint32_t base, int row, int col /*multiple of 8*/) {
   return base + row * 128 + (((col >> 3) ^ (row & 7)) << 4);
 }
 
-// qkv: [B, N, 3, H, 64] bf16 (the qkv Linear's output as stored);  out: [B, N, H*64] bf16.
-// CTA = up to 16 warps, each owning 16 query rows of one (image, head); K / V stream through 64-row tiles loaded once per
-// CTA (ViT-B/16: 197 tokens -> ONE CTA of 13 warps per (image, head), K and V read once); 8-column score tiles and 16-row
-// P.V steps that lie entirely beyond N are skipped.
-__global__ void __launch_bounds__(kAttMaxWarps * 32)
-attention_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, int B, int N, int H, float scale_log2e, __nv_bfloat16* __restrict__ out,
-                     float* __restrict__ lse2 /*[B,H,N] log2-domain log-sum-exp per row, or null*/) {
-  extern __shared__ __align__(128) uint8_t att_smem[];
-  const int nwarps = blockDim.x >> 5;
-  uint8_t* sq = att_smem;                       // [nwarps * 16][64]
-  uint8_t* skv = att_smem + nwarps * 16 * 128;  // 2 stages x { K [64][64], V [64][64] }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
-  const int q0 = (blockIdx.x * nwarps + warp) * 16, h = blockIdx.y, b = blockIdx.z;
-  const int64_t ld = static_cast<int64_t>(3) * H * kAttD;
-  const __nv_bfloat16* base = qkv + static_cast<int64_t>(b) * N * ld + h * kAttD;
-  const __nv_bfloat16* kp = base + static_cast<int64_t>(H) * kAttD;
-  const __nv_bfloat16* vp = base + static_cast<int64_t>(2) * H * kAttD;
-
-  // this warp's 16 query rows -> its private slice of sq -> A fragments for the 4 k-steps over d
-  uint32_t qa[4][4];
-  {
-    uint8_t* mine = sq + warp * 16 * 128;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const int idx = lane + c * 32;
-      const int r = idx >> 3, ch = idx & 7;
-      uint4 v = make_uint4(0u, 0u, 0u, 0u);
-      if (q0 + r < N) v = __ldg(reinterpret_cast<const uint4*>(base + static_cast<int64_t>(q0 + r) * ld + ch * 8));
-      *reinterpret_cast<uint4*>(mine + r * 128 + ((ch ^ (r & 7)) << 4)) = v;
-    }
-    __syncwarp();
-    const uint32_t sqb = smem_u32(mine);
-    const int i = lane >> 3, r = lane & 7;
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) ldmatrix_x4(qa[kk], att_tile_addr(sqb, (i & 1) * 8 + r, kk * 16 + (i >> 1) * 8));
-  }
-  float o[8][4];
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-#pragma unroll
-    for (int c = 0; c < 4; ++c) o[j][c] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // rows g and g + 8
-
-  // K / V tiles are double buffered with cp.async: tile t+1 is in flight while tile t is multiplied
-  auto issue_tile = [&](int kv0, int stage) {
-    uint8_t* dstb = skv + stage * (2 * kAttBN * 128);
-    for (int idx = threadIdx.x; idx < 2 * kAttBN * 8; idx += blockDim.x) {
-      const int m = idx >> 9, rem = idx & 511;  // m: 0 = K, 1 = V
-      const int r = rem >> 3, ch = rem & 7;
-      const bool ok = kv0 + r < N;
-      const __nv_bfloat16* src = (m ? vp : kp) + static_cast<int64_t>(ok ? kv0 + r : 0) * ld + ch * 8;
-      const uint32_t dst = smem_u32(dstb + m * (kAttBN * 128) + r * 128 + ((ch ^ (r & 7)) << 4));
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");  // 0: zero fill
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
-  const int n_tiles = (N + kAttBN - 1) / kAttBN;
-  issue_tile(0, 0);
-  for (int tile = 0; tile < n_tiles; ++tile) {
-    const int kv0 = tile * kAttBN;
-    if (tile + 1 < n_tiles) {
-      issue_tile(kv0 + kAttBN, (tile + 1) & 1);
-      asm volatile("cp.async.wait_group 1;" ::: "memory");
-    } else {
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
-    }
-    __syncthreads();  // every thread's part of tile `tile` has landed
-    const uint32_t skb = smem_u32(skv + (tile & 1) * (2 * kAttBN * 128)), svb = skb + kAttBN * 128;
-    const int n_valid = min(kAttBN, N - kv0);  // key columns of this tile that exist
-    // S = Q K^T for 16 rows x 64 key columns
-    float sacc[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) sacc[j][c] = 0.f;
-    {
-      const int i = lane >> 3, r = lane & 7;
-#pragma unroll
-      for (int jp = 0; jp < 4; ++jp) {  // pairs of 8-column tiles
-        if (jp * 16 < n_valid) {
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            uint32_t kb[4];
-            ldmatrix_x4(kb, att_tile_addr(skb, jp * 16 + (i >> 1) * 8 + r, kk * 16 + (i & 1) * 8));
-            mma_bf16_16816(sacc[2 * jp], qa[kk], kb[0], kb[1]);
-            mma_bf16_16816(sacc[2 * jp + 1], qa[kk], kb[2], kb[3]);
-          }
-        }
-      }
-    }
-    // scale, mask the columns beyond N, online softmax
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int col = j * 8 + 2 * t + (c & 1);
-        const float v = col < n_valid ? sacc[j][c] * scale_log2e : -INFINITY;
-        sacc[j][c] = v;
-        mx[c >> 1] = fmaxf(mx[c >> 1], v);
-      }
-    }
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 1));
-      mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 2));
-    }
-    float corr[2], m_new[2];
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      m_new[rr] = fmaxf(m_run[rr], mx[rr]);  // finite: every tile has at least one valid column
-      corr[rr] = fast_exp2(m_run[rr] - m_new[rr]);
-      m_run[rr] = m_new[rr];
-    }
-    float rs[2] = {0.f, 0.f};
-    uint32_t pa[4][4];  // P as A fragments: k-step kk covers key columns 16 kk .. 16 kk + 15 = score tiles 2kk, 2kk+1
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float p0 = fast_exp2(sacc[j][0] - m_new[0]), p1 = fast_exp2(sacc[j][1] - m_new[0]);
-      const float p2 = fast_exp2(sacc[j][2] - m_new[1]), p3 = fast_exp2(sacc[j][3] - m_new[1]);
-      rs[0] += p0 + p1;
-      rs[1] += p2 + p3;
-      __nv_bfloat162 lo = __floats2bfloat162_rn(p0, p1), hi = __floats2bfloat162_rn(p2, p3);
-      pa[j >> 1][(j & 1) * 2] = *reinterpret_cast<uint32_t*>(&lo);
-      pa[j >> 1][(j & 1) * 2 + 1] = *reinterpret_cast<uint32_t*>(&hi);
-    }
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      rs[rr] += __shfl_xor_sync(0xffffffffu, rs[rr], 1);
-      rs[rr] += __shfl_xor_sync(0xffffffffu, rs[rr], 2);
-      l_run[rr] = l_run[rr] * corr[rr] + rs[rr];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      o[j][0] *= corr[0]; o[j][1] *= corr[0];
-      o[j][2] *= corr[1]; o[j][3] *= corr[1];
-    }
-    // O += P V
-    {
-      const int i = lane >> 3, r = lane & 7;
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        if (kk * 16 < n_valid) {
-#pragma unroll
-          for (int jp = 0; jp < 4; ++jp) {  // pairs of 8-wide d tiles
-            uint32_t vb[4];
-            ldmatrix_x4_trans(vb, att_tile_addr(svb, kk * 16 + (i & 1) * 8 + r, jp * 16 + (i >> 1) * 8));
-            mma_bf16_16816(o[2 * jp], pa[kk], vb[0], vb[1]);
-            mma_bf16_16816(o[2 * jp + 1], pa[kk], vb[2], vb[3]);
-          }
-        }
-      }
-    }
-    __syncthreads();  // this stage is free again for the tile after next
-  }
-  // normalise and store: rows q0 + g (+8), columns h*64 + 8j + 2t
-  const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
-  const int r0 = q0 + g, r1 = r0 + 8;
-  if (lse2 != nullptr && t == 0) {  // saved for the backward: P = exp2(s * scale_log2e - lse2)
-    float* lp = lse2 + (static_cast<int64_t>(b) * H + h) * N;
-    if (r0 < N) lp[r0] = m_run[0] + log2f(l_run[0]);
-    if (r1 < N) lp[r1] = m_run[1] + log2f(l_run[1]);
-  }
-  __nv_bfloat16* ob = out + static_cast<int64_t>(b) * N * H * kAttD + h * kAttD;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    if (r0 < N)
-      *reinterpret_cast<__nv_bfloat162*>(ob + static_cast<int64_t>(r0) * H * kAttD + j * 8 + 2 * t) =
-          __floats2bfloat162_rn(o[j][0] * inv0, o[j][1] * inv0);
-    if (r1 < N)
-      *reinterpret_cast<__nv_bfloat162*>(ob + static_cast<int64_t>(r1) * H * kAttD + j * 8 + 2 * t) =
-          __floats2bfloat162_rn(o[j][2] * inv1, o[j][3] * inv1);
-  }
-}
-
-int launch_attention_tc(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
-                        cudaStream_t s);  // attention_tc.cu
-
-static int launch_attention_mma_sync(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
-                                     cudaStream_t s);
-
-// Forward attention: the wgmma kernel (attention_tc.cu, head_dim 64, 72 or 80) by default; VDK_ATT_TC=0 selects the earlier
-// mma.sync kernel (head_dim 64 only; kept as the comparison baseline and for A/B parity tests).
-static int launch_attention(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
-                            cudaStream_t s) {
-  static const bool use_tc = [] {
-    const char* e = getenv("VDK_ATT_TC");
-    return e ? atoi(e) != 0 : true;
-  }();
-  if (!use_tc) return launch_attention_mma_sync(qkv, B, N, H, head_dim, out, lse2, s);
-  VDK_REQUIRE(head_dim == 64 || head_dim == 72 || head_dim == 80, "attention: head_dim must be 64, 72 or 80 (got %d)", head_dim);
-  const double D = head_dim;
-  ProfScope prof(kProfAttention, 4.0 * static_cast<double>(B) * H * N * N * D, 2.0 * static_cast<double>(B) * N * H * D * 4.0, s);
-  return launch_attention_tc(qkv, B, N, H, head_dim, out, lse2, s);
-}
-
-static int launch_attention_mma_sync(const __nv_bfloat16* qkv, int B, int N, int H, int head_dim, __nv_bfloat16* out, float* lse2,
-                                     cudaStream_t s) {
-  // algorithmic work: QK^T and PV = 4 * N^2 * head_dim flops per (image, head); qkv (+ o, do, dqkv) read / written once
-  ProfScope prof(kProfAttention, 4.0 * static_cast<double>(B) * H * N * N * 64.0,
-                 2.0 * static_cast<double>(B) * N * H * 64.0 * 4.0, s);
-
-  VDK_REQUIRE(head_dim == kAttD, "attention: head_dim must be 64 (got %d)", head_dim);
-  VDK_REQUIRE(B > 0 && N > 0 && H > 0 && H <= 65535 && B <= 65535, "attention: bad shape");
-  const float scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(head_dim));
-  const int row_groups = (N + 15) / 16;
-  static const int warp_cap = [] {  // tuning switch: query-row groups (warps) per CTA
-    const char* e = getenv("VDK_ATT_WARPS");
-    const int v = e ? atoi(e) : 8;
-    return v < 1 ? 1 : (v > kAttMaxWarps ? kAttMaxWarps : v);
-  }();
-  const int ctas = (row_groups + warp_cap - 1) / warp_cap;
-  const int nwarps = (row_groups + ctas - 1) / ctas;  // balanced: 197 tokens -> 1 CTA x 13 warps; 577 -> 3 CTAs x 13 warps
-  const int smem = nwarps * 16 * 128 + 2 * (2 * kAttBN * 128);
-  static bool attr = false;
-  if (!attr) {
-    VDK_CUDA_OK(cudaFuncSetAttribute(attention_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    attr = true;
-  }
-  attention_fwd_kernel<<<dim3(ctas, H, B), nwarps * 32, smem, s>>>(qkv, B, N, H, scale_log2e, out, lse2);
-  VDK_CUDA_OK(cudaGetLastError());
-  return VDK_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// attention backward for N <= 208 tokens (ViT-*/16 at 224^2: 197): one CTA per (image, head) keeps Q, K, V, dO and the
-// whole probability matrix in shared memory and runs the five products of the backward as in-CTA GEMMs on mma.sync:
-//   P = exp2(scale' Q K^T - lse2)                    (recomputed from the saved log-sum-exp)
-//   dV = P^T dO;  dP = dO V^T;  dS = scale P (dP - D),  D_i = sum_d dO_id O_id;  dQ = dS K;  dK = dS^T Q
-// Warp w owns rows 16w .. 16w+15 of whichever matrix is being produced.
-// ------------------------------------------------------------------------------------------------
 constexpr int kAttBwdMaxRows = 208;
 constexpr int kAttPStride = 432;  // bytes per row of P (208 bf16 = 416, padded so that 8 rows hit 8 distinct 16-byte bank groups)
 
@@ -775,21 +557,6 @@ static int vit_train_layout(const vdk_vit_net* n, int batch, VitTrainLayout* L) 
   return VDK_OK;
 }
 
-__global__ void vit_slab_bias_kernel(const float* __restrict__ slabs, int n_slabs, size_t stride, const float* __restrict__ bias, int rows,
-                                     int cols, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= rows * cols) return;
-  float v = bias[i % cols];
-  for (int s = 0; s < n_slabs; ++s) v += slabs[s * stride + i];
-  out[i] = v;
-}
-__global__ void vit_colsum_f32_kernel(const float* __restrict__ x, int rows, int cols, float* __restrict__ out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= cols) return;
-  float s = 0.f;
-  for (int r = 0; r < rows; ++r) s += x[static_cast<size_t>(r) * cols + c];
-  out[c] += s;
-}
 // backward of vit_assemble: dtok[b, i] = dx[b, 1 + i];  dpos[t] += sum_b dx[b, t];  dcls += sum_b dx[b, 0]
 __global__ void __launch_bounds__(256)
 vit_assemble_bwd_kernel(const __nv_bfloat16* __restrict__ dx, int B, int N, int C, __nv_bfloat16* __restrict__ dtok,
@@ -914,8 +681,7 @@ extern "C" int vdk_vit_train_forward(const vdk_vit_net* net, const vdk_vit_tenso
     const size_t slab = static_cast<size_t>(batch) * F;
     RC(G.run(B16(L.f2), net->neck_w, F32(L.zslab), batch, F, Kn, Kn, Kn, F, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_FP32, split,
              split > 1 ? static_cast<long long>(slab) : 0, 0, 0));
-    vit_slab_bias_kernel<<<(batch * F + 255) / 256, 256, 0, s>>>(F32(L.zslab), split, slab, p->lin_b, batch, F, F32(L.z));
-    VDK_CUDA_OK(cudaGetLastError());
+    RC(launch_slab_reduce_bias(F32(L.zslab), split, slab, p->lin_b, batch, F, F32(L.z), s));
     RC(launch_bn_fwd_f32(F32(L.z), batch, F, p->bn1_w, p->bn1_b, 1e-5f, bn_momentum, out_feats, F32(L.bn_mean), F32(L.bn_rstd),
                          p->bn1_running_mean, p->bn1_running_var, s));
   }
@@ -946,8 +712,7 @@ static int vit_backward_range(const vdk_vit_net* net, const vdk_vit_tensors* p, 
   // ---- neck: BatchNorm1d (batch statistics) <- Linear <- LayerNorm(neck) <- LayerNorm(final) ----
   if (active(0)) {
   RC(launch_bn_bwd_f32(d_feats, F32(L.z), batch, F, p->bn1_w, F32(L.bn_mean), F32(L.bn_rstd), F32(L.dz), g->bn1_w, g->bn1_b, s));
-  vit_colsum_f32_kernel<<<(F + 255) / 256, 256, 0, s>>>(F32(L.dz), batch, F, g->lin_b);
-  VDK_CUDA_OK(cudaGetLastError());
+  RC(launch_col_sum_f32_small(F32(L.dz), batch, F, g->lin_b, s));
   RC(launch_cast_bf16(F32(L.dz), static_cast<int64_t>(batch) * F, B16(L.dzb), s));
   // dW[F, Kn] = dZ^T . f2 (contraction over the batch): plain stores into scratch, then += into the gradient
   RC(G.run(B16(L.dzb), B16(L.f2), F32(L.gw), F, Kn, batch, F, Kn, Kn, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_FP32, 1, 0, 1, 1));

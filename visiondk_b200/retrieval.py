@@ -14,7 +14,6 @@ candidates; every returned score is re-computed from the fp32 rows.
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import Optional, Tuple
 
 import numpy as np
@@ -381,19 +380,17 @@ def bound_from_sketches(sketches: torch.Tensor, ranks, k: int, bound: torch.Tens
 class _Exchange:
     """What the shards of a sharded search tell each other after every gallery range, and the range schedule they all follow.
 
-    sketch mode (default): every shard publishes lower bounds of its canonical scores at ranks k, k/2, k/4, ... (one all-gather
-    of 4 * n_ranks bytes per query) and each shard derives the best provable lower bound of the GLOBAL k-th score
-    (bound_from_sketches): ~ the k-th score of the union of all prefixes when a query's neighbours are spread over the shards,
-    the best shard's k-th when they sit in one.  VDK_SHARD_SKETCH=0: element-wise max of the shards' k-th bounds only."""
+    Every shard publishes lower bounds of its canonical scores at ranks k, k/2, k/4, ... (one all-gather of 4 * n_ranks bytes
+    per query) and each shard derives the best provable lower bound of the GLOBAL k-th score (bound_from_sketches): ~ the k-th
+    score of the union of all prefixes when a query's neighbours are spread over the shards, the best shard's k-th when they sit
+    in one.  At k = 1 the sketch is the k-th bound alone, and the exchange is its element-wise max over the shards."""
 
     def __init__(self, schedule, comm, k: int):
         self.schedule, self.comm, self.k = schedule, comm, int(k)
-        ranks = [self.k]
-        if os.environ.get("VDK_SHARD_SKETCH", "1") != "0":
-            r, w = self.k, 1
-            while w < comm.world and len(ranks) < 8 and r > 1:
-                r, w = -(-r // 2), w * 2
-                ranks.append(r)
+        ranks, r, w = [self.k], self.k, 1
+        while w < comm.world and len(ranks) < 8 and r > 1:
+            r, w = -(-r // 2), w * 2
+            ranks.append(r)
         self.ranks = ranks
 
     def __call__(self, bound: torch.Tensor, sketch) -> None:
@@ -408,10 +405,9 @@ def shard_schedule(ng_max: int, world: int, k: int):
     """Gallery range ends every shard of a `world`-way search follows (computed from the LARGEST shard).  After a range every
     shard knows (from the rank sketches) about the k-th score of the union of `world` prefixes, so the next range may grow `world`
     times faster at the same expected admissions per query: 2 ranges per shard on 8 GPUs instead of 3.
-    The first range is the single-GPU one and the growth 1 + 7 * world.  VDK_SHARD_FIRST / VDK_SHARD_GROWTH override (tuning)."""
-    first = int(os.environ.get("VDK_SHARD_FIRST", min(max(4096, (4 * k + 255) // 256 * 256), 16384)))
-    first = min(first, (max(ng_max, 1) + 255) // 256 * 256)
-    growth = int(os.environ.get("VDK_SHARD_GROWTH", 1 + 7 * world))
+    The first range is the single-GPU one and the growth 1 + 7 * world."""
+    first = min(max(4096, (4 * k + 255) // 256 * 256), 16384, (max(ng_max, 1) + 255) // 256 * 256)
+    growth = 1 + 7 * world
     schedule, e = [], first
     while e < ng_max and len(schedule) < 7:
         schedule.append(e)
