@@ -57,6 +57,12 @@ int vdk_device_check(void);
 #define VDK_EPI_SILU 7           /* D = silu(acc + bias[n])  (conv + folded BatchNorm + SiLU) */
 #define VDK_EPI_SILU_RESIDUAL 8  /* D = residual[m,n] + silu(acc + bias[n])  (timm's ConvBnAct with skip: the activation first) */
 #define VDK_EPI_HARDSWISH 9      /* D = v relu6(v + 3) / 6 with v = acc + bias[n]  (MobileNetV3's hard-swish, nn.Hardswish) */
+/* vdk_gemm, trans_a = 0, trans_b = 1, bf16 in and out only: the LayerNorm backward of the layer whose output gradient the
+ * GEMM computes.  dy = bf16(acc); per row and group of ln_group columns, with xh = (y - beta) / gamma from the saved
+ * LayerNorm output y = residual and g = dy gamma:  D = rstd (g - mean(g) - xh mean(g xh));  ln_dgamma += sum_rows dy xh,
+ * ln_dbeta += sum_rows dy (per-CTA partials reduced in a fixed order: deterministic).  The same arithmetic as
+ * vdk_layernorm_bwd on bf16(dy), including its gamma == 0 / |gamma| < 1e-12 handling. */
+#define VDK_EPI_LN_BWD 10
 
 typedef struct vdk_gemm_desc {
   const void* A; /* [M,K] 16-bit, pitch lda */
@@ -84,6 +90,16 @@ typedef struct vdk_gemm_desc {
   float* a_col_sums; /* may be NULL; trans_a with split_k > 1 and split_stride > 0 only: split s also stores the column
                         sums of A over its K range, sum_k A[k,m] in fp32, to a_col_sums[s*M + m] (the bias gradient of
                         the wgrad above, from the A tiles the GEMM streams anyway).  16-byte aligned. */
+  /* VDK_EPI_LN_BWD only (gamma, beta: the LayerNorm's weight and bias; residual: its saved bf16 output [M,ldr]): */
+  const float* ln_rstd; /* 1/sigma per LayerNorm row (pixel) */
+  float* ln_dgamma;     /* [ln_group] += */
+  float* ln_dbeta;      /* [ln_group] += */
+  float* ln_slab;       /* scratch of 2 * N * (number of SMs) floats, 16-byte aligned */
+  int ln_group;         /* LayerNorm width: 128, 256, 512 or 1024, dividing N (128 unless N % 256 == 0); a width above
+                           the 256-column tile runs as clusters of ln_group / 256 CTAs */
+  int ln_wo;            /* 0: D is [M,ldd] like the GEMM output.  > 0: row m holds the 2x2 patch (b, ho, wo) of an NHWC
+                           image of width 2 ln_wo, column q ln_group + c its pixel (2 ho + q / 2, 2 wo + q % 2), channel c
+                           (N = 4 ln_group); D and ln_rstd are in that image's [B, 2 Ho, 2 ln_wo, ln_group] pixel order */
 } vdk_gemm_desc;
 int vdk_gemm(const vdk_gemm_desc* desc, void* stream);
 /* Number of K splits vdk_gemm will actually use for (K, split_k). */

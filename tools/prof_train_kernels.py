@@ -124,6 +124,31 @@ if stage < 3:
     kernels["downsample (bias)"] = (lambda: gemm(x.reshape(Md, 4 * Cn), dsw, dso, Md, 2 * Cn, 4 * Cn, 4 * Cn, 4 * Cn, 2 * Cn,
                                                  bias=dsb.data_ptr()), 2.0 * Md * 2 * Cn * 4 * Cn,
                                     2.0 * (Md * 4 * Cn + 8 * Cn * Cn + Md * 2 * Cn), inst(2 * Cn))
+    # its backward: dgrad into the 2x2 patch rows, then the LayerNorm backward over them (ln_bwd patch mode 2)
+    dsdy = bf(Md, 2 * Cn)
+    kernels["downsample dgrad"] = (lambda: gemm(dsdy, dsw, x.reshape(Md, 4 * Cn), Md, 4 * Cn, 2 * Cn, 2 * Cn, 4 * Cn, 4 * Cn, tb=1),
+                                   2.0 * Md * 2 * Cn * 4 * Cn, 2.0 * (Md * 2 * Cn + 8 * Cn * Cn + Md * 4 * Cn), inst(4 * Cn, tb=1))
+    kernels["ln_bwd (2x2 patch rows)"] = (lambda: _lib.check(lib.vdk_layernorm_bwd(dy.data_ptr(), x.data_ptr(), rstd.data_ptr(), B, H, H, Cn,
+                                                                                  ln_w.data_ptr(), ln_b.data_ptr(), 2, y.data_ptr(), 0,
+                                                                                  dgamma.data_ptr(), dbeta.data_ptr(), sp), "lnb2"),
+                                          0.0, 6.0 * M * Cn, None)
+
+# the LayerNorm backward in the epilogue of the dgrad GEMM that produces its input gradient (VDK_EPI_LN_BWD): against the
+# sum of "fc1 dgrad" + "ln_bwd" and of "downsample dgrad" + "ln_bwd (2x2 patch rows)" (C = 512 / 1024: clusters of 2 / 4)
+if Cn in (128, 256, 512, 1024):
+    def ln_fused(A, Bw, N_, K_, wo):
+        g = _lib.GemmDesc(A=A.data_ptr(), B=Bw.data_ptr(), D=out.data_ptr(), M=A.shape[0], N=N_, K=K_, lda=K_, ldb=N_, ldd=N_,
+                          in_dtype=_lib.DTYPE_BF16, out_dtype=_lib.DTYPE_BF16, epilogue=_lib.EPI_LN_BWD, gamma=ln_w.data_ptr(),
+                          beta=ln_b.data_ptr(), residual=x.data_ptr(), ldr=N_, split_k=1, trans_b=1, ln_rstd=rstd.data_ptr(),
+                          ln_dgamma=dgamma.data_ptr(), ln_dbeta=dbeta.data_ptr(), ln_slab=slabs.data_ptr(), ln_group=Cn, ln_wo=wo)
+        _lib.check(lib.vdk_gemm(C.byref(g), sp), "gemm ln_bwd")
+
+    kernels["fc1 dgrad + LN bwd (fused)"] = (lambda: ln_fused(hpost, w1, Cn, 4 * Cn, 0), 8.0 * M * Cn * Cn, 2.0 * M * Cn * 7,
+                                             f"BN{256 if Cn % 256 == 0 else 128} ta0 tb1 ln_bwd cluster{max(1, Cn // 256)}")
+    if stage < 3:
+        kernels["downsample dgrad + LN bwd (fused)"] = (lambda: ln_fused(dsdy, dsw, 4 * Cn, 2 * Cn, H // 2), 2.0 * Md * 2 * Cn * 4 * Cn,
+                                                        2.0 * (Md * 2 * Cn + 8 * Cn * Cn) + 6.0 * M * Cn,
+                                                        f"BN256 ta0 tb1 ln_bwd cluster{max(1, Cn // 256)}")
 
 
 for name, (fn, flops, bytes_, instantiation) in kernels.items():

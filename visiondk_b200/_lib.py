@@ -18,6 +18,7 @@ EPI_NONE, EPI_GELU, EPI_SCALE_RESIDUAL, EPI_LAYERNORM, EPI_MUL_GELU_GRAD = 0, 1,
 EPI_RELU, EPI_RESIDUAL_RELU = 5, 6  # vdk_conv2d only
 EPI_SILU, EPI_SILU_RESIDUAL = 7, 8  # vdk_conv2d_ex only
 EPI_HARDSWISH = 9  # vdk_conv2d_ex only
+EPI_LN_BWD = 10  # vdk_gemm, trans_b only
 
 
 class HeadDesc(C.Structure):
@@ -63,6 +64,8 @@ class GemmDesc(C.Structure):
         ("bias", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("residual", C.c_void_p),
         ("ldr", C.c_int), ("ln_eps", C.c_float), ("split_k", C.c_int), ("split_stride", C.c_longlong), ("aux_out", C.c_void_p), ("trans_a", C.c_int),
         ("trans_b", C.c_int), ("a_col_sums", C.c_void_p),
+        ("ln_rstd", C.c_void_p), ("ln_dgamma", C.c_void_p), ("ln_dbeta", C.c_void_p), ("ln_slab", C.c_void_p),
+        ("ln_group", C.c_int), ("ln_wo", C.c_int),
     ]
 
 

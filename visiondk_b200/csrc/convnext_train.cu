@@ -16,6 +16,11 @@ namespace vdk {
 
 static size_t al(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 
+// A LayerNorm of C channels whose backward runs in the epilogue of the data-gradient GEMM that produces its input
+// gradient (VDK_EPI_LN_BWD): a row fills part of one GEMM tile, one tile, or 2 / 4 tiles of a cluster.  Other widths
+// take the GEMM + ln_bwd pair.
+static bool ln_bwd_fuses(int C) { return C == 128 || C == 256 || C == 512 || C == 1024; }
+
 struct StageDims {
   int H, W, C;
   size_t M;
@@ -83,7 +88,8 @@ static void make_layout(const vdk_convnext_net* net, int batch, TrainLayout* L) 
   // backward scratch
   L->dxa = take(max_mc * 2);
   L->dxb = take(max_mc * 2);
-  L->dy = take(max_mc * 2);
+  // also the fused LN-backward slab: 2 N sm_count() floats, N up to 4 x 1024 (the patch rows of a 1024-channel downsample)
+  L->dy = take(std::max(max_mc * 2, static_cast<size_t>(2) * 4096 * sm_count() * 4));
   L->dconv = take(max_mc * 2);
   L->G = take(max_cc4 * 4);
   // per-block scratch (zeroed once per backward): column sums of dOut, tap gradients in [49][C] layout
@@ -460,10 +466,16 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
                B16(L.hpre[k]), 4 * C, VDK_DTYPE_BF16, 1, 0, 0, 1));
       __nv_bfloat16* dh = B16(L.hpost[k]);
       RC(G.wgrad(dh, B16(L.y[k]), gb->fc1_w, 4 * C, C, M, 4 * C, C, F32(L.wslab), true, gb->fc1_b));
-      RC(G.run(dh, b->fc1_w, B16(L.dy), M, C, 4 * C, 4 * C, C, C, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_BF16, 1, 0, 0, 1));
-      // LayerNorm backward, depthwise weight gradient, depthwise data gradient (+ the residual branch)
-      RC(launch_ln_bwd(B16(L.dy), B16(L.y[k]), F32(L.rstd[k]), batch, H, W, C, b->ln_w, b->ln_b, 1, B16(L.dconv), nullptr, gb->ln_w,
-                       gb->ln_b, s));
+      // fc1 data gradient, then the LayerNorm backward: fused into the GEMM's epilogue where a row fits one tile
+      if (ln_bwd_fuses(C)) {
+        RC(G.ln_bwd(dh, b->fc1_w, B16(L.dconv), M, C, 4 * C, B16(L.y[k]), F32(L.rstd[k]), b->ln_w, b->ln_b, C, 0, gb->ln_w, gb->ln_b,
+                    F32(L.dy)));
+      } else {
+        RC(G.run(dh, b->fc1_w, B16(L.dy), M, C, 4 * C, 4 * C, C, C, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0, VDK_DTYPE_BF16, 1, 0, 0, 1));
+        RC(launch_ln_bwd(B16(L.dy), B16(L.y[k]), F32(L.rstd[k]), batch, H, W, C, b->ln_w, b->ln_b, 1, B16(L.dconv), nullptr, gb->ln_w,
+                         gb->ln_b, s));
+      }
+      // depthwise weight gradient, depthwise data gradient (+ the residual branch)
       // tap gradients stay in the kernel's [49][C] layout in this block's scratch; un-permuted per stage below
       RC(launch_dwconv7_wgrad(B16(L.xs[st][j]), B16(L.dconv), batch, H, W, C, F32(L.dw49) + static_cast<size_t>(k) * 49 * 2048, gb->dw_b, s));
       RC(launch_dwconv7(1, B16(L.dconv), batch, H, W, C, b->dw_w_flip, nullptr, nullptr, nullptr, 0.f, B16(dx_other), nullptr,
@@ -489,10 +501,15 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
       const int Cin = L.st[st - 1].C;
       RC(G.wgrad(B16(dx), B16(L.patch[st]), F32(L.gwc), C, 4 * Cin, M, C, 4 * Cin, F32(L.wslab), false, gd->conv_b));
       RC(launch_permute021(F32(L.gwc), C, 4, Cin, nullptr, nullptr, gd->conv_w, 1, s));  // [C][4][Cin] -> += [C][Cin][4]
-      RC(G.run(B16(dx), d->conv_w, B16(L.dy), M, 4 * Cin, C, C, 4 * Cin, 4 * Cin, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0,
-               VDK_DTYPE_BF16, 1, 0, 0, 1));
-      RC(launch_ln_bwd(B16(L.dy), B16(L.patch[st]), F32(L.prstd[st]), batch, L.st[st - 1].H, L.st[st - 1].W, Cin, d->ln_w, d->ln_b, 2,
-                       B16(dx_other), nullptr, gd->ln_w, gd->ln_b, s));
+      if (ln_bwd_fuses(Cin)) {  // the patch row's 4 Cin columns hold 4 LayerNorm groups
+        RC(G.ln_bwd(B16(dx), d->conv_w, B16(dx_other), M, 4 * Cin, C, B16(L.patch[st]), F32(L.prstd[st]), d->ln_w, d->ln_b, Cin,
+                    L.st[st].W, gd->ln_w, gd->ln_b, F32(L.dy)));
+      } else {
+        RC(G.run(B16(dx), d->conv_w, B16(L.dy), M, 4 * Cin, C, C, 4 * Cin, 4 * Cin, VDK_EPI_NONE, nullptr, nullptr, nullptr, 0,
+                 VDK_DTYPE_BF16, 1, 0, 0, 1));
+        RC(launch_ln_bwd(B16(L.dy), B16(L.patch[st]), F32(L.prstd[st]), batch, L.st[st - 1].H, L.st[st - 1].W, Cin, d->ln_w, d->ln_b,
+                         2, B16(dx_other), nullptr, gd->ln_w, gd->ln_b, s));
+      }
       std::swap(dx, dx_other);
     }
   }

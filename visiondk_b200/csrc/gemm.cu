@@ -20,6 +20,8 @@
 #include <algorithm>
 #include <cstdlib>
 
+#include "train_gemm.h"
+
 namespace vdk {
 
 constexpr int kBM = 128;
@@ -46,6 +48,8 @@ constexpr int kConvExIm2col = 5;
 // be 16-byte aligned), as cv_cpb 64-channel blocks per tap (channels past Cin are TMA zero fill; the packed weight is
 // zero outside each output channel's own group)
 constexpr int kConvGroupedEx = 6;
+// dense dgrad (kTA = 0, kTB = 1) with the LayerNorm-backward epilogue VDK_EPI_LN_BWD (ln_bwd_tile below)
+constexpr int kGemmLnBwd = 7;
 
 // The implicit-GEMM convolution modes (kConvIm2col) overlay their geometry on fields they do not use, so that the struct —
 // and with it the code of the plain GEMM instantiations — stays as it is.
@@ -74,7 +78,8 @@ struct GemmParams {
   int epilogue;
   union {
     float ln_eps;
-    int cv_cg_in;  // kConvGroupedEx: input channels per group
+    int cv_cg_in;    // kConvGroupedEx: input channels per group
+    int ln_cluster;  // kGemmLnBwd: ln_group / BN > 1: a row spans this many tiles, the CTAs of one thread-block cluster
   };
   int split_k;  // > 1: each tile's K range is split over split_k work items, fp32 partials are atomically added
   union {
@@ -88,9 +93,17 @@ struct GemmParams {
     // split-K slabs with an MN-major A only (the weight-gradient form): split s also stores the column sums of A over
     // its K range, sum_k A[k, m], to col_sums[s * M + m] (the bias gradient, summed in the producer warpgroup)
     float* col_sums;
+    float* ln_slab;  // kGemmLnBwd: one row [2][N] of dgamma / dbeta partials per group of num_n CTAs
   };
   int partial_out;  // the caller asked for split-K: raw fp32 partials are added / slab-stored even if one split remains
+  // kGemmLnBwd only (appended, so that the other instantiations read every field at the offset they did)
+  const float* ln_rstd;
+  int ln_group, ln_wo;
 };
+// kGemmLnBwd: the row-sum exchange of a cluster behind the barriers, per consumer warpgroup and tile parity: one float2
+// (sum g, sum g xh) per row from each of up to 4 ranks, and its mbarrier
+constexpr int kLnXchBytes = 2 * 2 * 4 * 64 * 8;
+constexpr int kLnSmemBytes = kLnXchBytes + 4 * 8;
 
 template <int BN>
 struct GemmCfg {
@@ -258,6 +271,201 @@ __device__ __forceinline__ void epi_publish(const CUtensorMap* map, const uint8_
 // byte offset of the 16-byte chunk `chunk` of row `row` in a 128-byte-swizzled box (the TMA SWIZZLE_128B pattern)
 __device__ __forceinline__ uint32_t box_off(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
 
+// kGemmLnBwd: the LayerNorm pixel of GEMM row m, group q (the rstd index; D's row in units of ln_group elements)
+__device__ __forceinline__ long long ln_pixel(const GemmParams& p, int m, int q) {
+  if (p.ln_wo == 0) return m;
+  const int bho = m / p.ln_wo, wo = m - bho * p.ln_wo;
+  return ((static_cast<long long>(bho) * 2 + (q >> 1)) * p.ln_wo + wo) * 2 + (q & 1);
+}
+
+// Sum of v[i] over the 8 lanes that hold the same fragment columns (lane bits 2-4), by recursive halving (14 shuffles,
+// not 48): afterwards v[0], v[1] hold the sums of entries 8 b4 + 4 b3 + 2 b2 + {0, 1} (b = the lane's bits).
+__device__ __forceinline__ void halve_columns(float (&v)[16], int lane) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const bool up = (lane & 16) != 0;
+    v[i] = (up ? v[i + 8] : v[i]) + __shfl_xor_sync(0xffffffffu, up ? v[i] : v[i + 8], 16);
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const bool up = (lane & 8) != 0;
+    v[i] = (up ? v[i + 4] : v[i]) + __shfl_xor_sync(0xffffffffu, up ? v[i] : v[i + 4], 8);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const bool up = (lane & 4) != 0;
+    v[i] = (up ? v[i + 2] : v[i]) + __shfl_xor_sync(0xffffffffu, up ? v[i] : v[i + 2], 4);
+  }
+}
+
+// st.async of a float2 into the shared memory of a CTA of the cluster, completing `bytes` on its mbarrier
+__device__ __forceinline__ void st_async_f2(uint32_t local_addr, uint32_t local_bar, uint32_t rank, float a, float b) {
+  uint32_t ra, rb;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(local_bar), "r"(rank));
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
+               :: "r"(ra), "f"(a), "f"(b), "r"(rb) : "memory");
+}
+
+// kGemmLnBwd epilogue of one warpgroup's 64 x BN half tile; the saved LayerNorm output y has landed in ring boxes
+// 0 .. BN / 64 - 1.  ln_bwd_kernel's arithmetic (train_ops.cu) on dy = bf16(acc): pass 1 rounds dy in place and sums, per
+// row and group, g = dy gamma and g xh with xh = (y - beta) (1 / gamma); pass 2 writes D = rstd (g - m1 - xh m2) through
+// the ring (stmatrix, then 128-byte row pieces, so that the patch layout needs no TMA view).  colp[box][2 qty + i]
+// accumulates over the CTA's tiles the column sum of dy xh (qty 0) / dy (qty 1) of box column 8 (4 b4 + 2 b3 + b2) +
+// fcol + i (halve_columns).  A tile holds at most two groups (ln_group >= 128).  A group wider than the tile (ln_cluster
+// > 1 CTAs, one per tile of the row) completes its row sums across the cluster: every CTA sends its partial of each row
+// to every rank's `xch` slot [own rank][row] with st.async on that rank's `xbar`, and adds the ranks' partials in rank
+// order, so that all of them use the same statistics.
+template <int BN>
+__device__ __forceinline__ void ln_bwd_tile(const GemmParams& p, float (&acc)[BN / 2], float (&colp)[BN / 64][4], const float* par,
+                                            uint8_t* ring, int wrow0, int n0, int fcol, int frow, int mrow, int mcb, int wl,
+                                            int lane, uint8_t* xch, uint64_t* xbar, uint32_t xphase, bool leader) {
+  constexpr int kGroups = BN / 128;
+  const int G = p.ln_group;
+  float rs[kGroups][2], s1[kGroups][2], s2[kGroups][2];
+#pragma unroll
+  for (int gi = 0; gi < kGroups; ++gi)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = wrow0 + frow + 8 * h;
+      rs[gi][h] = (gi * G < BN && m < p.M) ? __ldg(p.ln_rstd + ln_pixel(p, m, (n0 + gi * G) / G)) : 0.f;
+      s1[gi][h] = 0.f;
+      s2[gi][h] = 0.f;
+    }
+#pragma unroll
+  for (int sc = 0; sc < BN / 64; ++sc) {
+    const uint32_t box = smem_u32(ring + sc * kBoxBytes);
+    float v[16], t1[2] = {0.f, 0.f}, t2[2] = {0.f, 0.f};  // v[2 jj + e]: dy xh of box column 8 jj + fcol + e
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      uint32_t rin[4];
+      ldmatrix_x4(rin, box + box_off(mrow, 2 * q + mcb));
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int jj = 2 * q + (i >> 1), j = sc * 8 + jj, h = i & 1, c = j * 8 + fcol;
+        const float2 d = unpack2(pack2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], VDK_DTYPE_BF16), VDK_DTYPE_BF16);
+        acc[4 * j + 2 * h] = d.x;
+        acc[4 * j + 2 * h + 1] = d.y;
+        const float2 yv = unpack2(rin[i], VDK_DTYPE_BF16);
+        const float2 w = *reinterpret_cast<const float2*>(par + c);
+        const float2 iw = *reinterpret_cast<const float2*>(par + BN + c);
+        const float2 b = *reinterpret_cast<const float2*>(par + 2 * BN + c);
+        const float h0 = (yv.x - b.x) * iw.x, h1 = (yv.y - b.y) * iw.y;
+        const float g0 = d.x * w.x, g1 = d.y * w.y;
+        t1[h] += g0;
+        t2[h] = fmaf(g0, h0, t2[h]);
+        t1[h] += g1;
+        t2[h] = fmaf(g1, h1, t2[h]);
+        v[2 * jj] = h == 0 ? d.x * h0 : fmaf(d.x, h0, v[2 * jj]);
+        v[2 * jj + 1] = h == 0 ? d.y * h1 : fmaf(d.y, h1, v[2 * jj + 1]);
+      }
+    }
+    const int gi = sc * 64 / G;
+#pragma unroll
+    for (int gg = 0; gg < kGroups; ++gg)
+      if (gg == gi)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          s1[gg][h] += t1[h];
+          s2[gg][h] += t2[h];
+        }
+    halve_columns(v, lane);
+    colp[sc][0] += v[0];
+    colp[sc][1] += v[1];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) v[2 * jj + e] = acc[4 * (sc * 8 + jj) + e] + acc[4 * (sc * 8 + jj) + 2 + e];
+    halve_columns(v, lane);
+    colp[sc][2] += v[0];
+    colp[sc][3] += v[1];
+  }
+  const float inv_g = 1.0f / static_cast<float>(G);
+#pragma unroll
+  for (int gi = 0; gi < kGroups; ++gi) {
+    if (gi * G >= BN) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      s1[gi][h] += __shfl_xor_sync(0xffffffffu, s1[gi][h], 1);
+      s1[gi][h] += __shfl_xor_sync(0xffffffffu, s1[gi][h], 2);
+      s2[gi][h] += __shfl_xor_sync(0xffffffffu, s2[gi][h], 1);
+      s2[gi][h] += __shfl_xor_sync(0xffffffffu, s2[gi][h], 2);
+    }
+  }
+  if (p.ln_cluster > 1) {  // G > BN: one group per tile (gi = 0)
+    const uint32_t rank = cluster_ctarank();
+    if (leader) mbar_arrive_expect_tx(xbar, p.ln_cluster * 64 * 8);
+    if ((lane & 3) == 0)
+      for (int r = 0; r < p.ln_cluster; ++r)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          st_async_f2(smem_u32(xch + (rank * 64 + frow + 8 * h) * 8), smem_u32(xbar), r, s1[0][h], s2[0][h]);
+    mbar_wait<true>(xbar, xphase);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float a = 0.f, b = 0.f;
+      for (int r = 0; r < p.ln_cluster; ++r) {
+        const float2 t = *reinterpret_cast<const float2*>(xch + (r * 64 + frow + 8 * h) * 8);
+        a += t.x;
+        b += t.y;
+      }
+      s1[0][h] = a;
+      s2[0][h] = b;
+    }
+  }
+#pragma unroll
+  for (int gi = 0; gi < kGroups; ++gi)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      s1[gi][h] *= inv_g;
+      s2[gi][h] *= inv_g;
+    }
+  __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.D);
+#pragma unroll
+  for (int sc = 0; sc < BN / 64; ++sc) {
+    uint8_t* boxp = ring + sc * kBoxBytes;
+    const uint32_t box = smem_u32(boxp);
+    const int gi = sc * 64 / G;
+    float m1[2], m2[2], r[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // the group's row statistics, selected without dynamic register indexing
+      m1[h] = s1[0][h]; m2[h] = s2[0][h]; r[h] = rs[0][h];
+#pragma unroll
+      for (int gg = 1; gg < kGroups; ++gg)
+        if (gg == gi) { m1[h] = s1[gg][h]; m2[h] = s2[gg][h]; r[h] = rs[gg][h]; }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t addr = box + box_off(mrow, 2 * q + mcb);
+      uint32_t rin[4], rq[4];
+      ldmatrix_x4(rin, addr);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int j = sc * 8 + 2 * q + (i >> 1), h = i & 1, c = j * 8 + fcol;
+        const float2 yv = unpack2(rin[i], VDK_DTYPE_BF16);
+        const float2 w = *reinterpret_cast<const float2*>(par + c);
+        const float2 iw = *reinterpret_cast<const float2*>(par + BN + c);
+        const float2 b = *reinterpret_cast<const float2*>(par + 2 * BN + c);
+        const float h0 = (yv.x - b.x) * iw.x, h1 = (yv.y - b.y) * iw.y;
+        const float o0 = r[h] * (acc[4 * j + 2 * h] * w.x - m1[h] - h0 * m2[h]);
+        const float o1 = r[h] * (acc[4 * j + 2 * h + 1] * w.y - m1[h] - h1 * m2[h]);
+        rq[i] = pack2(o0, o1, VDK_DTYPE_BF16);
+      }
+      stmatrix_x4(addr, rq);
+    }
+    __syncwarp();  // the warp reads back only its own 16 rows
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+      const int row = wl * 16 + it * 4 + (lane >> 3), chunk = lane & 7, m = wrow0 + row;
+      if (m < p.M) {
+        const int n = n0 + sc * 64 + chunk * 8, qg = n / G;
+        const long long off = p.ln_wo == 0 ? static_cast<long long>(m) * p.ldd + n : ln_pixel(p, m, qg) * G + (n - qg * G);
+        *reinterpret_cast<uint4*>(dst + off) = *reinterpret_cast<const uint4*>(boxp + box_off(row, chunk));
+      }
+    }
+  }
+}
+
 // kTA / kTB: operand stored with the contraction index as the slow dimension ([K,M] / [K,N] row-major: MN-major)
 // kMode: kGemmPlain, kConvDense, kConvIm2col or kConvGrouped (see above)
 template <int BN, bool kBf16, int kTA, int kTB, int kMode>
@@ -288,7 +496,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     prefetch_tensormap(&map_b);
     prefetch_tensormap(&map_d);
     if (p.aux != nullptr) prefetch_tensormap(&map_aux);
-    if (p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
+    if (kMode == kGemmLnBwd || p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
         (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU) || (kConvEx && p.epilogue == VDK_EPI_SILU_RESIDUAL))
       prefetch_tensormap(&map_r);
     for (int i = 0; i < kStages; ++i) {
@@ -297,9 +505,14 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     }
     mbar_init(&res_bar[0], 1);
     mbar_init(&res_bar[1], 1);
+    if constexpr (kMode == kGemmLnBwd)
+      for (int i = 0; i < 4; ++i) mbar_init(reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(res_bar + 2) + kLnXchBytes) + i, 1);
     fence_mbar_init();
   }
   __syncthreads();
+  if constexpr (kMode == kGemmLnBwd) {
+    if (p.ln_cluster > 1) cluster_sync_all();  // every rank's exchange barriers are initialised before the first st.async
+  }
 
   if (threadIdx.x < 128) {
     // ===================== TMA producer =====================
@@ -458,7 +671,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     float* par = par_all + cg * Cfg::kParFloats;
     const bool f32 = p.out_dtype == VDK_DTYPE_FP32;
     const int box_cols = f32 ? 32 : 64;
-    const bool has_res = p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
+    const bool has_res = kMode == kGemmLnBwd || p.epilogue == VDK_EPI_SCALE_RESIDUAL || p.epilogue == VDK_EPI_MUL_GELU_GRAD ||
                          (kMode != kGemmPlain && p.epilogue == VDK_EPI_RESIDUAL_RELU) ||
                          (kConvEx && p.epilogue == VDK_EPI_SILU_RESIDUAL);
     const bool reduce = p.partial_out && p.split_stride == 0;  // atomic split-K: TMA reduce-add into D
@@ -467,6 +680,26 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
+    float colp[BN / 64][4] = {};  // kGemmLnBwd: this thread's column sums of dy xh / dy over the CTA's tiles
+    uint32_t ln_tiles = 0;        // kGemmLnBwd: tiles this warpgroup has finished (exchange slot parity and phase)
+    if constexpr (kMode == kGemmLnBwd) {
+      // the launch makes gridDim.x a multiple of num_n, so every tile of this CTA has the same columns: gamma, 1 / gamma
+      // and beta are staged once, with ln_bwd_kernel's handling of gamma == 0 and |gamma| < 1e-12
+      const int n0 = (blockIdx.x % num_n) * BN;
+      for (int c = ct & 127; c < BN; c += 128) {
+        const int ch = (n0 + c) % p.ln_group;  // a tile may hold several LayerNorm groups (the downsample's patch rows)
+        float w = p.gamma[ch];
+        float iw = 0.f;
+        if (w != 0.f) {
+          if (fabsf(w) < 1e-12f) w = w < 0.f ? -1e-12f : 1e-12f;
+          iw = 1.0f / w;
+        }
+        par[c] = w;
+        par[BN + c] = iw;
+        par[2 * BN + c] = p.beta[ch];
+      }
+      named_bar_sync(bar_id, 128);
+    }
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mn = tile % (num_m * num_n), split = tile / (num_m * num_n);
       const int m0 = (mn / num_n) * kBM;
@@ -480,7 +713,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       // the tile's per-column parameters (bias, gamma, beta) go to this warpgroup's copy in shared memory by cp.async, which
       // holds no registers while the MMAs run; the previous tile's epilogue has read that copy (its last barrier is behind
       // every thread of the warpgroup)
-      if (live && (ct & 127) < BN / 4) {
+      if (kMode != kGemmLnBwd && live && (ct & 127) < BN / 4) {
         const int c = (ct & 127) * 4;  // this thread's 4 columns of each array
         const bool in = n0 + c < p.N;  // N % 8 == 0: the 4 columns are all in or all out
         if (p.bias != nullptr) cp_async_16_zfill(par + c, p.bias + (in ? n0 + c : 0), in);
@@ -525,6 +758,18 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       wgmma_fence_regs(acc);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       if (!live) continue;
+      if constexpr (kMode == kGemmLnBwd) {
+        mbar_wait<true>(&res_bar[cg], res_phase);
+        res_phase ^= 1;
+        uint8_t* xch = reinterpret_cast<uint8_t*>(res_bar + 2) + (cg * 2 + (ln_tiles & 1)) * (4 * 64 * 8);
+        uint64_t* xbar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(res_bar + 2) + kLnXchBytes) + cg * 2 + (ln_tiles & 1);
+        ln_bwd_tile<BN>(p, acc, colp, par, ring, wrow0, n0, fcol, frow, mrow, mcb, wl, lane, xch, xbar, (ln_tiles >> 1) & 1, leader);
+        ++ln_tiles;
+        // every warp has read the ring before the leader loads the next tile's y into it
+        fence_proxy_async_smem();
+        named_bar_sync(bar_id, 128);
+        continue;
+      }
 
       cp_async_wait_all();
       named_bar_sync(bar_id, 128);  // the warpgroup's staged parameters are visible
@@ -673,6 +918,31 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       }
     }
     if (leader) tma_store_wait<0>();  // the ring stays valid until the last stores have read it
+    if constexpr (kMode == kGemmLnBwd) {
+      // the column sums of the 8 consumer warps meet in the (now idle) pipeline stages and are added in warp order into
+      // this CTA's slab row, laid out [N / ln_group][dgamma, dbeta][ln_group]
+      named_bar_sync(4, 256);  // both warpgroups are past their last MMAs
+      float* part = reinterpret_cast<float*>(smem);  // [8 warps][2][BN]
+      const int warp = ct >> 5, jj = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
+#pragma unroll
+      for (int sc = 0; sc < BN / 64; ++sc)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) part[(warp * 2 + (i >> 1)) * BN + sc * 64 + jj * 8 + fcol + (i & 1)] = colp[sc][i];
+      named_bar_sync(4, 256);
+      const int n0 = (blockIdx.x % num_n) * BN;
+      float* row = p.ln_slab + static_cast<size_t>(blockIdx.x / num_n) * 2 * p.N;
+      for (int t = ct; t < 2 * BN; t += 256) {
+        const int q = t / BN, c = t - q * BN;
+        float sum = 0.f;
+#pragma unroll
+        for (int w8 = 0; w8 < 8; ++w8) sum += part[(w8 * 2 + q) * BN + c];
+        const int n = n0 + c, grp = n / p.ln_group;
+        row[(grp * 2 + q) * p.ln_group + n - grp * p.ln_group] = sum;
+      }
+    }
+  }
+  if constexpr (kMode == kGemmLnBwd) {
+    if (p.ln_cluster > 1) cluster_sync_all();  // no CTA leaves while a peer's st.async may still target it
   }
 }
 
@@ -702,6 +972,94 @@ static int launch_gemm_major(const CUtensorMap* maps, const GemmParams& p, bool 
 
 namespace vdk {
 
+// kGemmLnBwd launch: a persistent grid of a multiple of num_n CTAs (each keeps one column range); rows wider than the
+// tile (cluster = G / BN > 1) run as clusters of `cluster` CTAs along N, as many as can be co-resident.  Returns the grid.
+template <int BN>
+static int launch_gemm_ln_bwd(const CUtensorMap* maps, const GemmParams& p, int cluster, cudaStream_t s, int* grid_out) {
+  constexpr int kSmem = GemmCfg<BN>::kSmemBytes + kLnSmemBytes;
+  static_assert(kSmem <= 227 * 1024, "LN-backward GEMM shared memory budget");
+  auto kern = gemm_tn_kernel<BN, true, 0, 1, kGemmLnBwd>;
+  static int fit[5] = {};  // per cluster size: co-resident CTAs (queried once)
+  cudaLaunchConfig_t cfg{};
+  cfg.blockDim = dim3(kGemmThreads);
+  cfg.dynamicSmemBytes = kSmem;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (fit[cluster] == 0) {
+    VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    int n = sm_count() / cluster;
+    if (cluster > 1) {
+      cfg.gridDim = dim3(cluster * sm_count());
+      VDK_CUDA_OK(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+    }
+    VDK_REQUIRE(n > 0, "vdk_gemm: no cluster of %d LN-backward GEMM CTAs fits on the device", cluster);
+    fit[cluster] = n * cluster;
+  }
+  const int num_n = p.N / BN, num_tiles = ((p.M + kBM - 1) / kBM) * num_n;
+  const int grid = std::min(num_tiles, fit[cluster] - fit[cluster] % num_n);
+  cfg.gridDim = dim3(grid);
+  VDK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, maps[0], maps[1], maps[2], maps[3], maps[4], p));
+  *grid_out = grid;
+  return VDK_OK;
+}
+
+// VDK_EPI_LN_BWD: dgrad D = LayerNorm_backward(bf16(A . B^T)) (B stored [K,N]), then the fixed-order reduction of the
+// per-CTA dgamma / dbeta partials
+static int gemm_ln_bwd_run(const vdk_gemm_desc& g, cudaStream_t s) {
+  const int G = g.ln_group;
+  VDK_REQUIRE(g.in_dtype == VDK_DTYPE_BF16 && g.out_dtype == VDK_DTYPE_BF16 && !g.trans_a && g.trans_b && g.split_k <= 1 &&
+                  !g.bias && !g.aux_out && !g.a_col_sums,
+              "vdk_gemm: LN_BWD needs bf16 in and out, trans_b only, no split-K, bias or auxiliary output");
+  VDK_REQUIRE(g.gamma && g.beta && g.residual && g.ln_rstd && g.ln_dgamma && g.ln_dbeta && g.ln_slab,
+              "vdk_gemm: LN_BWD needs gamma, beta, the saved output (residual), ln_rstd, ln_dgamma, ln_dbeta and ln_slab");
+  const int BN = (g.N % 256 == 0) ? 256 : 128;
+  // a group is a whole number of tiles (up to 4: one cluster), or a tile a whole number of groups
+  VDK_REQUIRE(G > 0 && G % 128 == 0 && g.N % G == 0 && (BN % G == 0 || (G % BN == 0 && G / BN <= 4 && G / BN != 3)),
+              "vdk_gemm: LN_BWD group %d must be 128, 256, 512 or 1024 and divide N=%d (tile width %d)", G, g.N, BN);
+  VDK_REQUIRE(g.lda >= g.K && g.lda % 8 == 0 && g.ldb >= g.N && g.ldb % 8 == 0 && g.ldd >= g.N && g.ldd % 8 == 0 &&
+                  (reinterpret_cast<uintptr_t>(g.D) & 15) == 0,
+              "vdk_gemm: LN_BWD pitches must cover the rows and keep them 16-byte aligned");
+  VDK_REQUIRE(g.ln_wo >= 0 && (g.ln_wo == 0 || (g.N == 4 * G && g.M % g.ln_wo == 0)),
+              "vdk_gemm: LN_BWD patch rows need N = 4 ln_group and M a multiple of ln_wo");
+  VDK_REQUIRE(g.ldr >= g.N && g.ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(g.residual) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(g.ln_slab) & 15) == 0,
+              "vdk_gemm: LN_BWD saved-output rows and ln_slab must be 16-byte aligned");
+  CUtensorMap maps[5];  // A, B, D (unused: D is written from the ring), aux_out (unused), y
+  int rc = make_tma_2d_16bit(&maps[0], g.A, (uint64_t)g.M, (uint64_t)g.K, (uint64_t)g.lda, kBM, kBK);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_2d_16bit(&maps[1], g.B, (uint64_t)g.K, (uint64_t)g.N, (uint64_t)g.ldb, kBK, 64);
+  if (rc != VDK_OK) return rc;
+  rc = make_tma_epilogue_map(&maps[4], g.residual, 2, (uint64_t)g.M, (uint64_t)g.N, (uint64_t)g.ldr, 1, 0);
+  if (rc != VDK_OK) return rc;
+  maps[2] = maps[4];
+  maps[3] = maps[4];
+  GemmParams p{};
+  p.M = g.M; p.N = g.N; p.K = g.K; p.D = g.D; p.ldd = g.ldd;
+  p.gamma = g.gamma; p.beta = g.beta; p.residual = g.residual; p.ldr = g.ldr;
+  p.out_dtype = VDK_DTYPE_BF16; p.epilogue = VDK_EPI_LN_BWD; p.split_k = 1;
+  p.ln_slab = g.ln_slab; p.ln_rstd = g.ln_rstd; p.ln_group = G; p.ln_wo = g.ln_wo;
+  p.ln_cluster = G > BN ? G / BN : 1;
+  int grid = 0;
+  {
+    // algorithmic bytes: both operands, the saved output and rstd once, the output once
+    ProfScope prof(kProfGemm, 2.0 * g.M * g.N * g.K,
+                   2.0 * (static_cast<double>(g.M) * g.K + static_cast<double>(g.N) * g.K) + 4.0 * g.M * g.N + 4.0 * g.M * (g.N / G), s);
+    rc = BN == 256 ? launch_gemm_ln_bwd<256>(maps, p, p.ln_cluster, s, &grid) : launch_gemm_ln_bwd<128>(maps, p, p.ln_cluster, s, &grid);
+    if (rc != VDK_OK) return rc;
+  }
+  // one slab row per num_n CTAs, [N / G][dgamma, dbeta][G]: grid / num_n x N / G partials of each, 2 G floats apart
+  const int n_part = grid / (g.N / BN) * (g.N / G);
+  rc = launch_slab_reduce(g.ln_slab, n_part, static_cast<size_t>(2) * G, G / 4, g.ln_dgamma, 1, s);
+  if (rc != VDK_OK) return rc;
+  return launch_slab_reduce(g.ln_slab + G, n_part, static_cast<size_t>(2) * G, G / 4, g.ln_dbeta, 1, s);
+}
+
 int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   VDK_REQUIRE(g.A && g.B && g.D, "vdk_gemm: null operand");
   VDK_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0, "vdk_gemm: empty problem M=%d N=%d K=%d", g.M, g.N, g.K);
@@ -716,6 +1074,7 @@ int gemm_run(const vdk_gemm_desc& g, cudaStream_t s) {
   const int dalign = g.out_dtype == VDK_DTYPE_FP32 ? 4 : 8;
   VDK_REQUIRE(g.ldd % dalign == 0, "vdk_gemm: ldd must keep rows 16-byte aligned");
   VDK_REQUIRE((reinterpret_cast<uintptr_t>(g.D) & 15) == 0, "vdk_gemm: D must be 16-byte aligned");
+  if (g.epilogue == VDK_EPI_LN_BWD) return gemm_ln_bwd_run(g, s);
   VDK_REQUIRE(g.epilogue >= VDK_EPI_NONE && g.epilogue <= VDK_EPI_MUL_GELU_GRAD, "vdk_gemm: bad epilogue");
   if (g.epilogue == VDK_EPI_MUL_GELU_GRAD) {
     VDK_REQUIRE(g.residual && g.out_dtype != VDK_DTYPE_FP32 && g.split_k <= 1 && !g.bias,

@@ -41,6 +41,20 @@ struct Gemm {
     g.a_col_sums = a_col_sums;
     return gemm_run(g, s);
   }
+  // data gradient dY = A . B^T (B stored [K,N]) through a LayerNorm of width `group` whose saved output is y [M,N]:
+  // dx = LayerNorm_backward(bf16(dY)) into D (wo > 0: the 2x2 patch rows of an image of width 2 wo, written to its NHWC
+  // pixels), dgamma / dbeta +=.  slab: 2 N sm_count() floats of scratch.
+  int ln_bwd(const void* A, const void* B, void* D, int M, int N, int K, const void* y, const float* rstd, const float* ln_w,
+             const float* ln_b, int group, int wo, float* dgamma, float* dbeta, float* slab) const {
+    vdk_gemm_desc g{};
+    g.A = A; g.B = B; g.D = D;
+    g.M = M; g.N = N; g.K = K; g.lda = K; g.ldb = N; g.ldd = N;
+    g.in_dtype = VDK_DTYPE_BF16; g.out_dtype = VDK_DTYPE_BF16; g.epilogue = VDK_EPI_LN_BWD;
+    g.gamma = ln_w; g.beta = ln_b; g.residual = y; g.ldr = N;
+    g.split_k = 1; g.trans_b = 1;
+    g.ln_rstd = rstd; g.ln_dgamma = dgamma; g.ln_dbeta = dbeta; g.ln_slab = slab; g.ln_group = group; g.ln_wo = wo;
+    return gemm_run(g, s);
+  }
   // weight gradient D[M,N] (+)= A^T B over a long K (A stored [K,M], B stored [K,N]): split-K partial slabs + fixed-order
   // reduction.  bias_grad (optional): += the column sums of A, sum_k A[k,m] (the bias gradient of the layer whose output
   // gradient A is), which the GEMM computes from the A tiles it streams and which are reduced over the splits the same way.
