@@ -1,8 +1,8 @@
 """Orchestrator of the faceX / CBIR embedding path on H100 — the surface of the reference's
 engine/vision_engine.py (yaml_load :35-38, increment_path :41-57, CenterProcessor.__init__ :67-167,
 run_embedding :438-560) over the visiondk_b200 kernels.  Written from scratch: model / step / eval come from
-visiondk_b200.{train,cbir} and engine.cbir.evaluation; the dataset layer is out of the hot-path scope, so `data.root`
-is a synthetic:// URL (engine/synthetic.py) or the caller drives FaceTrainer with its own (images, labels) iterables.
+visiondk_b200.{train,cbir} and engine.cbir.evaluation; `data.root` is a synthetic:// URL (engine/synthetic.py) or a local
+image folder (engine/folder_train.py: decoded on host threads, the config's train / val transform lists on the device).
 """
 from __future__ import annotations
 
@@ -19,6 +19,7 @@ import yaml
 
 from engine.cbir.evaluation import valuate as valuate_cbir
 from engine.faceX.evaluation import valuate as valuate_face
+from engine.folder_train import FolderTrainData
 from engine.synthetic import SyntheticFaceData, is_synthetic
 from visiondk_b200.train import FaceTrainer, FaceTrainingModel
 
@@ -109,11 +110,16 @@ class CenterProcessor:
                                       "H100 neck kernels (they use per-rank batch statistics); drop the flag")
         self.model = FaceTrainingModel(self.model_cfg).to(self.device)
         root = str(self.data_cfg["root"])
-        if not is_synthetic(root):
-            raise NotImplementedError("dataset loading is outside the H100 hot-path scope: use a synthetic:// root or drive "
-                                      "FaceTrainer / engine.cbir.evaluation with your own (images, labels) iterables")
-        self.data = SyntheticFaceData(root, self.model_cfg["image_size"], self.data_cfg["train"]["bs"], self.device,
-                                      max(rank, 0), self.world)
+        if is_synthetic(root):
+            self.data = SyntheticFaceData(root, self.model_cfg["image_size"], self.data_cfg["train"]["bs"], self.device,
+                                          max(rank, 0), self.world)
+        elif os.path.isdir(root):
+            head = next(iter(self.model_cfg["head"].values()))
+            self.data = FolderTrainData(root, self.data_cfg, head["num_class"], self.device, max(rank, 0), self.world,
+                                        warm_ep=self.hyp_cfg.get("warm_ep", 0))
+        else:
+            raise NotImplementedError(f"{root}: dataset roots are a synthetic:// URL or a local directory (HuggingFace hub "
+                                      "datasets need a network, which the GPU hosts may not have)")
 
     def log(self, msg: str):
         if self.rank in (-1, 0):

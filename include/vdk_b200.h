@@ -913,6 +913,53 @@ size_t vdk_preprocess_workspace_bytes(const vdk_image_desc* images, int n, int s
 int vdk_preprocess_resize_pad_normalize(const uint8_t* packed, const vdk_image_desc* images, int n, int size, const float* mean,
                                         const float* std_, float* out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- training-time image augmentation (the `data.train.augment` list of configs/faceX/{face,cbir}.yaml) ---------------- */
+/* Replaces, for a BATCH of decoded RGB images of different sizes at source resolution, the reference's training Compose
+ * (dataset/transforms.py:403-555 as built by create_AugTransforms): per image an ordered list of byte-exact PIL stages, then
+ * one resize stage into the size x size square, then ToTensor + Normalize.  The random draws are made on the host
+ * (visiondk_b200/augment.py, in the reference's order and streams); a plan holds their outcome.
+ *   BRIGHTNESS / SATURATION / CONTRAST : PIL.ImageEnhance.{Brightness,Color,Contrast}.enhance(alpha) (torchvision ColorJitter,
+ *                                        transforms.py:170-179); the contrast mean is reduced on the device
+ *   HUE        : torchvision adjust_hue on PIL (RGB->HSV, uint8 wrap-add of hue_shift, HSV->RGB)
+ *   CUTOUT     : Image.paste of n solid boxes (transforms.py:63-109): box = x1, y1, mask_w, mask_h; color = r, g, b
+ *   BLUR       : torchvision gaussian_blur on PIL (transforms.py:510-512): n-tap fp32 kernel, reflect padding, torch.round
+ *   ROTATE     : Image.rotate(angle, BILINEAR), no expand, fill 0 (transforms.py:463-465): matrix = Pillow's affine matrix
+ *   SHARPNESS  : ImageEnhance.Sharpness.enhance(alpha) (transforms.py:427-429)
+ *   HFLIP      : T.RandomHorizontalFlip (transforms.py:451-453)
+ * and the resize stage: ResizeAndPadding2Square(size, training=True) with BILINEAR or NEAREST (transforms.py:325-362), or
+ * RandomResizedCrop's crop box resized to size x size with BILINEAR (transforms.py:390-400).
+ *   packed : DEVICE uint8, every image as [height][width][3] (RGB) at images[i].offset
+ *   images, plans : HOST arrays of n entries
+ *   out    : DEVICE fp32 [n, 3, size, size]
+ * The call uploads the plans and resampling tables and synchronises the stream once before launching. */
+#define VDK_AUG_MAX_OPS 8
+#define VDK_AUG_MAX_HOLES 8
+#define VDK_AUG_MAX_KERNEL 9
+enum { VDK_AUG_BRIGHTNESS = 1, VDK_AUG_CONTRAST = 2, VDK_AUG_SATURATION = 3, VDK_AUG_HUE = 4, VDK_AUG_CUTOUT = 5,
+       VDK_AUG_BLUR = 6, VDK_AUG_ROTATE = 7, VDK_AUG_SHARPNESS = 8, VDK_AUG_HFLIP = 9 };
+enum { VDK_AUG_RESIZE_PAD_BILINEAR = 0, VDK_AUG_RESIZE_PAD_NEAREST = 1, VDK_AUG_CROP_RESIZE = 2 };
+typedef struct vdk_aug_op {
+  double matrix[6];                  /* ROTATE: output pixel centre -> input position, as Pillow's Image.rotate builds it */
+  float alpha;                       /* BRIGHTNESS, SATURATION, CONTRAST, SHARPNESS: the blend factor */
+  int kind;                          /* VDK_AUG_* */
+  int hue_shift;                     /* HUE: np.int32(hue_factor * 255).astype(np.uint8) */
+  int n;                             /* CUTOUT: hole count; BLUR: kernel size (odd, <= VDK_AUG_MAX_KERNEL) */
+  float kernel[VDK_AUG_MAX_KERNEL];  /* BLUR: torchvision's fp32 1-D gaussian kernel (the 2-D one is its fp32 outer product) */
+  int box[VDK_AUG_MAX_HOLES][4];     /* CUTOUT: x1, y1, mask_w, mask_h of each hole, pasted in order */
+  int color[VDK_AUG_MAX_HOLES][3];   /* CUTOUT: r, g, b of each hole */
+} vdk_aug_op;
+typedef struct vdk_aug_plan {
+  vdk_aug_op ops[VDK_AUG_MAX_OPS];   /* applied in order at source resolution */
+  int n_ops;
+  int resize;                        /* VDK_AUG_RESIZE_PAD_BILINEAR / _NEAREST / VDK_AUG_CROP_RESIZE */
+  int crop[4];                       /* CROP_RESIZE: left, top, width, height of the box (torchvision's j, i, w, h) */
+} vdk_aug_plan;
+size_t vdk_augment_workspace_bytes(const vdk_image_desc* images, const vdk_aug_plan* plans, int n, int size);
+int vdk_augment_batch(const uint8_t* packed, const vdk_image_desc* images, const vdk_aug_plan* plans, int n, int size,
+                      const float* mean, const float* std_, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_aug_op and vdk_aug_plan, in that order (vdk_struct_sizes' contract for these two). */
+int vdk_augment_struct_sizes(size_t* out, int n);
+
 /* Live kernel timing inside a real step (bench.py's roofline legs; not part of the reference's surface).  Between
  * vdk_prof_begin() and vdk_prof_end() every launch of the categories below is bracketed by two CUDA events on the stream it
  * is launched on; vdk_prof_end synchronises on them and returns, per category, the launch count, the summed event time and

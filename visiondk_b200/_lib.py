@@ -49,6 +49,21 @@ class ImageDesc(C.Structure):
     _fields_ = [("offset", C.c_int64), ("width", C.c_int), ("height", C.c_int)]
 
 
+AUG_MAX_OPS, AUG_MAX_HOLES, AUG_MAX_KERNEL = 8, 8, 9
+AUG_BRIGHTNESS, AUG_CONTRAST, AUG_SATURATION, AUG_HUE, AUG_CUTOUT, AUG_BLUR, AUG_ROTATE, AUG_SHARPNESS, AUG_HFLIP = range(1, 10)
+AUG_RESIZE_PAD_BILINEAR, AUG_RESIZE_PAD_NEAREST, AUG_CROP_RESIZE = 0, 1, 2
+
+
+class AugOp(C.Structure):
+    _fields_ = [("matrix", C.c_double * 6), ("alpha", C.c_float), ("kind", C.c_int), ("hue_shift", C.c_int), ("n", C.c_int),
+                ("kernel", C.c_float * AUG_MAX_KERNEL), ("box", (C.c_int * 4) * AUG_MAX_HOLES),
+                ("color", (C.c_int * 3) * AUG_MAX_HOLES)]
+
+
+class AugPlan(C.Structure):
+    _fields_ = [("ops", AugOp * AUG_MAX_OPS), ("n_ops", C.c_int), ("resize", C.c_int), ("crop", C.c_int * 4)]
+
+
 class ProfTotal(C.Structure):
     _fields_ = [("launches", C.c_longlong), ("ms", C.c_double), ("flops", C.c_double), ("bytes", C.c_double)]
 
@@ -86,6 +101,10 @@ SIGNATURES = {
     "vdk_preprocess_workspace_bytes": (_sz, [C.POINTER(ImageDesc), _i, _i]),
     "vdk_preprocess_resize_pad_normalize": (_i, [_p, C.POINTER(ImageDesc), _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_float), _p, _p,
                                                  _sz, _p]),
+    "vdk_augment_workspace_bytes": (_sz, [C.POINTER(ImageDesc), C.POINTER(AugPlan), _i, _i]),
+    "vdk_augment_batch": (_i, [_p, C.POINTER(ImageDesc), C.POINTER(AugPlan), _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_float), _p,
+                               _p, _sz, _p]),
+    "vdk_augment_struct_sizes": (_i, [_p, _i]),
     "vdk_prof_begin": (_i, []),
     "vdk_prof_end": (_i, [C.POINTER(ProfTotal), _i]),
     "vdk_gemm": (_i, [_p, _p]),

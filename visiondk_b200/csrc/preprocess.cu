@@ -9,7 +9,9 @@
 // intermediate image, 22-bit fixed-point coefficients from a double-precision triangle filter whose support scales with the
 // reduction factor) is restated on the host for the coefficient tables (a few hundred doubles per image) and on the device for
 // the two passes; the float tail is IEEE fp32 division / subtraction exactly as torch evaluates ToTensor and Normalize.
-// HBM-bound: one read of the packed uint8 images, one uint8 intermediate, one fp32 CHW write.
+// HBM-bound: one read of the packed uint8 images, one uint8 intermediate, one fp32 CHW write.  The resampler (resample.h) is
+// shared with the training pipeline (augment.cu), which adds crop boxes and NEAREST tables.
+#include "resample.h"
 #include "vdk_host.h"
 
 #include <cmath>
@@ -19,16 +21,6 @@
 namespace vdk {
 
 constexpr int kPrecisionBits = 32 - 8 - 2;
-
-struct PreImage {          // device-side view of one image's work
-  const uint8_t* src;      // [h][w][3]
-  uint8_t* tmp;            // [h][new_w][3]   horizontal pass output
-  const int* xb;           // [new_w][2] (first input column, tap count)
-  const int* kx;           // [new_w][kmax_x]
-  const int* yb;           // [new_h][2]
-  const int* ky;           // [new_h][kmax_y]
-  int w, h, new_w, new_h, left, top, kmax_x, kmax_y;
-};
 
 // Resample.c precompute_coeffs + normalize_coeffs_8bpc for the bilinear (triangle, support 1) filter
 static int resize_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::vector<int>& kk) {
@@ -66,6 +58,77 @@ static int resize_coeffs(int in_size, int out_size, std::vector<int>& bounds, st
   return kmax;
 }
 
+// Pillow's NEAREST resize (_imaging.c _resize: affine a = in_size / out_size as a float box width over an int, offset 0;
+// Geometry.c ImagingScaleAffine: source index COORD(a * 0.5 + k * a), the position ACCUMULATED in double, one add per output
+// pixel; an index outside the input leaves the fill, 0) as one-tap tables: a tap of weight 1 << kPrecisionBits copies the
+// byte through either pass, no tap gives 0
+static int nearest_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::vector<int>& kk) {
+  const double a = static_cast<double>(static_cast<float>(in_size)) / out_size;
+  bounds.assign(static_cast<size_t>(out_size) * 2, 0);
+  kk.assign(static_cast<size_t>(out_size), 1 << kPrecisionBits);
+  double pos = a * 0.5;
+  for (int xx = 0; xx < out_size; ++xx) {
+    const int xin = pos < 0.0 ? -1 : static_cast<int>(pos);
+    if (xin >= 0 && xin < in_size) {
+      bounds[2 * xx] = xin;
+      bounds[2 * xx + 1] = 1;
+    }
+    pos += a;
+  }
+  return 1;
+}
+
+static int kmax_of(int in_size, int out_size, int filter) {
+  if (filter == kResampleNearest) return 1;
+  const double scale = static_cast<double>(in_size) / static_cast<double>(out_size);
+  const double filterscale = scale > 1.0 ? scale : 1.0;
+  return static_cast<int>(std::ceil(1.0 * filterscale)) * 2 + 1;
+}
+
+void resized_shape(int w, int h, int size, PreLayout* L) {
+  const double scale_factor = static_cast<double>(size) / static_cast<double>(w > h ? w : h);
+  L->new_w = static_cast<int>(w * scale_factor);
+  L->new_h = static_cast<int>(h * scale_factor);
+  // python's floor division for the (possibly zero) non-negative differences
+  L->left = (size - L->new_w) / 2;
+  L->top = (size - L->new_h) / 2;
+}
+
+size_t layout_tables(int w, int h, size_t off, PreLayout* L) {
+  L->kmax_x = kmax_of(w, L->new_w, L->filter);
+  L->kmax_y = kmax_of(h, L->new_h, L->filter);
+  L->xb = off;  off += up256p(static_cast<size_t>(L->new_w) * 2 * sizeof(int));
+  L->kx = off;  off += up256p(static_cast<size_t>(L->new_w) * L->kmax_x * sizeof(int));
+  L->yb = off;  off += up256p(static_cast<size_t>(L->new_h) * 2 * sizeof(int));
+  L->ky = off;  off += up256p(static_cast<size_t>(L->new_h) * L->kmax_y * sizeof(int));
+  return off;
+}
+
+void fill_tables(int w, int h, const PreLayout& L, uint8_t* host_ws) {
+  std::vector<int> bounds, kk;
+  auto coeffs = L.filter == kResampleNearest ? nearest_coeffs : resize_coeffs;
+  coeffs(w, L.new_w, bounds, kk);
+  memcpy(host_ws + L.xb, bounds.data(), bounds.size() * sizeof(int));
+  memcpy(host_ws + L.kx, kk.data(), kk.size() * sizeof(int));
+  coeffs(h, L.new_h, bounds, kk);
+  memcpy(host_ws + L.yb, bounds.data(), bounds.size() * sizeof(int));
+  memcpy(host_ws + L.ky, kk.data(), kk.size() * sizeof(int));
+}
+
+PreImage describe(const PreLayout& L, const uint8_t* src, int stride, int w, int h, uint8_t* ws) {
+  PreImage d;
+  d.src = src;
+  d.stride = stride;
+  d.tmp = ws + L.tmp;
+  d.xb = reinterpret_cast<const int*>(ws + L.xb);
+  d.kx = reinterpret_cast<const int*>(ws + L.kx);
+  d.yb = reinterpret_cast<const int*>(ws + L.yb);
+  d.ky = reinterpret_cast<const int*>(ws + L.ky);
+  d.w = w; d.h = h;
+  d.new_w = L.new_w; d.new_h = L.new_h; d.left = L.left; d.top = L.top; d.kmax_x = L.kmax_x; d.kmax_y = L.kmax_y;
+  return d;
+}
+
 __device__ __forceinline__ uint8_t clip8(int v) { return static_cast<uint8_t>(v < 0 ? 0 : (v > 255 ? 255 : v)); }
 
 // horizontal pass: one thread per (row, output column), 3 channels
@@ -76,7 +139,7 @@ __global__ void __launch_bounds__(256) pre_horizontal_kernel(const PreImage* __r
     const int y = static_cast<int>(i / im.new_w), xx = static_cast<int>(i - static_cast<int64_t>(y) * im.new_w);
     const int xmin = im.xb[2 * xx], n = im.xb[2 * xx + 1];
     const int* k = im.kx + static_cast<size_t>(xx) * im.kmax_x;
-    const uint8_t* s = im.src + (static_cast<size_t>(y) * im.w + xmin) * 3;
+    const uint8_t* s = im.src + (static_cast<size_t>(y) * im.stride + xmin) * 3;
     int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
     for (int x = 0; x < n; ++x) {
       const int c = k[x];
@@ -124,27 +187,15 @@ __global__ void __launch_bounds__(256) pre_vertical_kernel(const PreImage* __res
   }
 }
 
-static size_t up256p(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
-
-struct PreLayout {
-  int new_w, new_h, left, top, kmax_x, kmax_y;
-  size_t tmp, xb, kx, yb, ky;  // offsets in the workspace
-};
-
-// ResizeAndPadding2Square arithmetic (transforms.py:344-357): python float `size / max_side`, int() truncation
-static void resized_shape(int w, int h, int size, PreLayout* L) {
-  const double scale_factor = static_cast<double>(size) / static_cast<double>(w > h ? w : h);
-  L->new_w = static_cast<int>(w * scale_factor);
-  L->new_h = static_cast<int>(h * scale_factor);
-  // python's floor division for the (possibly zero) non-negative differences
-  L->left = (size - L->new_w) / 2;
-  L->top = (size - L->new_h) / 2;
-}
-
-static int kmax_of(int in_size, int out_size) {
-  const double scale = static_cast<double>(in_size) / static_cast<double>(out_size);
-  const double filterscale = scale > 1.0 ? scale : 1.0;
-  return static_cast<int>(std::ceil(1.0 * filterscale)) * 2 + 1;
+int resample_launch(const PreImage* dimg, int n, int64_t max_tmp, int size, const float* mean, const float* std_, float* out,
+                    cudaStream_t s) {
+  const int bx = static_cast<int>(std::min<int64_t>((max_tmp + 255) / 256, 4096));
+  pre_horizontal_kernel<<<dim3(bx, n), 256, 0, s>>>(dimg);
+  VDK_CUDA_OK(cudaGetLastError());
+  const int by = static_cast<int>(std::min<int64_t>((static_cast<int64_t>(size) * size + 255) / 256, 4096));
+  pre_vertical_kernel<<<dim3(by, n), 256, 0, s>>>(dimg, size, mean[0], mean[1], mean[2], std_[0], std_[1], std_[2], out);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
 }
 
 // workspace = [descriptors | coefficient tables of every image | intermediate images]: the first two parts are built on the
@@ -158,12 +209,8 @@ static int plan(const vdk_image_desc* images, int n, int size, std::vector<PreLa
     PreLayout& L = (*layouts)[i];
     resized_shape(w, h, size, &L);
     VDK_REQUIRE(L.new_w > 0 && L.new_h > 0, "vdk_preprocess: image %d (%d x %d) collapses to an empty side at size %d", i, w, h, size);
-    L.kmax_x = kmax_of(w, L.new_w);
-    L.kmax_y = kmax_of(h, L.new_h);
-    L.xb = off;  off += up256p(static_cast<size_t>(L.new_w) * 2 * sizeof(int));
-    L.kx = off;  off += up256p(static_cast<size_t>(L.new_w) * L.kmax_x * sizeof(int));
-    L.yb = off;  off += up256p(static_cast<size_t>(L.new_h) * 2 * sizeof(int));
-    L.ky = off;  off += up256p(static_cast<size_t>(L.new_h) * L.kmax_y * sizeof(int));
+    L.filter = kResampleBilinear;
+    off = layout_tables(w, h, off, &L);
   }
   *tables_end = off;
   for (int i = 0; i < n; ++i) {
@@ -201,37 +248,15 @@ extern "C" int vdk_preprocess_resize_pad_normalize(const uint8_t* packed, const 
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
   std::vector<uint8_t> host(tables_end, 0);  // descriptors + coefficient tables
   PreImage* desc = reinterpret_cast<PreImage*>(host.data());
-  std::vector<int> bounds, kk;
   int64_t max_h = 0;
   for (int i = 0; i < n; ++i) {
     const PreLayout& L = layouts[i];
-    PreImage& d = desc[i];
-    d.src = packed + images[i].offset;
-    d.tmp = ws + L.tmp;
-    d.xb = reinterpret_cast<const int*>(ws + L.xb);
-    d.kx = reinterpret_cast<const int*>(ws + L.kx);
-    d.yb = reinterpret_cast<const int*>(ws + L.yb);
-    d.ky = reinterpret_cast<const int*>(ws + L.ky);
-    d.w = images[i].width; d.h = images[i].height;
-    d.new_w = L.new_w; d.new_h = L.new_h; d.left = L.left; d.top = L.top; d.kmax_x = L.kmax_x; d.kmax_y = L.kmax_y;
-    const int kx = resize_coeffs(d.w, d.new_w, bounds, kk);
-    VDK_REQUIRE(kx == L.kmax_x, "vdk_preprocess: coefficient width mismatch");
-    memcpy(host.data() + L.xb, bounds.data(), bounds.size() * sizeof(int));
-    memcpy(host.data() + L.kx, kk.data(), kk.size() * sizeof(int));
-    const int ky = resize_coeffs(d.h, d.new_h, bounds, kk);
-    VDK_REQUIRE(ky == L.kmax_y, "vdk_preprocess: coefficient height mismatch");
-    memcpy(host.data() + L.yb, bounds.data(), bounds.size() * sizeof(int));
-    memcpy(host.data() + L.ky, kk.data(), kk.size() * sizeof(int));
-    max_h = std::max<int64_t>(max_h, static_cast<int64_t>(d.h) * d.new_w);
+    const int w = images[i].width, h = images[i].height;
+    desc[i] = describe(L, packed + images[i].offset, w, w, h, ws);
+    fill_tables(w, h, L, host.data());
+    max_h = std::max<int64_t>(max_h, static_cast<int64_t>(h) * L.new_w);
   }
   VDK_CUDA_OK(cudaMemcpyAsync(ws, host.data(), tables_end, cudaMemcpyHostToDevice, s));
   VDK_CUDA_OK(cudaStreamSynchronize(s));  // `host` is pageable and goes out of scope: the copy must have left it
-  const PreImage* dimg = reinterpret_cast<const PreImage*>(ws);
-  const int bx = static_cast<int>(std::min<int64_t>((max_h + 255) / 256, 4096));
-  pre_horizontal_kernel<<<dim3(bx, n), 256, 0, s>>>(dimg);
-  VDK_CUDA_OK(cudaGetLastError());
-  const int by = static_cast<int>(std::min<int64_t>((static_cast<int64_t>(size) * size + 255) / 256, 4096));
-  pre_vertical_kernel<<<dim3(by, n), 256, 0, s>>>(dimg, size, mean[0], mean[1], mean[2], std_[0], std_[1], std_[2], out);
-  VDK_CUDA_OK(cudaGetLastError());
-  return VDK_OK;
+  return resample_launch(reinterpret_cast<const PreImage*>(ws), n, max_h, size, mean, std_, out, s);
 }

@@ -40,6 +40,21 @@ class ImagePreprocessor:
         n = len(images)
         if n == 0:
             return torch.empty((0, 3, self.size, self.size), dtype=torch.float32, device=self.device)
+        descs = self._upload(images)
+        with torch.cuda.device(self.device):
+            need = lib.vdk_preprocess_workspace_bytes(descs, n, self.size)
+            if need == 0:
+                raise RuntimeError("vdk_preprocess_workspace_bytes: " + _lib.last_error())
+            ws = self._workspace(need)
+            out = torch.empty((n, 3, self.size, self.size), dtype=torch.float32, device=self.device)
+            _lib.check(lib.vdk_preprocess_resize_pad_normalize(self._dev.data_ptr(), descs, n, self.size, self.mean, self.std,
+                                                               out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                               _lib.stream_ptr()), "vdk_preprocess_resize_pad_normalize")
+        return out
+
+    def _upload(self, images: Sequence[np.ndarray]):
+        """Packs the images into the pinned buffer and queues its copy to the device buffer; returns their descriptors."""
+        n = len(images)
         descs = (_lib.ImageDesc * n)()
         off = 0
         for i, im in enumerate(images):
@@ -60,16 +75,12 @@ class ImagePreprocessor:
             self._dev[:off].copy_(self._pinned[:off], non_blocking=True)
             self._copied = torch.cuda.Event()
             self._copied.record()
-            need = lib.vdk_preprocess_workspace_bytes(descs, n, self.size)
-            if need == 0:
-                raise RuntimeError("vdk_preprocess_workspace_bytes: " + _lib.last_error())
-            if self._ws is None or self._ws.numel() < need:
-                self._ws = torch.empty((need,), dtype=torch.uint8, device=self.device)
-            out = torch.empty((n, 3, self.size, self.size), dtype=torch.float32, device=self.device)
-            _lib.check(lib.vdk_preprocess_resize_pad_normalize(self._dev.data_ptr(), descs, n, self.size, self.mean, self.std,
-                                                               out.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                                                               _lib.stream_ptr()), "vdk_preprocess_resize_pad_normalize")
-        return out
+        return descs
+
+    def _workspace(self, need: int) -> torch.Tensor:
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty((need,), dtype=torch.uint8, device=self.device)
+        return self._ws
 
 
 def resize_pad_normalize(images: Sequence[np.ndarray], size: int = 224, mean: Sequence[float] = IMAGENET_MEAN,
