@@ -4,7 +4,9 @@
 
 read the way the reference reads it (`Image.open(path).convert('RGB')`, cv2 fallback: basedataset.py:234-241) and fed to the
 H100 path: decoded RGB bytes -> visiondk_b200.preprocess (the val transform list on the device, bit-exact with the reference's
-PIL / torchvision pipeline) -> embed -> index -> search.  Decoding stays on host threads (`nw`), one batch ahead of the device.
+PIL / torchvision pipeline) -> embed -> index -> search.  On a CUDA device the baseline JPEGs are decoded there
+(visiondk_b200.jpeg, bit-exact with `read_image`) and every other file with `read_image` on host threads (`nw`) inside the
+same batch, one batch ahead of the consumer; `decode_batches` / `decoded_batches` are the host path.
 
 Only the deterministic eval list of the reference's configs is built — `resize_and_padding(size, training=False)` ->
 `to_tensor` -> `normalize(mean, std)` (configs/faceX/cbir.yaml, data.val.augment); anything else raises with its name.
@@ -45,6 +47,16 @@ def read_image(path: str) -> np.ndarray:
         import cv2
         img = Image.fromarray(cv2.cvtColor(cv2.imread(path), cv2.COLOR_BGR2RGB))
     return np.asarray(img, dtype=np.uint8)
+
+
+def device_decode_batches(files: Sequence[str], batch: int, device, nw: int = 8):
+    """visiondk_b200.jpeg.DecodedBatch per `batch` files: what `decode_batches` yields, already on the device."""
+    from visiondk_b200.jpeg import JpegDecoder, decode_batches as jpeg_batches
+    decoder = JpegDecoder(device, read_image, nw)
+    try:
+        yield from jpeg_batches(files, batch, decoder)
+    finally:
+        decoder.close()
 
 
 def decode_batches(files: Sequence[str], batch: int, nw: int = 8) -> Iterable[List[np.ndarray]]:
@@ -116,7 +128,9 @@ class CBIRFolderData:
         from visiondk_b200.preprocess import ImagePreprocessor
         if self._pre is None:
             self._pre = ImagePreprocessor(self.size, self.mean, self.std, self.device)
-        for images in self.decoded_batches(files):
+        batches = (device_decode_batches(files, self.batch, self.device, self.nw) if self.device.type == "cuda"
+                   else self.decoded_batches(files))
+        for images in batches:
             yield self._pre(images)
 
     def gallery_batches(self, limit: Optional[int] = None) -> Iterable[torch.Tensor]:

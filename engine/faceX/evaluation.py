@@ -57,13 +57,17 @@ class Evaluator:
 
 def image_batches(paths: Sequence[str], augment, batch: int, device, nw: int = 8):
     """(None, device tensors [b, 3, S, S], file paths) per batch — what PredictImageDatasets.collate_fn yields
-    (dataset/basedataset.py:455-458) — with the decode on host threads and the val transform list on the device."""
-    from engine.cbir.folder import decode_batches, parse_val_augment
+    (dataset/basedataset.py:455-458) — with the baseline JPEGs decoded on the device (every other file on host threads)
+    and the val transform list on the device."""
+    from engine.cbir.folder import decode_batches, device_decode_batches, parse_val_augment
     from visiondk_b200.preprocess import ImagePreprocessor
     size, mean, std = parse_val_augment(augment)
     pre = ImagePreprocessor(size, mean, std, device)
     a = 0
-    for images in decode_batches(list(paths), int(batch), nw):
+    device = torch.device(device)
+    batches = (device_decode_batches(list(paths), int(batch), device, nw) if device.type == "cuda"
+               else decode_batches(list(paths), int(batch), nw))
+    for images in batches:
         yield None, pre(images), list(paths[a:a + len(images)])
         a += len(images)
 

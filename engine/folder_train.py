@@ -5,7 +5,8 @@
 with the reference's sampling (DistributedSampler over seed + epoch, padded to a multiple of the world size, rank-strided;
 a drop_last loader) and its epoch schedule of transform lists (engine/vision_engine.py:539-550 of the reference): epochs
 before `warm_ep` and from `aug_epoch` on take the val list (visiondk_b200.preprocess), the epochs between take the train list
-(visiondk_b200.augment).  Decoding stays on `nw` host threads, one batch ahead of the device."""
+(visiondk_b200.augment).  On a CUDA device the baseline JPEGs are decoded there (visiondk_b200.jpeg, bit-exact with
+`read_image`), every other file on `nw` host threads, one batch ahead of the device."""
 from __future__ import annotations
 
 import math
@@ -16,7 +17,7 @@ from typing import Iterable, List, Optional, Sequence
 import numpy as np
 import torch
 
-from engine.cbir.folder import decode_batches, parse_val_augment
+from engine.cbir.folder import decode_batches, device_decode_batches, parse_val_augment
 
 SUFFIXES = (".jpg", ".png")
 
@@ -99,5 +100,7 @@ class FolderTrainData:
         transform = self._transform(epoch)
         files = [self.files[i] for i in idx]
         labels = torch.from_numpy(self.labels[idx])
-        for b, images in enumerate(decode_batches(files, self.batch, self.nw)):
+        batches = (device_decode_batches(files, self.batch, self.device, self.nw) if self.device.type == "cuda"
+                   else decode_batches(files, self.batch, self.nw))
+        for b, images in enumerate(batches):
             yield transform(images), labels[b * self.batch:(b + 1) * self.batch].to(self.device, non_blocking=True)

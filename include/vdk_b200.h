@@ -960,6 +960,66 @@ int vdk_augment_batch(const uint8_t* packed, const vdk_image_desc* images, const
 /* sizeof() of vdk_aug_op and vdk_aug_plan, in that order (vdk_struct_sizes' contract for these two). */
 int vdk_augment_struct_sizes(size_t* out, int n);
 
+/* ---- baseline JPEG decoding (the image-folder input path: `Image.open(path).convert("RGB")`, dataset/basedataset.py:234-241) */
+/* Decodes, for a BATCH of compressed files, the baseline JPEGs that libjpeg-turbo (as Pillow calls it: JDCT_ISLOW, fancy
+ * upsampling, no draft mode) decodes, bit for bit: one SOF0/SOF1 frame of 8-bit samples, one interleaved Huffman scan over
+ * all components, 1 component (Y replicated into R, G, B) or 3 components in YCbCr (JFIF, Adobe transform 1, or neither
+ * marker and component ids other than 'R','G','B'), sampling 4:4:4, 4:2:2 (h2v1), 4:2:0 (h2v2) or 4:4:0 (h1v2), any restart
+ * interval.  Everything else gets a fallback reason and is left to the host decoder (oracle/jpeg.py restates the arithmetic).
+ *
+ * 1. vdk_jpeg_parse (host only, no GPU): reads the headers of n files at packed + descs[i].data_offset (descs[i].data_bytes
+ *    long) and fills the rest of each descriptor; descs[i].reason is VDK_JPEG_DEVICE or the fallback reason.  It also writes
+ *    where each restart interval of the VDK_JPEG_DEVICE images starts (bytes from the file's start) into segs: image i's
+ *    n_segments entries from segs[descs[i].seg_first], images one after the other.  Entries past seg_capacity are not
+ *    written: when the last device image's seg_first + n_segments exceeds it, call again with a larger array.  Returns
+ *    VDK_OK (a file the device does not take is not an error).
+ * 2. the caller sets descs[i].out_offset (256-byte aligned) for every VDK_JPEG_DEVICE image: where its packed
+ *    [height][width][3] RGB goes in `out` (the vdk_image_desc layout).
+ * 3. vdk_jpeg_workspace_bytes (host only): lays the device images out in the workspace — writes their ws_* and *_cta_base
+ *    fields and returns the bytes needed (2 bytes per coefficient + 1 per decoded sample), 0 on bad input.
+ * 4. the caller copies the descriptors and the restart-interval table to the device (`descs_dev`, `segs_dev`, same bytes) and
+ *    calls vdk_jpeg_decode with the same host descriptors: three kernels on `stream` (Huffman decode into int16
+ *    coefficients, dequantise + islow IDCT into component planes, upsampling + YCbCr->RGB into `out`).  status[i] (DEVICE
+ *    int32, n entries) is 0 when image i was decoded, or an OR of VDK_JPEG_BAD_* when its stream is not well formed (then
+ *    `out` holds no valid pixels for it and the host decodes it); images that are not VDK_JPEG_DEVICE get
+ *    VDK_JPEG_BAD_SKIPPED.  No allocation, no synchronisation.  `data` is the DEVICE copy of the packed files (same offsets
+ *    as at parse time). */
+enum { VDK_JPEG_DEVICE = 0, VDK_JPEG_NOT_JPEG = 1, VDK_JPEG_PROCESS = 2, VDK_JPEG_PRECISION = 3, VDK_JPEG_COLOR = 4,
+       VDK_JPEG_SAMPLING = 5, VDK_JPEG_SCAN = 6, VDK_JPEG_MALFORMED = 7, VDK_JPEG_MPO = 8, VDK_JPEG_RESTART = 9,
+       VDK_JPEG_TOO_LARGE = 10 /* a side above libjpeg's 65500, or more pixels than PIL.Image.MAX_IMAGE_PIXELS */ };
+enum { VDK_JPEG_BAD_CODE = 1,      /* no Huffman code matches the next 16 bits */
+       VDK_JPEG_BAD_AC_RUN = 2,    /* an AC run past coefficient 63 */
+       VDK_JPEG_BAD_SHORT = 4,     /* a marker or the end of the scan before the last MCU of a restart interval */
+       VDK_JPEG_BAD_EXTRA = 8,     /* whole bytes left over before a marker */
+       VDK_JPEG_BAD_SKIPPED = 16 };
+typedef struct vdk_jpeg_huff {
+  uint16_t lut[512];      /* next 9 bits -> (code length << 8) | symbol; 0 when the code is longer than 9 bits */
+  int32_t maxcode[18];    /* largest code of each length (-1: none); maxcode[17] is a sentinel above every 16-bit code */
+  int32_t valoffset[17];  /* symbol of a code of length l = huffval[code + valoffset[l]] */
+  uint8_t huffval[256];
+} vdk_jpeg_huff;
+typedef struct vdk_jpeg_desc {
+  int64_t data_offset, data_bytes;  /* in: the file within the packed buffer */
+  int64_t out_offset;               /* in (after parse): the RGB image within `out` */
+  int64_t scan_begin, scan_end;     /* entropy-coded bytes [begin, end) from data_offset; scan_end is the EOI marker */
+  int64_t seg_first;                /* set by vdk_jpeg_parse: the image's first entry in the restart-interval table */
+  int64_t ws_coef, ws_plane;        /* set by vdk_jpeg_workspace_bytes: workspace byte offsets */
+  int64_t idct_cta_base, color_cta_base;      /* set by vdk_jpeg_workspace_bytes: first CTA of the image in the grids */
+  int width, height, ncomp, reason;
+  int restart_interval;             /* MCUs per restart interval, 0 = none */
+  int n_segments;                   /* restart intervals in the scan (1 without DRI) */
+  int mcus_x, mcus_y, hmax, vmax;
+  int h[3], v[3];                   /* sampling factors (1 x 1 for a single component) */
+  int16_t quant[3][64];             /* natural order, cast to 16 bits like libjpeg's ISLOW_MULT_TYPE */
+  vdk_jpeg_huff dc[3], ac[3];       /* per component */
+} vdk_jpeg_desc;
+int vdk_jpeg_parse(const uint8_t* packed, vdk_jpeg_desc* descs, int n, int64_t* segs, int64_t seg_capacity);
+size_t vdk_jpeg_workspace_bytes(vdk_jpeg_desc* descs, int n);
+int vdk_jpeg_decode(const uint8_t* data, const vdk_jpeg_desc* descs, const vdk_jpeg_desc* descs_dev, const int64_t* segs_dev,
+                    int n, uint8_t* out, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_jpeg_huff and vdk_jpeg_desc, in that order. */
+int vdk_jpeg_struct_sizes(size_t* out, int n);
+
 /* Live kernel timing inside a real step (bench.py's roofline legs; not part of the reference's surface).  Between
  * vdk_prof_begin() and vdk_prof_end() every launch of the categories below is bracketed by two CUDA events on the stream it
  * is launched on; vdk_prof_end synchronises on them and returns, per category, the launch count, the summed event time and

@@ -64,6 +64,24 @@ class AugPlan(C.Structure):
     _fields_ = [("ops", AugOp * AUG_MAX_OPS), ("n_ops", C.c_int), ("resize", C.c_int), ("crop", C.c_int * 4)]
 
 
+JPEG_DEVICE, JPEG_NOT_JPEG, JPEG_PROCESS, JPEG_PRECISION, JPEG_COLOR, JPEG_SAMPLING, JPEG_SCAN, JPEG_MALFORMED, JPEG_MPO, \
+    JPEG_RESTART, JPEG_TOO_LARGE = range(11)
+JPEG_BAD_CODE, JPEG_BAD_AC_RUN, JPEG_BAD_SHORT, JPEG_BAD_EXTRA, JPEG_BAD_SKIPPED = 1, 2, 4, 8, 16
+
+
+class JpegHuff(C.Structure):
+    _fields_ = [("lut", C.c_uint16 * 512), ("maxcode", C.c_int32 * 18), ("valoffset", C.c_int32 * 17), ("huffval", C.c_uint8 * 256)]
+
+
+class JpegDesc(C.Structure):
+    _fields_ = [("data_offset", C.c_int64), ("data_bytes", C.c_int64), ("out_offset", C.c_int64), ("scan_begin", C.c_int64),
+                ("scan_end", C.c_int64), ("seg_first", C.c_int64), ("ws_coef", C.c_int64), ("ws_plane", C.c_int64),
+                ("idct_cta_base", C.c_int64), ("color_cta_base", C.c_int64), ("width", C.c_int), ("height", C.c_int),
+                ("ncomp", C.c_int), ("reason", C.c_int), ("restart_interval", C.c_int), ("n_segments", C.c_int),
+                ("mcus_x", C.c_int), ("mcus_y", C.c_int), ("hmax", C.c_int), ("vmax", C.c_int), ("h", C.c_int * 3),
+                ("v", C.c_int * 3), ("quant", (C.c_int16 * 64) * 3), ("dc", JpegHuff * 3), ("ac", JpegHuff * 3)]
+
+
 class ProfTotal(C.Structure):
     _fields_ = [("launches", C.c_longlong), ("ms", C.c_double), ("flops", C.c_double), ("bytes", C.c_double)]
 
@@ -105,6 +123,10 @@ SIGNATURES = {
     "vdk_augment_batch": (_i, [_p, C.POINTER(ImageDesc), C.POINTER(AugPlan), _i, _i, C.POINTER(C.c_float), C.POINTER(C.c_float), _p,
                                _p, _sz, _p]),
     "vdk_augment_struct_sizes": (_i, [_p, _i]),
+    "vdk_jpeg_parse": (_i, [_p, C.POINTER(JpegDesc), _i, _p, _i64]),
+    "vdk_jpeg_workspace_bytes": (_sz, [C.POINTER(JpegDesc), _i]),
+    "vdk_jpeg_decode": (_i, [_p, C.POINTER(JpegDesc), _p, _p, _i, _p, _p, _p, _sz, _p]),
+    "vdk_jpeg_struct_sizes": (_i, [_p, _i]),
     "vdk_prof_begin": (_i, []),
     "vdk_prof_end": (_i, [C.POINTER(ProfTotal), _i]),
     "vdk_gemm": (_i, [_p, _p]),

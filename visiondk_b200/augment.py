@@ -21,6 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .jpeg import DecodedBatch
 from .preprocess import IMAGENET_MEAN, IMAGENET_STD, ImagePreprocessor
 
 PIXEL_OPS = ("random_color_jitter", "random_cutout", "random_gaussianblur", "random_rotate", "random_adjustsharpness",
@@ -311,9 +312,10 @@ class TrainAugmenter(ImagePreprocessor):
         super().__init__(spec.size, spec.mean, spec.std, device)
         self.spec = spec
 
-    def plans(self, images: Sequence[np.ndarray], py: _random.Random, nprs: np.random.RandomState,
+    def plans(self, images: Sequence[np.ndarray] | DecodedBatch, py: _random.Random, nprs: np.random.RandomState,
               g: torch.Generator) -> List[ImagePlan]:
-        return [sample_plan(self.spec, im.shape[1], im.shape[0], py, nprs, g) for im in images]
+        shapes = images.shapes if isinstance(images, DecodedBatch) else [im.shape for im in images]
+        return [sample_plan(self.spec, s[1], s[0], py, nprs, g) for s in shapes]
 
     def __call__(self, images: Sequence[np.ndarray], py: _random.Random, nprs: np.random.RandomState,
                  g: torch.Generator) -> torch.Tensor:
@@ -325,13 +327,13 @@ class TrainAugmenter(ImagePreprocessor):
         if n == 0:
             return torch.empty((0, 3, self.size, self.size), dtype=torch.float32, device=self.device)
         recs = pack_plans(plans)
-        descs = self._upload(images)
+        packed, descs = self._stage(images)
         with torch.cuda.device(self.device):
             need = lib.vdk_augment_workspace_bytes(descs, recs, n, self.size)
             if need == 0:
                 raise RuntimeError("vdk_augment_workspace_bytes: " + _lib.last_error())
             ws = self._workspace(need)
             out = torch.empty((n, 3, self.size, self.size), dtype=torch.float32, device=self.device)
-            _lib.check(lib.vdk_augment_batch(self._dev.data_ptr(), descs, recs, n, self.size, self.mean, self.std, out.data_ptr(),
+            _lib.check(lib.vdk_augment_batch(packed, descs, recs, n, self.size, self.mean, self.std, out.data_ptr(),
                                              ws.data_ptr(), ws.numel(), _lib.stream_ptr()), "vdk_augment_batch")
         return out

@@ -4,7 +4,8 @@ configs/faceX/cbir.yaml val.augment) — for a batch of decoded RGB images of di
 
     batch = resize_pad_normalize([np.uint8 [h, w, 3], ...], size=224, device="cuda")      # fp32 [n, 3, size, size]
 
-Decoding (PIL / cv2) stays on the host; the decoded bytes are packed into one pinned buffer, cross PCIe once, and the two
+Decoded images come either from the host (PIL / cv2; the decoded bytes are packed into one pinned buffer and cross PCIe once) or
+already on the device (visiondk_b200.jpeg.DecodedBatch); the two
 resampling passes + padding + ToTensor + Normalize run in csrc/preprocess.cu — bit-exact with Pillow's 8-bit BILINEAR resize and
 torch's fp32 arithmetic (tests/test_preprocess_gpu.py).  No CPU fallback."""
 from __future__ import annotations
@@ -16,6 +17,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .jpeg import DecodedBatch
 
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
 
@@ -35,22 +37,30 @@ class ImagePreprocessor:
         self._ws = None
         self._copied = None  # event after the last host->device copy out of the pinned buffer
 
-    def __call__(self, images: Sequence[np.ndarray]) -> torch.Tensor:
+    def __call__(self, images: Sequence[np.ndarray] | DecodedBatch) -> torch.Tensor:
+        """`images`: decoded RGB arrays on the host, or a DecodedBatch already on the device."""
         lib = _lib.load()
         n = len(images)
         if n == 0:
             return torch.empty((0, 3, self.size, self.size), dtype=torch.float32, device=self.device)
-        descs = self._upload(images)
+        packed, descs = self._stage(images)
         with torch.cuda.device(self.device):
             need = lib.vdk_preprocess_workspace_bytes(descs, n, self.size)
             if need == 0:
                 raise RuntimeError("vdk_preprocess_workspace_bytes: " + _lib.last_error())
             ws = self._workspace(need)
             out = torch.empty((n, 3, self.size, self.size), dtype=torch.float32, device=self.device)
-            _lib.check(lib.vdk_preprocess_resize_pad_normalize(self._dev.data_ptr(), descs, n, self.size, self.mean, self.std,
+            _lib.check(lib.vdk_preprocess_resize_pad_normalize(packed, descs, n, self.size, self.mean, self.std,
                                                                out.data_ptr(), ws.data_ptr(), ws.numel(),
                                                                _lib.stream_ptr()), "vdk_preprocess_resize_pad_normalize")
         return out
+
+    def _stage(self, images):
+        """(device pointer of the packed RGB images, their descriptors): a DecodedBatch as it is, host arrays uploaded."""
+        if isinstance(images, DecodedBatch):
+            return images.data.data_ptr(), images.descs
+        descs = self._upload(images)
+        return self._dev.data_ptr(), descs
 
     def _upload(self, images: Sequence[np.ndarray]):
         """Packs the images into the pinned buffer and queues its copy to the device buffer; returns their descriptors."""
