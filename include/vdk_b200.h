@@ -615,6 +615,8 @@ int vdk_convnext_train_backward_range(const vdk_convnext_net* net, const vdk_con
  *   vdk_dwconv7             mode 0: LayerNorm_C(dwconv7(x)+bias) (rstd_out optional); mode 1: dwconv7(x) with `w49` (+addend)
  *                           — with reversed taps this is the depthwise backward-data pass
  *   vdk_dwconv7_wgrad       dw49[tap][c] += sum dconv * shifted x; dbias[c] += sum dconv (C a multiple of 8)
+ *   vdk_dwconv7_bwd         both from one pass over dconv: dx = bf16(dwconv7(dconv) with `w49` (+addend)), and the
+ *                           vdk_dwconv7_wgrad accumulation into dw49 / dbias (the training step's depthwise backward)
  *   vdk_layernorm_bwd       LayerNorm backward from the saved OUTPUT y and 1/sigma (patch = 2: through the 2x2 regrouping;
  *                           C a multiple of 8, <= 1536).  xhat = (y - beta) / gamma carries ulp(y) / (2 |gamma|) of error,
  *                           |beta / gamma| / |xhat| times bf16 precision; gamma = 0 takes xhat = 0 (that dgamma gets nothing)
@@ -623,6 +625,8 @@ int vdk_dwconv7(int mode, const void* x, int batch, int H, int W, int C, const f
                 const float* ln_w, const float* ln_b, float eps, void* y, float* rstd_out, const void* addend, void* stream);
 int vdk_dwconv7_wgrad(const void* x, const void* dconv, int batch, int H, int W, int C, float* dw49, float* dbias,
                       void* stream);
+int vdk_dwconv7_bwd(const void* x, const void* dconv, int batch, int H, int W, int C, const float* w49, const void* addend,
+                    void* dx, float* dw49, float* dbias, void* stream);
 int vdk_layernorm_bwd(const void* dy, const void* y, const float* rstd, int batch, int H, int W, int C, const float* ln_w,
                       const float* ln_b, int patch, void* dx, const void* addend, float* dgamma, float* dbeta, void* stream);
 int vdk_batchnorm_train_fwd(const void* x, int rows, int C, int is_bf16, const float* weight, const float* bias, float eps,

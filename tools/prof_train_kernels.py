@@ -92,6 +92,10 @@ kernels = {
                                                             x.data_ptr(), sp), "dw1"), 2.0 * M * Cn * 49, 6.0 * M * Cn, None),
     "dwconv7 wgrad": (lambda: _lib.check(lib.vdk_dwconv7_wgrad(x.data_ptr(), dy.data_ptr(), B, H, H, Cn, dw49.data_ptr(), dbias.data_ptr(), sp),
                                          "dww"), 2.0 * M * Cn * 49, 4.0 * M * Cn, None),
+    # the train step's depthwise backward: both of the above from one pass over the gradient
+    "dwconv7 bwd (data + wgrad)": (lambda: _lib.check(lib.vdk_dwconv7_bwd(x.data_ptr(), dy.data_ptr(), B, H, H, Cn, w49.data_ptr(),
+                                                                          x.data_ptr(), y.data_ptr(), dw49.data_ptr(), dbias.data_ptr(),
+                                                                          sp), "dwb"), 4.0 * M * Cn * 49, 8.0 * M * Cn, None),
     "ln_bwd": (lambda: _lib.check(lib.vdk_layernorm_bwd(dy.data_ptr(), x.data_ptr(), rstd.data_ptr(), B, H, H, Cn, ln_w.data_ptr(),
                                                         ln_b.data_ptr(), 1, y.data_ptr(), 0, dgamma.data_ptr(), dbeta.data_ptr(), sp), "lnb"),
                0.0, 6.0 * M * Cn, None),

@@ -167,6 +167,7 @@ SIGNATURES = {
     "vdk_layernorm_patchify": (_i, [_p, _i, _i, _i, _i, _p, _p, C.c_float, _i, _p, _p]),
     "vdk_dwconv7": (_i, [_i, _p, _i, _i, _i, _i, _p, _p, _p, _p, C.c_float, _p, _p, _p, _p]),
     "vdk_dwconv7_wgrad": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _p]),
+    "vdk_dwconv7_bwd": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
     "vdk_layernorm_bwd": (_i, [_p, _p, _p, _i, _i, _i, _i, _p, _p, _i, _p, _p, _p, _p, _p]),
     "vdk_batchnorm_train_fwd": (_i, [_p, _i, _i, _i, _p, _p, C.c_float, C.c_float, _p, _p, _p, _p, _p, _p]),
     "vdk_batchnorm_train_bwd": (_i, [_p, _p, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p]),

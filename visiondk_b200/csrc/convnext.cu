@@ -66,18 +66,15 @@ int launch_stem_patchify(const float* images, int B, int S, __nv_bfloat16* out, 
 // checks.  A "group" of C/4 threads (4 contiguous channels each: conflict-free 8-byte LDS, coalesced 8-byte STG)
 // owns one output row of the tile at a time; the 49 taps of a thread's 4 channels are read one filter row at a
 // time (L1-resident), accumulators stay in registers, and LayerNorm over C is a reduction inside the group.
-// FMA-bound: 49 FMAs per output against 2 + 2 bytes of HBM traffic.
-// MODE 0: y = LayerNorm_C(conv + bias) (forward; optionally saves 1/sigma per pixel for the backward)
-// MODE 1: y = conv (+ addend)           (backward-data: the same correlation with the taps reversed, plus the
-//                                        gradient arriving through the residual connection)
-template <int TW, int MODE>
+// FMA-bound: 49 FMAs per output against 2 + 2 bytes of HBM traffic.  y = LayerNorm_C(conv + bias), optionally saving
+// 1/sigma per pixel for the backward (the backward-data pass is dwconv7_bwd_kernel, train_ops.cu).
+template <int TW>
 __global__ void __launch_bounds__(512)
 dwconv7_ln_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W, int C, int TH, int box_c,
                   int tpg /*threads per group, whole warps*/,
                   const float* __restrict__ w49,  // [49][C]
                   const float* __restrict__ bias, const float* __restrict__ ln_w, const float* __restrict__ ln_b,
-                  float eps, __nv_bfloat16* __restrict__ y, float* __restrict__ rstd_out,
-                  const __nv_bfloat16* __restrict__ addend) {
+                  float eps, __nv_bfloat16* __restrict__ y, float* __restrict__ rstd_out) {
   extern __shared__ uint8_t dw_smem_raw[];
   // aligned without a pointer->integer->pointer round trip, so the tile reads below stay LDS (not generic LD)
   uint8_t* smem = dw_smem_raw + ((128u - (smem_u32(dw_smem_raw) & 127u)) & 127u);
@@ -114,7 +111,7 @@ dwconv7_ln_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W
   }
   // weights / affine parameters of this thread's channels while the tile is in flight
   float4 bc = make_float4(0.f, 0.f, 0.f, 0.f), g4 = bc, b4 = bc;
-  if (has_c && MODE == 0) {
+  if (has_c) {
     bc = __ldg(reinterpret_cast<const float4*>(bias + c0));
     g4 = __ldg(reinterpret_cast<const float4*>(ln_w + c0));
     b4 = __ldg(reinterpret_cast<const float4*>(ln_b + c0));
@@ -157,29 +154,6 @@ dwconv7_ln_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W
           }
         }
       }
-    }
-    if (MODE == 1) {
-      if (active) {
-#pragma unroll
-        for (int p = 0; p < TW; ++p) {
-          const int ox = ox0 + p;
-          if (ox >= W) continue;
-          const int64_t off = ((static_cast<int64_t>(b) * H + oy0 + oyl) * W + ox) * C + c0;
-          float o0 = acc[p][0], o1 = acc[p][1], o2 = acc[p][2], o3 = acc[p][3];
-          if (addend) {
-            const uint2 t = *reinterpret_cast<const uint2*>(addend + off);
-            const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.x));
-            const float2 c = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.y));
-            o0 += a.x; o1 += a.y; o2 += c.x; o3 += c.y;
-          }
-          __nv_bfloat162 lo = __floats2bfloat162_rn(o0, o1), hi = __floats2bfloat162_rn(o2, o3);
-          uint2 t;
-          t.x = *reinterpret_cast<uint32_t*>(&lo);
-          t.y = *reinterpret_cast<uint32_t*>(&hi);
-          *reinterpret_cast<uint2*>(y + off) = t;
-        }
-      }
-      continue;
     }
     // LayerNorm over C for the TW pixels of this row: mean, then centred second moment, reduced in the group
     float mean[TW], rstd[TW];
@@ -249,7 +223,7 @@ dwconv7_ln_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W
 // chunks of a pixel: the C / chunk CTAs of a tile form a thread-block CLUSTER, each publishes (mean, centred sum of
 // squares) of its channels per pixel in shared memory, and every CTA combines the partials of its peers through
 // distributed shared memory (Chan's parallel-variance update: same two-pass numerics as the reference LayerNorm,
-// one cluster barrier).  MODE as above.
+// one cluster barrier).
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 __device__ __forceinline__ float2 ld_dsmem_f2(const void* local_smem, uint32_t rank) {
@@ -262,12 +236,11 @@ __device__ __forceinline__ float2 ld_dsmem_f2(const void* local_smem, uint32_t r
 
 constexpr int kDwTW = 7;
 
-template <int MODE, int CHUNK>
+template <int CHUNK>
 __global__ void __launch_bounds__(224, 3)
 dwconv7_chunk_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W, int C, int TH, int nchunks,
                      const float* __restrict__ w49, const float* __restrict__ bias, const float* __restrict__ ln_w,
-                     const float* __restrict__ ln_b, float eps, __nv_bfloat16* __restrict__ y, float* __restrict__ rstd_out,
-                     const __nv_bfloat16* __restrict__ addend) {
+                     const float* __restrict__ ln_b, float eps, __nv_bfloat16* __restrict__ y, float* __restrict__ rstd_out) {
   extern __shared__ uint8_t dwc_smem_raw[];
   uint8_t* smem = dwc_smem_raw + ((128u - (smem_u32(dwc_smem_raw) & 127u)) & 127u);
   constexpr int box_w = kDwTW + 6;
@@ -300,7 +273,7 @@ dwconv7_chunk_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, in
     tma_load_4d(smem, &map_x, bar, ck * chunk, ox0 - 3, oy0 - 3, b);
   }
   float4 bc = make_float4(0.f, 0.f, 0.f, 0.f), g4 = bc, b4 = bc;
-  if (has_c && MODE == 0) {
+  if (has_c) {
     bc = __ldg(reinterpret_cast<const float4*>(bias + c0));
     g4 = __ldg(reinterpret_cast<const float4*>(ln_w + c0));
     b4 = __ldg(reinterpret_cast<const float4*>(ln_b + c0));
@@ -349,29 +322,6 @@ dwconv7_chunk_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, in
         }
       }
     }
-  }
-  if (MODE == 1) {
-    if (active) {
-#pragma unroll
-      for (int p = 0; p < kDwTW; ++p) {
-        const int ox = ox0 + p;
-        if (ox >= W) continue;
-        const int64_t off = ((static_cast<int64_t>(b) * H + oy0 + warp) * W + ox) * C + c0;
-        float o0 = acc[p][0].x, o1 = acc[p][0].y, o2 = acc[p][1].x, o3 = acc[p][1].y;
-        if (addend) {
-          const uint2 t = __ldg(reinterpret_cast<const uint2*>(addend + off));
-          const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.x));
-          const float2 c = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.y));
-          o0 += a.x; o1 += a.y; o2 += c.x; o3 += c.y;
-        }
-        __nv_bfloat162 lo = __floats2bfloat162_rn(o0, o1), hi = __floats2bfloat162_rn(o2, o3);
-        uint2 t;
-        t.x = *reinterpret_cast<uint32_t*>(&lo);
-        t.y = *reinterpret_cast<uint32_t*>(&hi);
-        *reinterpret_cast<uint2*>(y + off) = t;
-      }
-    }
-    return;
   }
   // ---- LayerNorm over C: local two-pass statistics of this chunk, then the cluster-wide combination ----
   float mean[kDwTW], rstd[kDwTW];
@@ -446,12 +396,11 @@ dwconv7_chunk_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, in
 // (one output row each) run the tap loop of tile i+1 while the LayerNorm statistics of tile i cross the cluster
 // (split-phase barrier.cluster: arrive after publishing the chunk's (mean, M2), wait only after the next tile's taps).
 // LayerNorm numerics are unchanged: two-pass statistics per chunk, Chan's combination across the chunks of a pixel.
-template <int MODE, int CHUNK, int TH>
+template <int CHUNK, int TH>
 __global__ void __launch_bounds__((TH + 1) * 32, TH == 7 ? 2 : 1)
 dwconv7_pipe_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int W, int C, int nchunks, int n_tiles,
                     const float* __restrict__ w49, const float* __restrict__ bias, const float* __restrict__ ln_w,
-                    const float* __restrict__ ln_b, float eps, __nv_bfloat16* __restrict__ y, float* __restrict__ rstd_out,
-                    const __nv_bfloat16* __restrict__ addend) {
+                    const float* __restrict__ ln_b, float eps, __nv_bfloat16* __restrict__ y, float* __restrict__ rstd_out) {
   extern __shared__ uint8_t dwp_smem_raw[];
   uint8_t* smem = dwp_smem_raw + ((128u - (smem_u32(dwp_smem_raw) & 127u)) & 127u);
   constexpr int box_w = kDwTW + 6, box_h = TH + 6;
@@ -463,11 +412,11 @@ dwconv7_pipe_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int
   uint64_t* empty_bar = full_bar + 2;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ck = blockIdx.x % nchunks;  // == rank inside the cluster (MODE 0, nchunks > 1)
+  const int ck = blockIdx.x % nchunks;  // == rank inside the cluster (nchunks > 1)
   const int group = blockIdx.x / nchunks, n_groups = gridDim.x / nchunks;
   const int tiles_w = (W + kDwTW - 1) / kDwTW, tiles_h = (H + TH - 1) / TH;
   const int n_my = group < n_tiles ? (n_tiles - group + n_groups - 1) / n_groups : 0;
-  const bool clustered = MODE == 0 && nchunks > 1;
+  const bool clustered = nchunks > 1;
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&map_x);
@@ -529,7 +478,7 @@ dwconv7_pipe_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int
   const bool has_c = cl < CHUNK;
   const int c0 = ck * CHUNK + cl;
   float4 bc = make_float4(0.f, 0.f, 0.f, 0.f), g4 = bc, b4 = bc;
-  if (has_c && MODE == 0) {
+  if (has_c) {
     bc = __ldg(reinterpret_cast<const float4*>(bias + c0));
     g4 = __ldg(reinterpret_cast<const float4*>(ln_w + c0));
     b4 = __ldg(reinterpret_cast<const float4*>(ln_b + c0));
@@ -573,42 +522,7 @@ dwconv7_pipe_kernel(const __grid_constant__ CUtensorMap map_x, int B, int H, int
     }
   };
 
-  if (MODE == 1) {
-    for (int it = 0; it < n_my; ++it) {
-      const int buf = it & 1;
-      int b, oy0, ox0;
-      tile_coords(it, b, oy0, ox0);
-      const bool active = has_c && oy0 + warp < H;
-      float2 acc[kDwTW][2];
-      mbar_wait(&full_bar[buf], (it >> 1) & 1);
-      if (active) conv_row(smem + buf * tile_stride, acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[buf]);
-      if (active) {
-#pragma unroll
-        for (int p = 0; p < kDwTW; ++p) {
-          const int ox = ox0 + p;
-          if (ox >= W) continue;
-          const int64_t off = ((static_cast<int64_t>(b) * H + oy0 + warp) * W + ox) * C + c0;
-          float o0 = acc[p][0].x, o1 = acc[p][0].y, o2 = acc[p][1].x, o3 = acc[p][1].y;
-          if (addend) {
-            const uint2 t = __ldg(reinterpret_cast<const uint2*>(addend + off));
-            const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.x));
-            const float2 c = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.y));
-            o0 += a.x; o1 += a.y; o2 += c.x; o3 += c.y;
-          }
-          __nv_bfloat162 lo = __floats2bfloat162_rn(o0, o1), hi = __floats2bfloat162_rn(o2, o3);
-          uint2 t;
-          t.x = *reinterpret_cast<uint32_t*>(&lo);
-          t.y = *reinterpret_cast<uint32_t*>(&hi);
-          *reinterpret_cast<uint2*>(y + off) = t;
-        }
-      }
-    }
-    return;
-  }
-
-  // ---- MODE 0: conv + bias + LayerNorm over C, statistics exchanged across the cluster one tile behind the tap loop ----
+  // ---- conv + bias + LayerNorm over C, statistics exchanged across the cluster one tile behind the tap loop ----
   float2 acc[kDwTW][2];     // tile whose LayerNorm is pending
   float mean[kDwTW], m2[kDwTW];
   int pb = 0, poy0 = 0, pox0 = 0;
@@ -891,28 +805,28 @@ static int check_net(const vdk_convnext_net* n) {
 
 using namespace vdk;
 
-template <int TW, int MODE>
+template <int TW>
 static int launch_dwconv_tw(const CUtensorMap& mx, int batch, int H, int W, int C, int TH, int box_c, const float* w49,
                             const float* bias, const float* ln_w, const float* ln_b, float eps, __nv_bfloat16* y,
-                            float* rstd_out, const __nv_bfloat16* addend, cudaStream_t s) {
+                            float* rstd_out, cudaStream_t s) {
   const int tpg = ((C / 4) + 31) / 32 * 32;
   const int groups = std::max(1, std::min(512 / tpg, TH));
   const int n_chunks = C / box_c;
   const int smem = n_chunks * (((TH + 6) * (TW + 6) * box_c * 2 + 127) & ~127) + 16 * TW * 16 * 4 + 16 + 128;
-  auto kern = dwconv7_ln_kernel<TW, MODE>;
+  auto kern = dwconv7_ln_kernel<TW>;
   VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   const unsigned grid = static_cast<unsigned>(batch) * ((H + TH - 1) / TH) * ((W + TW - 1) / TW);
-  kern<<<grid, groups * tpg, smem, s>>>(mx, batch, H, W, C, TH, box_c, tpg, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend);
+  kern<<<grid, groups * tpg, smem, s>>>(mx, batch, H, W, C, TH, box_c, tpg, w49, bias, ln_w, ln_b, eps, y, rstd_out);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }
 
 
 // Persistent launch: one CTA per SM (two for the 7-row tile), grid = co-resident clusters x chunks.
-template <int MODE, int CHUNK, int TH>
+template <int CHUNK, int TH>
 static int launch_dwconv7_pipe_t(const __nv_bfloat16* x, int batch, int H, int W, int C, const float* w49, const float* bias,
                                  const float* ln_w, const float* ln_b, float eps, __nv_bfloat16* y, float* rstd_out,
-                                 const __nv_bfloat16* addend, cudaStream_t s) {
+                                 cudaStream_t s) {
   const int nchunks = C / CHUNK;
   constexpr int tile_stride = ((TH + 6) * (kDwTW + 6) * CHUNK * 2 + 127) & ~127;
   constexpr int smem = 2 * tile_stride + 49 * CHUNK * 4 + 2 * TH * 8 * 8 + 4 * 8 + 128;
@@ -920,8 +834,8 @@ static int launch_dwconv7_pipe_t(const __nv_bfloat16* x, int batch, int H, int W
   CUtensorMap mx;
   int rc = make_tma_nhwc_16bit(&mx, x, batch, H, W, C, TH + 6, kDwTW + 6, CHUNK);
   if (rc != VDK_OK) return rc;
-  auto kern = dwconv7_pipe_kernel<MODE, CHUNK, TH>;
-  const int cluster = (MODE == 0) ? nchunks : 1;
+  auto kern = dwconv7_pipe_kernel<CHUNK, TH>;
+  const int cluster = nchunks;
   struct Fit { int clusters; };
   static Fit fit[17] = {};  // per cluster size: co-resident clusters of this instantiation (queried once)
   cudaLaunchConfig_t cfg{};
@@ -951,41 +865,32 @@ static int launch_dwconv7_pipe_t(const __nv_bfloat16* x, int batch, int H, int W
   const int n_tiles = batch * ((H + TH - 1) / TH) * ((W + kDwTW - 1) / kDwTW);
   const int groups = std::min(n_tiles, fit[cluster].clusters);
   cfg.gridDim = dim3(static_cast<unsigned>(groups) * nchunks);
-  if (MODE == 1) {
-    // no cluster: any CTA is a "group member"; spread tiles x chunks over every SM slot
-    const int slots = fit[cluster].clusters;
-    const int g = std::max(1, std::min(n_tiles, slots / nchunks));
-    cfg.gridDim = dim3(static_cast<unsigned>(g) * nchunks);
-  }
-  VDK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, mx, batch, H, W, C, nchunks, n_tiles, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend));
+  VDK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, mx, batch, H, W, C, nchunks, n_tiles, w49, bias, ln_w, ln_b, eps, y, rstd_out));
   return VDK_OK;
 }
 
-static int launch_dwconv7_pipe(int mode, const __nv_bfloat16* x, int batch, int H, int W, int C, int chunk, const float* w49,
+static int launch_dwconv7_pipe(const __nv_bfloat16* x, int batch, int H, int W, int C, int chunk, const float* w49,
                                const float* bias, const float* ln_w, const float* ln_b, float eps, __nv_bfloat16* y, float* rstd_out,
-                               const __nv_bfloat16* addend, cudaStream_t s) {
+                               cudaStream_t s) {
   const bool tall = H > 7;  // 14-row tiles (15 warps, one CTA per SM) unless the map is 7 rows high
-#define VDK_DWP(MODEV, CHV)                                                                                                           \
-  return tall ? launch_dwconv7_pipe_t<MODEV, CHV, 14>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)          \
-              : launch_dwconv7_pipe_t<MODEV, CHV, 7>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)
-  if (mode == 0) {
-    if (chunk == 128) { VDK_DWP(0, 128); }
-    if (chunk == 96) { VDK_DWP(0, 96); }
-    VDK_DWP(0, 64);
-  }
-  if (chunk == 128) { VDK_DWP(1, 128); }
-  if (chunk == 96) { VDK_DWP(1, 96); }
-  VDK_DWP(1, 64);
+#define VDK_DWP(CHV)                                                                                                                  \
+  return tall ? launch_dwconv7_pipe_t<CHV, 14>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, s)                         \
+              : launch_dwconv7_pipe_t<CHV, 7>(x, batch, H, W, C, w49, bias, ln_w, ln_b, eps, y, rstd_out, s)
+  if (chunk == 128) { VDK_DWP(128); }
+  if (chunk == 96) { VDK_DWP(96); }
+  VDK_DWP(64);
 #undef VDK_DWP
 }
 
-// mode 0: forward conv + bias + LayerNorm (rstd_out optional); mode 1: plain conv with `w49` (+ addend)
+// mode 0: forward conv + bias + LayerNorm (rstd_out optional); mode 1: plain conv with `w49` (+ addend), the depthwise
+// backward-data pass (dwconv7_bwd_kernel with its weight-gradient half off)
 int vdk::launch_dwconv7(int mode, const __nv_bfloat16* x, int batch, int H, int W, int C, const float* w49, const float* bias,
                           const float* ln_w, const float* ln_b, float eps, __nv_bfloat16* y, float* rstd_out,
                           const __nv_bfloat16* addend, cudaStream_t s) {
   VDK_REQUIRE(C % 8 == 0 && C <= 2048, "dwconv7: C must be a multiple of 8, <= 2048 (got %d)", C);
+  if (mode == 1) return launch_dwconv7_bwd(nullptr, x, batch, H, W, C, w49, addend, y, nullptr, nullptr, s);
   const double dw_elems = static_cast<double>(batch) * H * W * C;
-  ProfScope prof(kProfDepthwise, 2.0 * 49.0 * dw_elems, 2.0 * dw_elems * (addend ? 3.0 : 2.0), s);  // read x (+ addend), write y
+  ProfScope prof(kProfDepthwise, 2.0 * 49.0 * dw_elems, 2.0 * dw_elems * 2.0, s);  // read x, write y
   {
     // channel-chunked kernel (clustered LayerNorm) whenever C splits into <= 16 chunks of <= 128 channels
     int chunk = 0;
@@ -999,7 +904,7 @@ int vdk::launch_dwconv7(int mode, const __nv_bfloat16* x, int batch, int H, int 
       return e ? atoi(e) != 0 : true;
     }();
     if (use_pipe && chunk > 0 && C / chunk <= 16) {
-      const int rc = launch_dwconv7_pipe(mode, x, batch, H, W, C, chunk, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s);
+      const int rc = launch_dwconv7_pipe(x, batch, H, W, C, chunk, w49, bias, ln_w, ln_b, eps, y, rstd_out, s);
       if (rc != VDK_ERR_WORKSPACE) return rc;  // VDK_ERR_WORKSPACE: the persistent grid does not fit this device -> fall through
     }
     if (chunk > 0 && C / chunk <= 16) {
@@ -1017,27 +922,21 @@ int vdk::launch_dwconv7(int mode, const __nv_bfloat16* x, int batch, int H, int 
       cfg.stream = s;
       cudaLaunchAttribute attr[1];
       attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = (mode == 0) ? nchunks : 1;
+      attr[0].val.clusterDim.x = nchunks;
       attr[0].val.clusterDim.y = 1;
       attr[0].val.clusterDim.z = 1;
       cfg.attrs = attr;
       cfg.numAttrs = 1;
-#define VDK_DWC(MODEV, CHV)                                                                                              \
+#define VDK_DWC(CHV)                                                                                                     \
   do {                                                                                                                   \
-    auto kern = dwconv7_chunk_kernel<MODEV, CHV>;                                                                        \
+    auto kern = dwconv7_chunk_kernel<CHV>;                                                                               \
     VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));                     \
-    if (MODEV == 0 && nchunks > 8) VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1)); \
-    VDK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, mx, batch, H, W, C, TH, nchunks, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend)); \
+    if (nchunks > 8) VDK_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));         \
+    VDK_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, mx, batch, H, W, C, TH, nchunks, w49, bias, ln_w, ln_b, eps, y, rstd_out)); \
   } while (0)
-      if (mode == 0) {
-        if (chunk == 128) VDK_DWC(0, 128);
-        else if (chunk == 96) VDK_DWC(0, 96);
-        else VDK_DWC(0, 64);
-      } else {
-        if (chunk == 128) VDK_DWC(1, 128);
-        else if (chunk == 96) VDK_DWC(1, 96);
-        else VDK_DWC(1, 64);
-      }
+      if (chunk == 128) VDK_DWC(128);
+      else if (chunk == 96) VDK_DWC(96);
+      else VDK_DWC(64);
 #undef VDK_DWC
       return VDK_OK;
     }
@@ -1053,13 +952,9 @@ int vdk::launch_dwconv7(int mode, const __nv_bfloat16* x, int batch, int H, int 
   CUtensorMap mx;
   int rc = make_tma_nhwc_16bit(&mx, x, batch, H, W, C, TH + 6, T + 6, box_c);
   if (rc != VDK_OK) return rc;
-#define VDK_DW(TWV)                                                                                                    \
-  return mode == 0 ? launch_dwconv_tw<TWV, 0>(mx, batch, H, W, C, TH, box_c, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s) \
-                   : launch_dwconv_tw<TWV, 1>(mx, batch, H, W, C, TH, box_c, w49, bias, ln_w, ln_b, eps, y, rstd_out, addend, s)
-  if (T == 7) { VDK_DW(7); }
-  if (T == 4) { VDK_DW(4); }
-  VDK_DW(2);
-#undef VDK_DW
+  if (T == 7) return launch_dwconv_tw<7>(mx, batch, H, W, C, TH, box_c, w49, bias, ln_w, ln_b, eps, y, rstd_out, s);
+  if (T == 4) return launch_dwconv_tw<4>(mx, batch, H, W, C, TH, box_c, w49, bias, ln_w, ln_b, eps, y, rstd_out, s);
+  return launch_dwconv_tw<2>(mx, batch, H, W, C, TH, box_c, w49, bias, ln_w, ln_b, eps, y, rstd_out, s);
 }
 
 static int launch_dwconv7_ln(const __nv_bfloat16* x, int batch, int H, int W, int C, const float* w49, const float* bias,

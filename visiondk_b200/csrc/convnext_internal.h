@@ -67,8 +67,10 @@ namespace vdk {
 int launch_ln_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, const float* rstd, int B, int H, int W, int C,
                   const float* ln_w, const float* ln_b, int patch, __nv_bfloat16* dx, const __nv_bfloat16* addend,
                   float* dgamma, float* dbeta, cudaStream_t s);
-int launch_dwconv7_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dconv, int B, int H, int W, int C, float* dw49,
-                         float* dbias, cudaStream_t s);
+// depthwise 7x7 backward from one staging of dconv: dx = bf16(correlation of dconv with w49 + addend) unless w49 is null,
+// dw49 += / dbias += the weight gradient against x unless dw49 is null
+int launch_dwconv7_bwd(const __nv_bfloat16* x, const __nv_bfloat16* dconv, int B, int H, int W, int C, const float* w49,
+                       const __nv_bfloat16* addend, __nv_bfloat16* dx, float* dw49, float* dbias, cudaStream_t s);
 int launch_permute021(const float* in, int A, int Bd, int Cd, const float* row_scale, __nv_bfloat16* out_bf16,
                       float* out_f32, int accumulate, cudaStream_t s);
 int launch_cast_bf16(const float* in, int64_t n, __nv_bfloat16* out, cudaStream_t s);

@@ -475,11 +475,10 @@ static int backward_range(const vdk_convnext_net* net, const vdk_convnext_tensor
         RC(launch_ln_bwd(B16(L.dy), B16(L.y[k]), F32(L.rstd[k]), batch, H, W, C, b->ln_w, b->ln_b, 1, B16(L.dconv), nullptr, gb->ln_w,
                          gb->ln_b, s));
       }
-      // depthwise weight gradient, depthwise data gradient (+ the residual branch)
+      // depthwise data gradient (+ the residual branch) and weight gradient, from one pass over dconv
       // tap gradients stay in the kernel's [49][C] layout in this block's scratch; un-permuted per stage below
-      RC(launch_dwconv7_wgrad(B16(L.xs[st][j]), B16(L.dconv), batch, H, W, C, F32(L.dw49) + static_cast<size_t>(k) * 49 * 2048, gb->dw_b, s));
-      RC(launch_dwconv7(1, B16(L.dconv), batch, H, W, C, b->dw_w_flip, nullptr, nullptr, nullptr, 0.f, B16(dx_other), nullptr,
-                        B16(dx), s));
+      RC(launch_dwconv7_bwd(B16(L.xs[st][j]), B16(L.dconv), batch, H, W, C, b->dw_w_flip, B16(dx), B16(dx_other),
+                            F32(L.dw49) + static_cast<size_t>(k) * 49 * 2048, gb->dw_b, s));
       std::swap(dx, dx_other);
     }
     // tap gradients of the blocks this call executed: [49][C] scratch -> += timm's [C][1][7][7], one launch per <= 32 blocks

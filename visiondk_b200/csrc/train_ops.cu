@@ -1,7 +1,7 @@
 // train_ops.cu — the HBM-bound kernels of the ConvNeXt training backward (everything that is not a GEMM):
 // column sums (bias gradients), LayerNorm backward (with the 2x2 un-patchify of the downsample layers), depthwise-7x7
-// weight gradient, BatchNorm forward/backward with batch statistics (the neck in train mode), layer-scale gradient
-// finalisation, weight packing (fp32 master -> bf16 kernel layouts) and the inverse permutation for gradients.
+// backward (data and weight gradient), BatchNorm forward/backward with batch statistics (the neck in train mode),
+// layer-scale gradient finalisation, weight packing (fp32 master -> bf16 kernel layouts) and the inverse permutation for gradients.
 //
 // Replaces the autograd backward of timm's ConvNeXtBlock / downsample / stem and of the reference neck
 // (models/faceX/backbone/timm_wrapper.py:30-38 in train mode: BatchNorm with batch statistics), i.e. what
@@ -253,167 +253,304 @@ int launch_ln_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* y, const float* 
 }
 
 // ------------------------------------------------------------------------------------------------
-// depthwise 7x7 weight gradient: dw[tap][c] += sum_{b,y,x} dconv[b,y,x,c] * x[b,y+dy-3,x+dx-3,c]; dbias[c] += sum dconv
+// depthwise 7x7 backward of a block, from one staging of the output gradient g = dconv:
+//   data gradient    dx[b,y,x,c] = bf16(sum_{dy,dx} w[dy*7+dx][c] g[b,y+dy-3,x+dx-3,c] + addend[b,y,x,c])  (w: reversed taps)
+//   weight gradient  dw[tap][c] += sum_{b,y,x} g[b,y,x,c] x[b,y+dy-3,x+dx-3,c];  dbias[c] += sum g
 // ------------------------------------------------------------------------------------------------
-// CTA = (group of images, T x T pixel tile, 64-channel chunk): per image the x halo and the dconv tile arrive by TMA
-// (zero-filled out of bounds, so no masks).  A thread owns 4 channels, ONE filter row dy and one 7-pixel half of
-// every tile row: per strip it reads 7 gradient and 13 input vectors for 7 x 7 x 4 FMAs (the 7 taps of its filter row
-// stay in 28 registers over all strips and all images of the group), so the loop is FMA-issue bound, not LDS bound.
-// The two halves meet in shared memory and each CTA issues one atomic per (tap, channel).  C need only be a multiple of
-// 8 (ConvNeXt atto / femto / nano / tiny have 40 / 48 / 80 / 96 channels in stage 0): the last chunk reads channels past
-// C as TMA zero fill and stores nothing for them.
-constexpr int kWgT = 14;
-constexpr int kWgC = 64;
-constexpr int kWgR = 7;  // strip length (pixels) = taps per filter row
+// CTA = (group of images, T x T pixel tile, 64-channel chunk).  A producer warp streams each image's x halo and g halo
+// ((T+6)^2 x 64, zero-filled out of bounds by TMA, so no masks) through a two-stage mbarrier ring, so image i+1 loads
+// while image i computes.  Fourteen consumer warps read the same stage at once:
+//   warps 0-6 (weight gradient): a thread owns 4 channels, ONE filter row dy and one 7-pixel half of every tile row; per
+//     strip it reads 7 gradient (the halo's interior) and 13 input vectors for 7 x 7 x 4 FMAs, the 28 accumulators of its
+//     filter row staying in registers.  Every image starts a fresh chain that is then added to the thread's total, so
+//     a CTA can take many images (one wave of CTAs, each pipelining its images) without lengthening any chain.
+//   warps 7-13 (data gradient): a thread owns 4 channels of a 7-pixel strip of a tile row: 7 filter rows, each 13 g
+//     vectors against 7 taps (fp32, staged once per CTA) for 7 x 7 x 4 FMAs, then the addend and one bf16 store.
+// After the last image the weight-gradient halves meet in shared memory and each CTA issues one atomic per (tap, channel).
+// Either half may be switched off (null taps / null dw49).  C need only be a multiple of 8: the last chunk reads channels
+// past C as TMA zero fill and stores nothing for them.
+//
+// Roundings.  Data gradient: 49 FMAs from zero, then the addend: 50 per output.  Weight gradient: a term passes its image's
+// chain (T x 7 FMAs), the adds of the per-image partials (ipc - 1), the nh strip partials and one atomic per CTA:
+// T * 7 + ipc - 1 + nh + groups * tiles, with groups = ceil(B / ipc).
+constexpr int kBwdT = 14;
+constexpr int kBwdC = 64;
+constexpr int kBwdR = 7;             // strip length (pixels) = taps per filter row
+constexpr int kBwdHalfWarps = 7;     // consumer warps per half
+constexpr int kBwdThreads = (2 * kBwdHalfWarps + 1) * 32;
+
+__device__ __forceinline__ float2 bf16lo_hi(uint32_t t) {  // bf16 pair -> fp32 pair: a shift and a mask
+  return make_float2(__uint_as_float(t << 16), __uint_as_float(t & 0xffff0000u));
+}
 
 // TT: compile-time tile edge (14 or 7: every shared-memory offset an immediate, no bounds predicates) or 0 = runtime
 template <int TT>
-__global__ void __launch_bounds__(224)
-dwconv7_wgrad_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, int B, int H,
-                     int W, int C, int T_rt, int ipc, float* __restrict__ dw49, float* __restrict__ dbias) {
-  extern __shared__ uint8_t wg_raw[];
-  uint8_t* smem = wg_raw + ((128u - (smem_u32(wg_raw) & 127u)) & 127u);
+__global__ void __launch_bounds__(kBwdThreads, 1)
+dwconv7_bwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, int B, int H,
+                   int W, int C, int T_rt, int ipc, const float* __restrict__ w49, const __nv_bfloat16* __restrict__ addend,
+                   __nv_bfloat16* __restrict__ dx_out, float* __restrict__ dw49, float* __restrict__ dbias) {
+  extern __shared__ uint8_t bw_raw[];
+  uint8_t* smem = bw_raw + ((128u - (smem_u32(bw_raw) & 127u)) & 127u);
   const int T = TT > 0 ? TT : T_rt;
   const int halo = T + 6;
-  const int nh = (T + kWgR - 1) / kWgR;   // strips per tile row
-  const int planes = 7 * nh;              // (half, dy) pairs
-  const int x_bytes = halo * halo * kWgC * 2, g_bytes = T * T * kWgC * 2;
-  const int red_bytes = (planes * 7 + nh) * kWgC * 4;
-  const int first = ((x_bytes > red_bytes ? x_bytes : red_bytes) + 127) & ~127;
-  uint8_t* sx = smem;
-  float* red = reinterpret_cast<float*>(smem);  // aliases the x halo once the last image is done
-  uint8_t* sg = smem + first;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sg + ((g_bytes + 127) & ~127));
+  const int nh = (T + kBwdR - 1) / kBwdR;  // strips per tile row
+  const int planes = 7 * nh;               // (half, dy) pairs of the weight gradient
+  const int h_bytes = (halo * halo * kBwdC * 2 + 127) & ~127;
+  const int stage_bytes = 2 * h_bytes;     // x halo, then g halo
+  float* wsm = reinterpret_cast<float*>(smem + 2 * stage_bytes);  // [49][64] taps of this chunk (data gradient)
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(wsm + 49 * kBwdC);
+  uint64_t* empty_bar = full_bar + 2;
+  float* red = reinterpret_cast<float*>(smem);  // aliases stage 0 once every image is done
+  const bool do_data = w49 != nullptr, do_wgrad = dw49 != nullptr;
 
   const int tiles_w = (W + T - 1) / T, tiles_h = (H + T - 1) / T;
-  const int n_cc = (C + kWgC - 1) / kWgC;
+  const int n_cc = (C + kBwdC - 1) / kBwdC;
   int bid = blockIdx.x;
   const int cc = bid % n_cc; bid /= n_cc;
   const int tw = bid % tiles_w; bid /= tiles_w;
   const int th = bid % tiles_h;
   const int b0 = (bid / tiles_h) * ipc;
-  const int b1 = min(B, b0 + ipc);
+  const int n_img = min(B, b0 + ipc) - b0;
   const int oy0 = th * T, ox0 = tw * T;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    prefetch_tensormap(&map_x);
     prefetch_tensormap(&map_g);
-    mbar_init(bar, 1);
+    if (do_wgrad) prefetch_tensormap(&map_x);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2 * kBwdHalfWarps);
+    }
     fence_mbar_init();
   }
+  if (do_data) {
+    for (int i = threadIdx.x; i < 49 * (kBwdC / 4); i += blockDim.x) {
+      const int t = i / (kBwdC / 4), q = i - t * (kBwdC / 4);
+      const int c = cc * kBwdC + q * 4;
+      *reinterpret_cast<float4*>(wsm + t * kBwdC + q * 4) =
+          c < C ? __ldg(reinterpret_cast<const float4*>(w49 + static_cast<size_t>(t) * C + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
   __syncthreads();
 
-  const int quad = threadIdx.x & 15, plane = threadIdx.x >> 4;
-  const bool active = plane < planes;
-  const int hh = plane / 7, dy = plane - hh * 7;
-  const int px0 = hh * kWgR;
-  float2 acc[7][2];  // channel pairs
+  const int quad = threadIdx.x & 15;
+  const int cq = cc * kBwdC + quad * 4;  // first of this thread's 4 channels
+  float2 tot[7][2];                      // weight gradient: this thread's filter row over all its images
+  float btot[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-  for (int dx = 0; dx < 7; ++dx) {
-    acc[dx][0] = make_float2(0.f, 0.f);
-    acc[dx][1] = make_float2(0.f, 0.f);
-  }
-  float bsum[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int d = 0; d < 7; ++d) tot[d][0] = tot[d][1] = make_float2(0.f, 0.f);
+  const int plane = (threadIdx.x >> 4) % (2 * kBwdHalfWarps);  // weight-gradient plane / data-gradient strip slot
+  const int hh = plane / 7, dy = plane - hh * 7;                 // (weight gradient)
 
-  uint32_t phase = 0;
-  for (int b = b0; b < b1; ++b) {
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(bar, x_bytes + g_bytes);
-      tma_load_4d(sx, &map_x, bar, cc * kWgC, ox0 - 3, oy0 - 3, b);
-      tma_load_4d(sg, &map_g, bar, cc * kWgC, ox0, oy0, b);
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1u;
-    if (active) {
-#pragma unroll 1
-      for (int py = 0; py < T; ++py) {
-        float2 g[kWgR][2], x[kWgR + 6][2];
-        const uint8_t* gr = sg + ((py * T + px0) * kWgC + quad * 4) * 2;
-#pragma unroll
-        for (int r = 0; r < kWgR; ++r) {
-          uint2 t = make_uint2(0u, 0u);
-          if (TT > 0 || px0 + r < T) t = *reinterpret_cast<const uint2*>(gr + r * kWgC * 2);
-          g[r][0] = make_float2(__uint_as_float(t.x << 16), __uint_as_float(t.x & 0xffff0000u));  // bf16 -> fp32
-          g[r][1] = make_float2(__uint_as_float(t.y << 16), __uint_as_float(t.y & 0xffff0000u));
-        }
-        const uint8_t* xr = sx + (((py + dy) * halo + px0) * kWgC + quad * 4) * 2;
-#pragma unroll
-        for (int i = 0; i < kWgR + 6; ++i) {
-          uint2 t = make_uint2(0u, 0u);
-          if (TT > 0 || px0 + i < halo) t = *reinterpret_cast<const uint2*>(xr + i * kWgC * 2);
-          x[i][0] = make_float2(__uint_as_float(t.x << 16), __uint_as_float(t.x & 0xffff0000u));
-          x[i][1] = make_float2(__uint_as_float(t.y << 16), __uint_as_float(t.y & 0xffff0000u));
-        }
-        if (dy == 0) {
-#pragma unroll
-          for (int r = 0; r < kWgR; ++r) {
-            bsum[0] += g[r][0].x; bsum[1] += g[r][0].y; bsum[2] += g[r][1].x; bsum[3] += g[r][1].y;
-          }
-        }
-#pragma unroll
-        for (int r = 0; r < kWgR; ++r)
-#pragma unroll
-          for (int dx = 0; dx < 7; ++dx) {
-            acc[dx][0] = ffma2(g[r][0], x[r + dx][0], acc[dx][0]);
-            acc[dx][1] = ffma2(g[r][1], x[r + dx][1], acc[dx][1]);
-          }
+  if (warp == 2 * kBwdHalfWarps) {
+    // ===================== producer: one image ahead of the consumers =====================
+    if (lane == 0) {
+      for (int i = 0; i < n_img; ++i) {
+        const int buf = i & 1;
+        mbar_wait_relaxed(&empty_bar[buf], ((i >> 1) & 1) ^ 1);  // both halves are done with image i - 2
+        uint8_t* st = smem + buf * stage_bytes;
+        mbar_arrive_expect_tx(&full_bar[buf], (do_wgrad ? 2 : 1) * halo * halo * kBwdC * 2);
+        if (do_wgrad) tma_load_4d(st, &map_x, &full_bar[buf], cc * kBwdC, ox0 - 3, oy0 - 3, b0 + i);
+        tma_load_4d(st + h_bytes, &map_g, &full_bar[buf], cc * kBwdC, ox0 - 3, oy0 - 3, b0 + i);
       }
     }
-    __syncthreads();  // every read of this image's tiles is done before the next TMA (or the reduction) overwrites them
-  }
-
-  if (active) {
+    __syncwarp();  // the warp reaches the final __syncthreads converged
+  } else if (warp < kBwdHalfWarps) {
+    // ===================== weight gradient =====================
+    const bool active = do_wgrad && plane < planes;
+    const int px0 = hh * kBwdR;
+    for (int i = 0; i < n_img; ++i) {
+      const int buf = i & 1;
+      mbar_wait(&full_bar[buf], (i >> 1) & 1);
+      if (active) {
+        const uint8_t* sx = smem + buf * stage_bytes;
+        const uint8_t* sg = sx + h_bytes;
+        float2 acc[7][2];
 #pragma unroll
-    for (int dx = 0; dx < 7; ++dx)
-      *reinterpret_cast<float4*>(red + (plane * 7 + dx) * kWgC + quad * 4) =
-          make_float4(acc[dx][0].x, acc[dx][0].y, acc[dx][1].x, acc[dx][1].y);
+        for (int d = 0; d < 7; ++d) acc[d][0] = acc[d][1] = make_float2(0.f, 0.f);
+        float bsum[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 1
+        for (int py = 0; py < T; ++py) {
+          float2 g[kBwdR][2];
+          const uint8_t* gr = sg + (((py + 3) * halo + px0 + 3) * kBwdC + quad * 4) * 2;  // the halo's interior
+#pragma unroll
+          for (int r = 0; r < kBwdR; ++r) {
+            uint2 t = make_uint2(0u, 0u);
+            if (TT > 0 || px0 + r < T) t = *reinterpret_cast<const uint2*>(gr + r * kBwdC * 2);
+            g[r][0] = bf16lo_hi(t.x);
+            g[r][1] = bf16lo_hi(t.y);
+          }
+          if (dy == 0) {
+#pragma unroll
+            for (int r = 0; r < kBwdR; ++r) {
+              bsum[0] += g[r][0].x; bsum[1] += g[r][0].y; bsum[2] += g[r][1].x; bsum[3] += g[r][1].y;
+            }
+          }
+          const uint8_t* xr = sx + (((py + dy) * halo + px0) * kBwdC + quad * 4) * 2;
+#pragma unroll
+          for (int ix = 0; ix < kBwdR + 6; ++ix) {
+            uint2 t = make_uint2(0u, 0u);
+            if (TT > 0 || px0 + ix < halo) t = *reinterpret_cast<const uint2*>(xr + ix * kBwdC * 2);
+            const float2 a = bf16lo_hi(t.x), c = bf16lo_hi(t.y);
+#pragma unroll
+            for (int r = 0; r < kBwdR; ++r) {  // input column ix meets strip pixel r through tap ix - r
+              const int d = ix - r;
+              if (d >= 0 && d < 7) {
+                acc[d][0] = ffma2(g[r][0], a, acc[d][0]);
+                acc[d][1] = ffma2(g[r][1], c, acc[d][1]);
+              }
+            }
+          }
+        }
+#pragma unroll
+        for (int d = 0; d < 7; ++d) {
+          tot[d][0] = make_float2(tot[d][0].x + acc[d][0].x, tot[d][0].y + acc[d][0].y);
+          tot[d][1] = make_float2(tot[d][1].x + acc[d][1].x, tot[d][1].y + acc[d][1].y);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) btot[k] += bsum[k];
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[buf]);
+    }
+  } else {
+    // ===================== data gradient =====================
+    const int strips = T * nh;
+    const bool has_c = do_data && cq < C;
+    for (int i = 0; i < n_img; ++i) {
+      const int buf = i & 1;
+      const int b = b0 + i;
+      mbar_wait(&full_bar[buf], (i >> 1) & 1);
+      const uint8_t* sg = smem + buf * stage_bytes + h_bytes;
+      for (int s = plane; has_c && s < strips; s += 2 * kBwdHalfWarps) {
+        const int py = s / nh, px0 = (s - py * nh) * kBwdR;
+        const int oy = oy0 + py;
+        // the strip's addend is requested before its taps run, so its global-memory latency hides under them
+        bool out[kBwdR];
+        uint2 ad[kBwdR];
+#pragma unroll
+        for (int p = 0; p < kBwdR; ++p) {
+          const int ox = ox0 + px0 + p;
+          out[p] = oy < H && ox < W && (TT > 0 || px0 + p < T);
+          ad[p] = make_uint2(0u, 0u);
+          if (addend && out[p])
+            ad[p] = __ldg(reinterpret_cast<const uint2*>(addend + ((static_cast<int64_t>(b) * H + oy) * W + ox) * C + cq));
+        }
+        float2 acc[kBwdR][2];
+#pragma unroll
+        for (int p = 0; p < kBwdR; ++p) acc[p][0] = acc[p][1] = make_float2(0.f, 0.f);
+#pragma unroll 1
+        for (int fy = 0; fy < 7; ++fy) {
+          float2 wlo[7], whi[7];
+          const float* wrow = wsm + fy * (7 * kBwdC) + quad * 4;
+#pragma unroll
+          for (int d = 0; d < 7; ++d) {
+            const float4 t = *reinterpret_cast<const float4*>(wrow + d * kBwdC);
+            wlo[d] = make_float2(t.x, t.y);
+            whi[d] = make_float2(t.z, t.w);
+          }
+          const uint8_t* gr = sg + (((py + fy) * halo + px0) * kBwdC + quad * 4) * 2;
+#pragma unroll
+          for (int ix = 0; ix < kBwdR + 6; ++ix) {
+            uint2 t = make_uint2(0u, 0u);
+            if (TT > 0 || px0 + ix < halo) t = *reinterpret_cast<const uint2*>(gr + ix * kBwdC * 2);
+            const float2 a = bf16lo_hi(t.x), c = bf16lo_hi(t.y);
+#pragma unroll
+            for (int p = 0; p < kBwdR; ++p) {  // g column ix feeds output pixel p through tap ix - p
+              const int d = ix - p;
+              if (d >= 0 && d < 7) {
+                acc[p][0] = ffma2(a, wlo[d], acc[p][0]);
+                acc[p][1] = ffma2(c, whi[d], acc[p][1]);
+              }
+            }
+          }
+        }
+#pragma unroll
+        for (int p = 0; p < kBwdR; ++p) {
+          if (!out[p]) continue;
+          const int64_t off = ((static_cast<int64_t>(b) * H + oy) * W + ox0 + px0 + p) * C + cq;
+          float o0 = acc[p][0].x, o1 = acc[p][0].y, o2 = acc[p][1].x, o3 = acc[p][1].y;
+          if (addend) {
+            const float2 a = bf16lo_hi(ad[p].x), c = bf16lo_hi(ad[p].y);
+            o0 += a.x; o1 += a.y; o2 += c.x; o3 += c.y;
+          }
+          __nv_bfloat162 lo = __floats2bfloat162_rn(o0, o1), hi = __floats2bfloat162_rn(o2, o3);
+          uint2 t;
+          t.x = *reinterpret_cast<uint32_t*>(&lo);
+          t.y = *reinterpret_cast<uint32_t*>(&hi);
+          *reinterpret_cast<uint2*>(dx_out + off) = t;
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[buf]);
+    }
+  }
+  if (!do_wgrad) return;  // uniform over the CTA
+
+  __syncthreads();  // every stage read is done: red may overwrite stage 0
+  if (warp < kBwdHalfWarps && plane < planes) {
+#pragma unroll
+    for (int d = 0; d < 7; ++d)
+      *reinterpret_cast<float4*>(red + (plane * 7 + d) * kBwdC + quad * 4) =
+          make_float4(tot[d][0].x, tot[d][0].y, tot[d][1].x, tot[d][1].y);
     if (dy == 0) {
 #pragma unroll
-      for (int c = 0; c < 4; ++c) red[(planes * 7 + hh) * kWgC + quad * 4 + c] = bsum[c];
+      for (int k = 0; k < 4; ++k) red[(planes * 7 + hh) * kBwdC + quad * 4 + k] = btot[k];
     }
   }
   __syncthreads();
-  for (int o = threadIdx.x; o < 50 * kWgC; o += blockDim.x) {
-    const int slot = o / kWgC, ch = o - slot * kWgC;  // slot = dy * 7 + dx, or 49 for the bias
-    if (cc * kWgC + ch >= C) continue;                // zero-filled channels of a ragged last chunk
+  for (int o = threadIdx.x; o < 50 * kBwdC; o += blockDim.x) {
+    const int slot = o / kBwdC, ch = o - slot * kBwdC;  // slot = dy * 7 + dx, or 49 for the bias
+    if (cc * kBwdC + ch >= C) continue;                 // zero-filled channels of a ragged last chunk
     float s = 0.f;
     if (slot < 49) {
       const int sdy = slot / 7, sdx = slot - sdy * 7;
-      for (int h2 = 0; h2 < nh; ++h2) s += red[((h2 * 7 + sdy) * 7 + sdx) * kWgC + ch];
-      atomicAdd(dw49 + slot * C + cc * kWgC + ch, s);
+      for (int h2 = 0; h2 < nh; ++h2) s += red[((h2 * 7 + sdy) * 7 + sdx) * kBwdC + ch];
+      atomicAdd(dw49 + slot * C + cc * kBwdC + ch, s);
     } else {
-      for (int h2 = 0; h2 < nh; ++h2) s += red[(planes * 7 + h2) * kWgC + ch];
-      atomicAdd(dbias + cc * kWgC + ch, s);
+      for (int h2 = 0; h2 < nh; ++h2) s += red[(planes * 7 + h2) * kBwdC + ch];
+      atomicAdd(dbias + cc * kBwdC + ch, s);
     }
   }
 }
 
-int launch_dwconv7_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dconv, int B, int H, int W, int C, float* dw49,
-                         float* dbias, cudaStream_t s) {
-  const double wg_elems = static_cast<double>(B) * H * W * C;
-  ProfScope prof(kProfDepthwise, 2.0 * 49.0 * wg_elems, 2.0 * 2.0 * wg_elems, s);  // read x and the output gradient
-
-  VDK_REQUIRE(C % 8 == 0, "dwconv7_wgrad: C must be a multiple of 8 (got %d)", C);
-  const int T = std::min(kWgT, std::max(H, W));
+// x / dw49 / dbias null: no weight gradient; w49 null: no data gradient
+int launch_dwconv7_bwd(const __nv_bfloat16* x, const __nv_bfloat16* dconv, int B, int H, int W, int C, const float* w49,
+                       const __nv_bfloat16* addend, __nv_bfloat16* dx, float* dw49, float* dbias, cudaStream_t s) {
+  VDK_REQUIRE(C % 8 == 0, "dwconv7 backward: C must be a multiple of 8 (got %d)", C);
+  VDK_REQUIRE((w49 == nullptr || dx != nullptr) && (dw49 == nullptr || (x != nullptr && dbias != nullptr)),
+              "dwconv7 backward: missing operand");
+  const double elems = static_cast<double>(B) * H * W * C;
+  const int halves = (w49 ? 1 : 0) + (dw49 ? 1 : 0);
+  // read g (+ x), write dx (+ read the addend)
+  ProfScope prof(kProfDepthwise, 2.0 * 49.0 * elems * halves, 2.0 * elems * (1 + (dw49 ? 1 : 0) + (w49 ? (addend ? 2 : 1) : 0)), s);
+  if (halves == 0) return VDK_OK;
+  const int T = std::min(kBwdT, std::max(H, W));
   CUtensorMap mx, mg;
-  int rc = make_tma_nhwc_16bit(&mx, x, B, H, W, C, T + 6, T + 6, kWgC);
+  int rc = make_tma_nhwc_16bit(&mg, dconv, B, H, W, C, T + 6, T + 6, kBwdC);
   if (rc != VDK_OK) return rc;
-  rc = make_tma_nhwc_16bit(&mg, dconv, B, H, W, C, T, T, kWgC);
-  if (rc != VDK_OK) return rc;
-  const int halo = T + 6, nh = (T + kWgR - 1) / kWgR, planes = 7 * nh;
-  const int x_bytes = halo * halo * kWgC * 2, red_bytes = (planes * 7 + nh) * kWgC * 4;
-  const int smem = ((std::max(x_bytes, red_bytes) + 127) & ~127) + ((T * T * kWgC * 2 + 127) & ~127) + 16 + 128;
-  VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_wgrad_kernel<14>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-  VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_wgrad_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-  VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_wgrad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-  // images per CTA: keep >= ~4 CTAs per SM, and amortise the final atomics over as many images as that allows
-  const int64_t per_image = static_cast<int64_t>((H + T - 1) / T) * ((W + T - 1) / T) * ((C + kWgC - 1) / kWgC);
-  const int ipc = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(16, (per_image * B) / (sm_count() * 4))));
+  mx = mg;
+  if (dw49) {
+    rc = make_tma_nhwc_16bit(&mx, x, B, H, W, C, T + 6, T + 6, kBwdC);
+    if (rc != VDK_OK) return rc;
+  }
+  const int halo = T + 6, nh = (T + kBwdR - 1) / kBwdR;
+  const int h_bytes = (halo * halo * kBwdC * 2 + 127) & ~127;
+  VDK_REQUIRE((7 * 7 * nh + nh) * kBwdC * 4 <= 2 * h_bytes, "dwconv7 backward: reduction does not fit stage 0");
+  const int smem = 4 * h_bytes + 49 * kBwdC * 4 + 4 * 8 + 128;
+  VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_bwd_kernel<14>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_bwd_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  VDK_CUDA_OK(cudaFuncSetAttribute(dwconv7_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  // images per CTA: one wave of CTAs (one per SM), each pipelining its images through the ring.  Never fewer than the
+  // weight-gradient-only grouping of earlier releases (>= ~4 CTAs per SM, at most 16 images), so that the per-image
+  // chains plus the fewer atomics never exceed that grouping's roundings (T*7*ipc + nh + groups*tiles).
+  const int64_t per_image = static_cast<int64_t>((H + T - 1) / T) * ((W + T - 1) / T) * ((C + kBwdC - 1) / kBwdC);
+  const int64_t ipc_min = std::max<int64_t>(1, std::min<int64_t>(16, (per_image * B) / (sm_count() * 4)));
+  const int ipc = static_cast<int>(std::min<int64_t>(B, std::max<int64_t>(ipc_min, (per_image * B + sm_count() - 1) / sm_count())));
   const unsigned grid = static_cast<unsigned>(((B + ipc - 1) / ipc) * per_image);
-  const int threads = ((16 * planes + 31) / 32) * 32;
-  if (T == 14) dwconv7_wgrad_kernel<14><<<grid, threads, smem, s>>>(mx, mg, B, H, W, C, T, ipc, dw49, dbias);
-  else if (T == 7) dwconv7_wgrad_kernel<7><<<grid, threads, smem, s>>>(mx, mg, B, H, W, C, T, ipc, dw49, dbias);
-  else dwconv7_wgrad_kernel<0><<<grid, threads, smem, s>>>(mx, mg, B, H, W, C, T, ipc, dw49, dbias);
+  if (T == 14) dwconv7_bwd_kernel<14><<<grid, kBwdThreads, smem, s>>>(mx, mg, B, H, W, C, T, ipc, w49, addend, dx, dw49, dbias);
+  else if (T == 7) dwconv7_bwd_kernel<7><<<grid, kBwdThreads, smem, s>>>(mx, mg, B, H, W, C, T, ipc, w49, addend, dx, dw49, dbias);
+  else dwconv7_bwd_kernel<0><<<grid, kBwdThreads, smem, s>>>(mx, mg, B, H, W, C, T, ipc, w49, addend, dx, dw49, dbias);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }
@@ -825,8 +962,16 @@ extern "C" int vdk_dwconv7(int mode, const void* x, int batch, int H, int W, int
 extern "C" int vdk_dwconv7_wgrad(const void* x, const void* dconv, int batch, int H, int W, int C, float* dw49, float* dbias,
                                  void* stream) {
   VDK_REQUIRE(x && dconv && dw49 && dbias, "vdk_dwconv7_wgrad: null operand");
-  return launch_dwconv7_wgrad(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dconv), batch, H, W,
-                              C, dw49, dbias, reinterpret_cast<cudaStream_t>(stream));
+  return launch_dwconv7_bwd(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dconv), batch, H, W, C,
+                            nullptr, nullptr, nullptr, dw49, dbias, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vdk_dwconv7_bwd(const void* x, const void* dconv, int batch, int H, int W, int C, const float* w49,
+                               const void* addend, void* dx, float* dw49, float* dbias, void* stream) {
+  VDK_REQUIRE(x && dconv && w49 && dx && dw49 && dbias, "vdk_dwconv7_bwd: null operand");
+  return launch_dwconv7_bwd(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dconv), batch, H, W, C,
+                            w49, reinterpret_cast<const __nv_bfloat16*>(addend), reinterpret_cast<__nv_bfloat16*>(dx), dw49, dbias,
+                            reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vdk_batchnorm_train_fwd(const void* x, int rows, int C, int is_bf16, const float* weight, const float* bias,
