@@ -1016,6 +1016,8 @@ typedef struct vdk_jpeg_desc {
   int h[3], v[3];                   /* sampling factors (1 x 1 for a single component) */
   int16_t quant[3][64];             /* natural order, cast to 16 bits like libjpeg's ISLOW_MULT_TYPE */
   vdk_jpeg_huff dc[3], ac[3];       /* per component */
+  int64_t scan_first;               /* set by vdk_jpeg_parse_progressive: the image's first entry in the scan table */
+  int n_scans, n_levels;            /* set by vdk_jpeg_parse_progressive: its scans, and 1 + their largest level */
 } vdk_jpeg_desc;
 int vdk_jpeg_parse(const uint8_t* packed, vdk_jpeg_desc* descs, int n, int64_t* segs, int64_t seg_capacity);
 size_t vdk_jpeg_workspace_bytes(vdk_jpeg_desc* descs, int n);
@@ -1023,6 +1025,54 @@ int vdk_jpeg_decode(const uint8_t* data, const vdk_jpeg_desc* descs, const vdk_j
                     int n, uint8_t* out, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 /* sizeof() of vdk_jpeg_huff and vdk_jpeg_desc, in that order. */
 int vdk_jpeg_struct_sizes(size_t* out, int n);
+
+/* ---- progressive JPEG decoding (the same input path; the same descriptors, workspace and status words) */
+/* Decodes, bit for bit with the same libjpeg-turbo call, the progressive JPEGs whose frame the baseline decoder would take:
+ * one SOF2 frame of 8-bit samples, 1 component or 3 in YCbCr, sampling 4:4:4 / 4:2:2 / 4:2:0 / 4:4:0, any restart interval,
+ * and any scan script that libjpeg (jdphuff.c) accepts without a warning and that brings every coefficient of every
+ * component to full precision (so libjpeg's block smoothing of incomplete scripts never applies).  Each scan uses the DHT and
+ * DRI in force at its SOS; quantisation tables are latched at the first scan that contains the component (jdinput.c).
+ * oracle/jpeg_progressive.py restates the arithmetic.
+ *
+ * 1. vdk_jpeg_parse as for baseline files; it gives progressive files VDK_JPEG_PROCESS.
+ * 2. vdk_jpeg_parse_progressive (host only, no GPU): re-reads only the descriptors whose reason is VDK_JPEG_PROCESS and
+ *    fills them like a baseline descriptor (size, components, sampling, MCU grid, latched quantisation tables; dc / ac are
+ *    not used).  Their reason becomes VDK_JPEG_DEVICE_PROGRESSIVE or a fallback reason (VDK_JPEG_PROCESS for arithmetic,
+ *    lossless and hierarchical frames; VDK_JPEG_SCAN for scripts that leave a coefficient unsent or not fully refined, or
+ *    that libjpeg warns about (JWRN_BOGUS_PROGRESSION); VDK_JPEG_MALFORMED for scan parameters libjpeg refuses
+ *    (JERR_BAD_PROGRESSION) and the header faults vdk_jpeg_parse refuses).  Every scan of a progressive image goes into
+ *    `scans` (n_scans entries from scans[descs[i].scan_first]), and the restart-interval starts of each scan go into `segs`
+ *    after those vdk_jpeg_parse wrote (scan j's n_segments entries from segs[scan.seg_first]; the image's descriptor spans
+ *    them all with seg_first / n_segments).  Entries past scan_capacity / seg_capacity are not written: call both parsers
+ *    again with larger arrays.  Returns VDK_OK.
+ * 3. out_offset as in step 2 above, for the VDK_JPEG_DEVICE and VDK_JPEG_DEVICE_PROGRESSIVE images; vdk_jpeg_workspace_bytes
+ *    lays out both kinds.
+ * 4. vdk_jpeg_decode_ex: vdk_jpeg_decode plus the scan table (host `scans`, device copy `scans_dev`): the baseline Huffman
+ *    kernel, then one progressive Huffman launch per dependency level across the batch (one thread per image, scan of that
+ *    level and restart interval: jdphuff.c's DC first / DC refine / AC first / AC refine into the same zero-initialised int16
+ *    store), then the IDCT and colour kernels once over both kinds.  Status words as for vdk_jpeg_decode (0 for a decoded
+ *    image of either kind).  vdk_jpeg_decode itself skips VDK_JPEG_DEVICE_PROGRESSIVE images (VDK_JPEG_BAD_SKIPPED). */
+enum { VDK_JPEG_DEVICE_PROGRESSIVE = 11 };
+typedef struct vdk_jpeg_scan {
+  int64_t scan_begin, scan_end;     /* entropy-coded bytes [begin, end) from the file's start; scan_end is the next marker */
+  int64_t seg_first;                /* the scan's first entry in the restart-interval table */
+  int n_segments;                   /* restart intervals in the scan (1 without DRI) */
+  int restart_interval;             /* DRI in force at the SOS: MCUs (blocks in a one-component scan) per interval, 0 = none */
+  int level;                        /* 1 + the largest level of the earlier scans that share a component and a coefficient
+                                       with this one (0 if none): scans of one level write disjoint coefficients */
+  int ncomp;                        /* components in the scan; more than one only in a DC scan (interleaved over MCUs) */
+  int comp[3];                      /* their frame indexes, in frame order */
+  int ss, se, ah, al;               /* spectral selection and successive approximation */
+  int units_x, units_y;             /* MCU grid of an interleaved scan; the component's own blocks in a one-component scan */
+  vdk_jpeg_huff tbl[3];             /* DC first: the DC table of each scan component; AC: tbl[0] is the AC table */
+} vdk_jpeg_scan;
+int vdk_jpeg_parse_progressive(const uint8_t* packed, vdk_jpeg_desc* descs, int n, vdk_jpeg_scan* scans, int64_t scan_capacity,
+                               int64_t* segs, int64_t seg_capacity);
+int vdk_jpeg_decode_ex(const uint8_t* data, const vdk_jpeg_desc* descs, const vdk_jpeg_desc* descs_dev, const int64_t* segs_dev,
+                       const vdk_jpeg_scan* scans, const vdk_jpeg_scan* scans_dev, int n, uint8_t* out, int32_t* status,
+                       void* workspace, size_t workspace_bytes, void* stream);
+/* sizeof() of vdk_jpeg_scan. */
+int vdk_jpeg_progressive_struct_sizes(size_t* out, int n);
 
 /* Live kernel timing inside a real step (bench.py's roofline legs; not part of the reference's surface).  Between
  * vdk_prof_begin() and vdk_prof_end() every launch of the categories below is bracketed by two CUDA events on the stream it

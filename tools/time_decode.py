@@ -10,7 +10,9 @@ Per corpus:
 and for corpus A, alternating host and device decoding on the same folder: folder-fed ConvNeXt-B extraction
 (CBIRFolderData -> embed, batch 256) and a folder-fed ConvNeXt-B train step (FolderTrainData val list -> FaceTrainer.step,
 batch 128), in images/s.
-    python tools/time_decode.py [--reps 3]"""
+With --progressive every file of both corpora is saved progressive (Pillow's default scan script, 10 scans), and kernel_ms
+also lists the progressive Huffman kernel's time per dependency level (level_ms, one launch each).
+    python tools/time_decode.py [--reps 3] [--progressive]"""
 import argparse
 import json
 import os
@@ -28,14 +30,15 @@ import torch  # noqa: E402
 from PIL import Image  # noqa: E402
 
 
-def write_corpora(root):
+def write_corpora(root, progressive=False):
     from time_augment import images
     a_dir = os.path.join(root, "A", "gallery", "id0")
     os.makedirs(a_dir)
     for k, im in enumerate(images(256)):
-        Image.fromarray(im).save(os.path.join(a_dir, f"{k:04d}.jpg"), quality=90, subsampling=2)
+        Image.fromarray(im).save(os.path.join(a_dir, f"{k:04d}.jpg"), quality=90, subsampling=2, progressive=progressive)
     os.makedirs(os.path.join(root, "A", "query", "id0"))
-    Image.fromarray(images(1)[0]).save(os.path.join(root, "A", "query", "id0", "q.jpg"), quality=90, subsampling=2)
+    Image.fromarray(images(1)[0]).save(os.path.join(root, "A", "query", "id0", "q.jpg"), quality=90, subsampling=2,
+                                       progressive=progressive)
     rng = np.random.default_rng(1)
     for name, kw in (("B", {}), ("B_dri", {"restart_marker_rows": 1})):
         os.makedirs(os.path.join(root, name))
@@ -43,8 +46,9 @@ def write_corpora(root):
         small = rng.integers(0, 256, (48, 63, 3), dtype=np.uint8)
         base = np.asarray(Image.fromarray(small).resize((4032, 3024), Image.BICUBIC), np.int16)
         im = Image.fromarray(np.clip(base + rng.integers(-12, 13, (3024, 4032, 3)), 0, 255).astype(np.uint8))
-        im.save(os.path.join(root, "B", f"{k:02d}.jpg"), quality=90, subsampling=2)
-        im.save(os.path.join(root, "B_dri", f"{k:02d}.jpg"), quality=90, subsampling=2, restart_marker_rows=1)
+        im.save(os.path.join(root, "B", f"{k:02d}.jpg"), quality=90, subsampling=2, progressive=progressive)
+        im.save(os.path.join(root, "B_dri", f"{k:02d}.jpg"), quality=90, subsampling=2, restart_marker_rows=1,
+                progressive=progressive)
 
 
 def host_rate(files, nw, reps):
@@ -78,11 +82,16 @@ def device_rate(files, batch, reps):
         torch.cuda.synchronize()
     split = {}
     for ev in prof.key_averages():
-        for k in ("entropy", "idct", "color"):
+        for k in ("entropy", "progressive", "idct", "color"):
             if f"jpeg_{k}_kernel" in ev.key:
                 split[k] = split.get(k, 0.0) + ev.device_time_total / 1e3
+    split = {k: round(v, 3) for k, v in split.items()}
+    levels = [round(e.time_range.elapsed_us() / 1e3, 3) for e in prof.events()
+              if "jpeg_progressive_kernel" in e.name and e.device_type.name == "CUDA"]
+    if levels:
+        split["level_ms"] = levels
     dec.close()
-    return rate, {k: round(v, 3) for k, v in split.items()}, len(chunks[0])
+    return rate, split, len(chunks[0])
 
 
 def folder_fed(root_a, reps):
@@ -158,13 +167,15 @@ def folder_fed(root_a, reps):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--progressive", action="store_true", help="save both corpora as progressive JPEGs")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("time_decode.py measures on a CUDA device; none is visible")
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
     with tempfile.TemporaryDirectory() as root:  # the corpora (about 210 MB) are removed when the run ends
-        write_corpora(root)
-        res = {"gpu": q.stdout.strip().splitlines()[0] if q.stdout else "unknown", "host_cores": os.cpu_count()}
+        write_corpora(root, args.progressive)
+        res = {"gpu": q.stdout.strip().splitlines()[0] if q.stdout else "unknown", "host_cores": os.cpu_count(),
+               "progressive": args.progressive}
         for name, d, batch in (("A", os.path.join(root, "A", "gallery", "id0"), 256), ("B", os.path.join(root, "B"), 32),
                                ("B_dri", os.path.join(root, "B_dri"), 32)):
             files = sorted(os.path.join(d, f) for f in os.listdir(d))

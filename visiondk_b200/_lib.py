@@ -79,7 +79,18 @@ class JpegDesc(C.Structure):
                 ("idct_cta_base", C.c_int64), ("color_cta_base", C.c_int64), ("width", C.c_int), ("height", C.c_int),
                 ("ncomp", C.c_int), ("reason", C.c_int), ("restart_interval", C.c_int), ("n_segments", C.c_int),
                 ("mcus_x", C.c_int), ("mcus_y", C.c_int), ("hmax", C.c_int), ("vmax", C.c_int), ("h", C.c_int * 3),
-                ("v", C.c_int * 3), ("quant", (C.c_int16 * 64) * 3), ("dc", JpegHuff * 3), ("ac", JpegHuff * 3)]
+                ("v", C.c_int * 3), ("quant", (C.c_int16 * 64) * 3), ("dc", JpegHuff * 3), ("ac", JpegHuff * 3),
+                ("scan_first", C.c_int64), ("n_scans", C.c_int), ("n_levels", C.c_int)]
+
+
+JPEG_DEVICE_PROGRESSIVE = 11
+
+
+class JpegScan(C.Structure):
+    _fields_ = [("scan_begin", C.c_int64), ("scan_end", C.c_int64), ("seg_first", C.c_int64), ("n_segments", C.c_int),
+                ("restart_interval", C.c_int), ("level", C.c_int), ("ncomp", C.c_int), ("comp", C.c_int * 3), ("ss", C.c_int),
+                ("se", C.c_int), ("ah", C.c_int), ("al", C.c_int), ("units_x", C.c_int), ("units_y", C.c_int),
+                ("tbl", JpegHuff * 3)]
 
 
 class ProfTotal(C.Structure):
@@ -127,6 +138,9 @@ SIGNATURES = {
     "vdk_jpeg_workspace_bytes": (_sz, [C.POINTER(JpegDesc), _i]),
     "vdk_jpeg_decode": (_i, [_p, C.POINTER(JpegDesc), _p, _p, _i, _p, _p, _p, _sz, _p]),
     "vdk_jpeg_struct_sizes": (_i, [_p, _i]),
+    "vdk_jpeg_parse_progressive": (_i, [_p, C.POINTER(JpegDesc), _i, _p, _i64, _p, _i64]),
+    "vdk_jpeg_decode_ex": (_i, [_p, C.POINTER(JpegDesc), _p, _p, _p, _p, _i, _p, _p, _p, _sz, _p]),
+    "vdk_jpeg_progressive_struct_sizes": (_i, [_p, _i]),
     "vdk_prof_begin": (_i, []),
     "vdk_prof_end": (_i, [C.POINTER(ProfTotal), _i]),
     "vdk_gemm": (_i, [_p, _p]),

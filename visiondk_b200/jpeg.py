@@ -1,13 +1,14 @@
-"""Baseline JPEG decoding on the device (csrc/jpeg.cu), bit-exact with `Image.open(path).convert("RGB")` for the files it takes,
-with the host decoder inside the same batch for every other file.
+"""Baseline and progressive JPEG decoding on the device (csrc/jpeg.cu), bit-exact with `Image.open(path).convert("RGB")` for
+the files it takes, with the host decoder inside the same batch for every other file.
 
     dec = JpegDecoder("cuda", host_decode=read_image)
     batch = dec(paths)              # DecodedBatch: device uint8 RGB buffer + vdk_image_desc array + shapes
     ImagePreprocessor(224)(batch)   # or TrainAugmenter(...)(batch, ...): no host round trip
 
-Per batch, `start`: read the files on host threads, parse their headers (vdk_jpeg_parse, host), submit every file the device
-does not take (not a JPEG, outside the baseline set, more pixels than PIL.Image.MAX_IMAGE_PIXELS) to `host_decode` on host
-threads, upload only the compressed bytes, descriptors and restart-interval table (one copy), launch the decode.  `finish`:
+Per batch, `start`: read the files on host threads, parse their headers (vdk_jpeg_parse, then vdk_jpeg_parse_progressive on
+the files the first parser leaves as VDK_JPEG_PROCESS; host), submit every file the device does not take (not a JPEG,
+outside the baseline and progressive sets, more pixels than PIL.Image.MAX_IMAGE_PIXELS) to `host_decode` on host threads,
+upload only the compressed bytes, descriptors, restart-interval table and scan table (one copy), launch the decode.  `finish`:
 read back the per-image status words (one small copy), decode with `host_decode` the streams the device flagged as not well
 formed, and upload the host-decoded images into their slots.  An exception `host_decode` raises is raised by `finish`, for
 the first failing file of the batch, as a host decoder would raise it for that batch.
@@ -71,7 +72,8 @@ class JpegDecoder:
         self.host_decode, self.nw, self.budget = host_decode, max(1, int(nw)), int(workspace_budget)
         self._pool = None
         self._pinned = self._dev = self._ws = None
-        self._segs = np.zeros(1 << 12, np.int64)  # restart-interval starts, filled by the parser
+        self._segs = np.zeros(1 << 12, np.int64)  # restart-interval starts, filled by the parsers
+        self._scans = (_lib.JpegScan * 64)()  # scans of the progressive files, filled by vdk_jpeg_parse_progressive
         self._copied = None  # event after the last copy out of _pinned
         self._img_pinned = None
         self._img_copied = None  # event after the last copy out of _img_pinned
@@ -119,23 +121,30 @@ class JpegDecoder:
         host = self._pinned.numpy()
         for i, b in enumerate(blobs):
             host[offs[i]:offs[i] + len(b)] = np.frombuffer(b, np.uint8)
-        while n:  # parse; again with a larger restart-interval table when this one was too small
+        device = (_lib.JPEG_DEVICE, _lib.JPEG_DEVICE_PROGRESSIVE)
+        while n:  # parse; again with larger restart-interval and scan tables when these were too small
             _lib.check(lib.vdk_jpeg_parse(self._pinned.data_ptr(), descs, n, self._segs.ctypes.data, len(self._segs)),
                        "vdk_jpeg_parse")
-            need = max([descs[i].seg_first + descs[i].n_segments for i in range(n) if descs[i].reason == _lib.JPEG_DEVICE],
-                       default=0)
-            if need <= len(self._segs):
+            _lib.check(lib.vdk_jpeg_parse_progressive(self._pinned.data_ptr(), descs, n, self._scans, len(self._scans),
+                                                      self._segs.ctypes.data, len(self._segs)), "vdk_jpeg_parse_progressive")
+            need = max([descs[i].seg_first + descs[i].n_segments for i in range(n) if descs[i].reason in device], default=0)
+            need_scans = max([descs[i].scan_first + descs[i].n_scans for i in range(n)
+                              if descs[i].reason == _lib.JPEG_DEVICE_PROGRESSIVE], default=0)
+            if need <= len(self._segs) and need_scans <= len(self._scans):
                 break
-            self._segs = np.zeros(need * 2, np.int64)
+            if need > len(self._segs):
+                self._segs = np.zeros(need * 2, np.int64)
+            if need_scans > len(self._scans):
+                self._scans = (_lib.JpegScan * (need_scans * 2))()
             for i, b in enumerate(blobs):
                 descs[i].data_offset, descs[i].data_bytes = offs[i], len(b)
         limit = Image.MAX_IMAGE_PIXELS  # read per call: users set it; above it Image.open warns, above twice it raises
         for i in range(n):
-            if descs[i].reason == _lib.JPEG_DEVICE and limit is not None and descs[i].width * descs[i].height > limit:
+            if descs[i].reason in device and limit is not None and descs[i].width * descs[i].height > limit:
                 descs[i].reason = _lib.JPEG_TOO_LARGE
         reasons = [int(descs[i].reason) for i in range(n)]
-        on_dev = [i for i in range(n) if reasons[i] == _lib.JPEG_DEVICE]
-        host_jobs = {i: self.pool().submit(self.host_decode, files[i]) for i in range(n) if reasons[i] != _lib.JPEG_DEVICE}
+        on_dev = [i for i in range(n) if reasons[i] in device]
+        host_jobs = {i: self.pool().submit(self.host_decode, files[i]) for i in range(n) if reasons[i] not in device}
         shapes: List[Optional[tuple]] = [None] * n
         slots, out_bytes = [0] * n, 0
         for i in on_dev:
@@ -166,11 +175,15 @@ class JpegDecoder:
             at += C.sizeof(arr)
         seg_at = _up(at, 256)
         n_segs = max([descs[i].seg_first + descs[i].n_segments for i in on_dev], default=0)
-        total = seg_at + 8 * n_segs
+        scan_at = _up(seg_at + 8 * n_segs, 256)
+        n_scans = max([descs[i].scan_first + descs[i].n_scans for i in on_dev if reasons[i] == _lib.JPEG_DEVICE_PROGRESSIVE],
+                      default=0)
+        total = scan_at + C.sizeof(_lib.JpegScan) * n_scans
         self._reserve(total)
         for g, arr, g_at in launches:
             C.memmove(self._pinned.data_ptr() + g_at, C.addressof(arr), C.sizeof(arr))
         C.memmove(self._pinned.data_ptr() + seg_at, self._segs.ctypes.data, 8 * n_segs)
+        C.memmove(self._pinned.data_ptr() + scan_at, C.addressof(self._scans), C.sizeof(_lib.JpegScan) * n_scans)
         out = torch.empty((max(out_bytes, 256),), dtype=torch.uint8, device=self.device)
         status = torch.zeros((max(len(on_dev), 1),), dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
@@ -182,9 +195,15 @@ class JpegDecoder:
             s = 0
             base = self._dev.data_ptr()
             for g, arr, g_at in launches:
-                _lib.check(lib.vdk_jpeg_decode(base, arr, base + g_at, base + seg_at, len(g), out.data_ptr(),
-                                               status.data_ptr() + 4 * s, self._ws.data_ptr(), self._ws.numel(),
-                                               _lib.stream_ptr()), "vdk_jpeg_decode")
+                if n_scans:  # baseline and progressive images
+                    _lib.check(lib.vdk_jpeg_decode_ex(base, arr, base + g_at, base + seg_at, C.addressof(self._scans),
+                                                      base + scan_at, len(g), out.data_ptr(), status.data_ptr() + 4 * s,
+                                                      self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()),
+                               "vdk_jpeg_decode_ex")
+                else:
+                    _lib.check(lib.vdk_jpeg_decode(base, arr, base + g_at, base + seg_at, len(g), out.data_ptr(),
+                                                   status.data_ptr() + 4 * s, self._ws.data_ptr(), self._ws.numel(),
+                                                   _lib.stream_ptr()), "vdk_jpeg_decode")
                 s += len(g)
             status_host = status.to("cpu", non_blocking=True) if on_dev else None
             done = torch.cuda.Event()
