@@ -610,6 +610,21 @@ int vdk_convnext_train_backward_units(const vdk_convnext_net* net);
 int vdk_convnext_train_backward_range(const vdk_convnext_net* net, const vdk_convnext_tensors* params,
                                       const vdk_convnext_tensors* grads, const float* d_feats, int batch, void* workspace,
                                       size_t workspace_bytes, void* stream, int unit_begin, int unit_end);
+/* Where the train workspace keeps one buffer: the saved activations of vdk_convnext_train_forward and the backward's scratch,
+ * as a byte offset into the workspace and a size (both from the layout the train entry points use).  `index` selects the
+ * block (Y, RSTD, HPRE, HPOST: 0 .. sum(depths) - 1, stage-major), the stage (PATCH, PRSTD: 1 .. 3) or, for XS, the
+ * residual-stream node stage * (VDK_CONVNEXT_MAX_BLOCKS + 1) + j, j = 0 .. depths[stage]; it is ignored for the others.
+ * An unknown id or an index out of range is refused with VDK_ERR_INVALID. */
+enum {
+  VDK_CONVNEXT_TRAIN_P0, VDK_CONVNEXT_TRAIN_Z0, VDK_CONVNEXT_TRAIN_RSTD0, VDK_CONVNEXT_TRAIN_XS, VDK_CONVNEXT_TRAIN_Y,
+  VDK_CONVNEXT_TRAIN_RSTD, VDK_CONVNEXT_TRAIN_HPRE, VDK_CONVNEXT_TRAIN_HPOST, VDK_CONVNEXT_TRAIN_PATCH, VDK_CONVNEXT_TRAIN_PRSTD,
+  VDK_CONVNEXT_TRAIN_F, VDK_CONVNEXT_TRAIN_FRSTD, VDK_CONVNEXT_TRAIN_FN, VDK_CONVNEXT_TRAIN_BN2_MEAN, VDK_CONVNEXT_TRAIN_BN2_RSTD,
+  VDK_CONVNEXT_TRAIN_Z, VDK_CONVNEXT_TRAIN_ZSLAB, VDK_CONVNEXT_TRAIN_BN1_MEAN, VDK_CONVNEXT_TRAIN_BN1_RSTD, VDK_CONVNEXT_TRAIN_DXA,
+  VDK_CONVNEXT_TRAIN_DXB, VDK_CONVNEXT_TRAIN_DY, VDK_CONVNEXT_TRAIN_DCONV, VDK_CONVNEXT_TRAIN_G, VDK_CONVNEXT_TRAIN_SDO,
+  VDK_CONVNEXT_TRAIN_DW49, VDK_CONVNEXT_TRAIN_GWC, VDK_CONVNEXT_TRAIN_GWNECK, VDK_CONVNEXT_TRAIN_DZ, VDK_CONVNEXT_TRAIN_DZB,
+  VDK_CONVNEXT_TRAIN_DFN, VDK_CONVNEXT_TRAIN_WSLAB, VDK_CONVNEXT_TRAIN_NUM_BUFFERS
+};
+int vdk_convnext_train_buffer(const vdk_convnext_net* net, int batch, int id, int index, size_t* offset, size_t* bytes);
 
 /* Building blocks of the backward, exported for unit parity tests (NHWC bf16 activations, fp32 parameter grads +=):
  *   vdk_dwconv7             mode 0: LayerNorm_C(dwconv7(x)+bias) (rstd_out optional); mode 1: dwconv7(x) with `w49` (+addend)
@@ -720,6 +735,16 @@ int vdk_vit_train_backward_units(const vdk_vit_net* net);
 int vdk_vit_train_backward_range(const vdk_vit_net* net, const vdk_vit_tensors* params, const vdk_vit_tensors* grads,
                                  const float* d_feats, int batch, void* workspace, size_t workspace_bytes, void* stream, int unit_begin,
                                  int unit_end);
+/* The vdk_convnext_train_buffer of the ViT train workspace.  `index` selects the block (Y1 .. XO: 0 .. depth - 1); it is
+ * ignored for the others. */
+enum {
+  VDK_VIT_TRAIN_ROWS, VDK_VIT_TRAIN_TOK, VDK_VIT_TRAIN_X0, VDK_VIT_TRAIN_Y1, VDK_VIT_TRAIN_R1, VDK_VIT_TRAIN_QKV, VDK_VIT_TRAIN_ATT,
+  VDK_VIT_TRAIN_LSE, VDK_VIT_TRAIN_XM, VDK_VIT_TRAIN_Y2, VDK_VIT_TRAIN_R2, VDK_VIT_TRAIN_HPRE, VDK_VIT_TRAIN_HPOST, VDK_VIT_TRAIN_XO,
+  VDK_VIT_TRAIN_F1, VDK_VIT_TRAIN_RF1, VDK_VIT_TRAIN_F2, VDK_VIT_TRAIN_RF2, VDK_VIT_TRAIN_Z, VDK_VIT_TRAIN_ZSLAB,
+  VDK_VIT_TRAIN_BN_MEAN, VDK_VIT_TRAIN_BN_RSTD, VDK_VIT_TRAIN_DXA, VDK_VIT_TRAIN_DXB, VDK_VIT_TRAIN_DY, VDK_VIT_TRAIN_DBIG,
+  VDK_VIT_TRAIN_DZ, VDK_VIT_TRAIN_DZB, VDK_VIT_TRAIN_GW, VDK_VIT_TRAIN_WSLAB, VDK_VIT_TRAIN_DTOK, VDK_VIT_TRAIN_NUM_BUFFERS
+};
+int vdk_vit_train_buffer(const vdk_vit_net* net, int batch, int id, int index, size_t* offset, size_t* bytes);
 /* unit-test surface of the attention pair: forward that also saves the log2-domain log-sum-exp [batch, heads, tokens] (head_dim
  * 64, 72 or 80), and the backward dqkv = d(attention)/d(qkv) for d_out (both [batch, tokens, heads*64] bf16; head_dim 64 only). */
 int vdk_attention_fwd_lse(const void* qkv, int batch, int tokens, int heads, int head_dim, void* out, float* lse2, void* stream);

@@ -647,3 +647,123 @@ def batchnorm_bwd_bound(ref, weight, save_rstd, dw_init, db_init, out_dtype):
     e32 = (wr * inner + 3 * a * ref["dx"].abs()) * 1.01
     dxb = e32 + (0.5 * ulp(ref["dx"].abs() + e32, torch.bfloat16) if out_dtype == torch.bfloat16 else a * (ref["dx"].abs() + e32))
     return dxb, dw_b, db_b
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# wgmma GEMM (csrc/gemm.cu): accumulator, epilogues, split-K and the fused LayerNorm-backward epilogue
+
+# Documented accuracy of the fp16x2 activations (gemm.cu, include/vdk_b200.h).  test_gemm_gpu.py's sweeps run every finite
+# 16-bit pre-activation through them: on an H100 the worst GELU error was 4.3e-4 |x|, the worst GELU' error 7.6e-3 (near
+# |x| = 3, where the error of tanh.approx.f16 in 1 - tanh^2 is multiplied by x (c1 + 3 c3 x^2) ~ 5)
+GELU_REL_ERR = 6e-4     # |gelu~(x) - gelu(x)| <= GELU_REL_ERR |x|
+GELU_GRAD_ERR = 8e-3    # |gelu~'(x) - gelu'(x)| <= GELU_GRAD_ERR
+GELU_GRAD_MAX = 1.13    # max |gelu'(x)| = 1.1289...
+
+
+def gelu64(x):
+    return 0.5 * x * (1.0 + torch.special.erf(x / math.sqrt(2.0)))
+
+
+def gelu_grad64(x):
+    return 0.5 * (1.0 + torch.special.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
+
+
+def out_rounding(ref, dtype):
+    return torch.zeros_like(ref) if dtype == torch.float32 else ulp(ref, dtype)
+
+
+def acc_reference(a, b):
+    """fp64 A . B^T of the 16-bit operands and the fp32 accumulation bound (ceil(K/16) + 17) 2^-23 (|A| |B|^T)."""
+    A, Bm = a.double(), b.double()
+    K = A.shape[1]
+    return A @ Bm.t(), (-(-K // 16) + 17) * U32 * (A.abs() @ Bm.abs().t())
+
+
+def epilogue_reference(a, b, epilogue, out_dtype, bias=None, gamma=None, beta=None, residual=None, aux=None, ln_eps=1e-6):
+    """fp64 epilogue of the exact accumulator A . B^T (a [M, K], b [N, K]) and the elementwise bound of vdk_gemm's D.
+    Returns a dict with ref and bound, and with aux_ref / aux_bound when `aux` (the kernel's saved pre-activation of a
+    GELU epilogue) is given.
+
+      x = acc + bias in fp32:         |x~ - x| <= ex = e_acc + 2^-24 |x|  (no rounding without a bias)
+      NONE                            ref = x, bound ex
+      GELU                            ref = gelu(x), bound max|gelu'| ex + GELU_REL_ERR |x| + 2^-24 |ref|
+      GELU + aux_out                  aux: ref x, bound ex + ulp(x); out: ref gelu(aux), bound GELU_REL_ERR |aux| + 2^-24 |ref|
+      SCALE_RESIDUAL                  ref = res + gamma x, bound |gamma| ex + 2^-24 (|gamma x| + |ref|)
+      MUL_GELU_GRAD                   ref = acc gelu'(pre), bound (|gelu'(pre)| + GELU_GRAD_ERR) e_acc + GELU_GRAD_ERR |acc|
+                                      + 2^-24 |ref|
+      LAYERNORM (row of n = N values, E = max_j ex_j, r = 1/sqrt(var + eps), d_i = x_i - mean):
+        mean: ~n/4 sequential fp32 adds per thread, 2 shuffles, a divide: |dmean| <= E + (n/4 + 3) 2^-24 mean|x| = dm
+        d~_i off by D_i = ex_i + dm + 2^-24 |d_i|; the two-pass variance off by the relative
+        rho = (2 max D sqrt(var) + max D^2) / (var + eps) + (n/4 + 4) 2^-24, rsqrtf adds 2^-22:
+        bound |g_i| r D_i + |g_i d_i| r (rho / 2 + 2^-22) + 2^-24 (3 |g_i d_i| r + |ref|)
+    plus one ulp of a 16-bit output type at |ref| everywhere.
+    """
+    from visiondk_b200 import _lib
+    acc, e = acc_reference(a, b)
+    N = acc.shape[1]
+    x = acc + bias.double() if bias is not None else acc
+    ex = e + 2.0 ** -24 * x.abs() if bias is not None else e
+    out = {}
+    if epilogue == _lib.EPI_NONE:
+        ref, bound = x, ex
+    elif epilogue == _lib.EPI_GELU and aux is not None:
+        out["aux_ref"], out["aux_bound"] = x, ex + ulp(x, out_dtype)
+        pre = aux.double()
+        ref = gelu64(pre)
+        bound = GELU_REL_ERR * pre.abs() + 2.0 ** -24 * ref.abs()
+    elif epilogue == _lib.EPI_GELU:
+        ref = gelu64(x)
+        bound = GELU_GRAD_MAX * ex + GELU_REL_ERR * x.abs() + 2.0 ** -24 * ref.abs()
+    elif epilogue == _lib.EPI_SCALE_RESIDUAL:
+        g = gamma.double()
+        ref = residual.double() + g * x
+        bound = g.abs() * ex + 2.0 ** -24 * ((g * x).abs() + ref.abs())
+    elif epilogue == _lib.EPI_MUL_GELU_GRAD:
+        gp = gelu_grad64(residual.double())
+        ref = acc * gp
+        bound = (gp.abs() + GELU_GRAD_ERR) * e + GELU_GRAD_ERR * acc.abs() + 2.0 ** -24 * ref.abs()
+    elif epilogue == _lib.EPI_LAYERNORM:
+        mean = x.mean(1, keepdim=True)
+        dv = x - mean
+        var = (dv * dv).mean(1, keepdim=True)
+        r = 1.0 / torch.sqrt(var + ln_eps)
+        g, bt = gamma.double(), beta.double()
+        ref = dv * r * g + bt
+        E = ex.amax(1, keepdim=True)
+        dm = E + (N / 4 + 3) * 2.0 ** -24 * x.abs().mean(1, keepdim=True)
+        Di = ex + dm + 2.0 ** -24 * dv.abs()
+        Dmax = Di.amax(1, keepdim=True)
+        rho = (2 * Dmax * var.sqrt() + Dmax * Dmax) / (var + ln_eps) + (N / 4 + 4) * 2.0 ** -24
+        gd = (g * dv).abs()
+        bound = g.abs() * r * Di + gd * r * (rho / 2 + 2.0 ** -22) + 2.0 ** -24 * (3 * gd * r + ref.abs())
+    else:
+        raise ValueError(epilogue)
+    out["ref"], out["bound"] = ref, bound + out_rounding(ref, out_dtype)
+    return out
+
+
+def split_k_bound(a, b, n_split):
+    """Each split's partial is one wgmma chain over its K range; adding n_split partials (atomics or the slab sum) adds at most
+    n_split more roundings, each 2^-23 of the running |sum|: (ceil(K/16) + 17 + n_split) 2^-23 (|A| |B|^T).  At K = 12544 and
+    50176 the measured error is a few 1e-4 of this bound: the bound takes every one of the ~800 / ~3200 roundings at its maximum
+    and of one sign, and |A| |B|^T of random-sign operands exceeds |A B^T| by ~sqrt(K), while the rounding errors of the real
+    sums cancel like a random walk.  It stays the worst-case model; a lost or doubled split (one partial, ~sqrt(K / n_split)
+    times the operand scales) is still several times larger than it."""
+    A, Bm = a.double(), b.double()
+    return A @ Bm.t(), (-(-A.shape[1] // 16) + 17 + n_split) * U32 * (A.abs() @ Bm.abs().t())
+
+
+def fused_launch(M, N, G, sm):
+    """Summation depths of the fused LayerNorm-backward epilogue (VDK_EPI_LN_BWD) in ln_bwd_launch's terms
+    (layernorm_bwd_bound): a row group's sums chain 16 adds per 64-column box, G / 64 boxes and 2 shuffles (n1 = 8 IT +
+    log2 LPP with IT = G / 64, LPP = 4 covers it); a column sum chains 6 roundings per tile over a CTA's tiles, 8 warps and
+    the slab reduction's partials (8 groups)."""
+    BN = 256 if N % 256 == 0 else 128
+    num_n = N // BN
+    tiles = -(-M // 128) * num_n
+    # clusters (G > BN): at least half the SMs hold a co-resident cluster; fewer CTAs only lengthen the chains
+    slots = sm if G <= BN else sm // 2
+    grid = min(tiles, slots - slots % num_n)
+    per_cta = -(-tiles // grid)
+    parts = (grid // num_n) * (N // G)
+    return dict(lpp=4, it=G // 64, u=1, max_trips=6 * per_cta + 8 + -(-parts // 8) + 8, blocks=0, per_cta=per_cta)

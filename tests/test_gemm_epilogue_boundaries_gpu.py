@@ -15,8 +15,8 @@ import ctypes as C
 import pytest
 import torch
 
-from kernel_ref import check_within
-from test_gemm_gpu import E, check_epilogue, describe_tiles, operands, run, split_k_bound, tile_n
+from kernel_ref import check_within, split_k_bound
+from test_gemm_gpu import E, check_epilogue, describe_tiles, operands, run, tile_n
 from visiondk_b200 import _lib
 
 pytestmark = pytest.mark.gpu

@@ -9,12 +9,12 @@ device's SM count to give every CTA at least three tiles, and one case exactly S
 buffers (padding columns for ldd > N, trailing rows, a tail); a failure names the wrong tiles and the CTA that ran them.
 """
 import ctypes as C
-import math
 
 import pytest
 import torch
 
-from kernel_ref import U32, Guarded, check_within, ulp
+from kernel_ref import (GELU_GRAD_ERR, GELU_REL_ERR, Guarded, check_within, epilogue_reference, gelu64, gelu_grad64,
+                        split_k_bound, ulp)
 from visiondk_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -22,14 +22,6 @@ pytestmark = pytest.mark.gpu
 DT = {"bf16": (torch.bfloat16, _lib.DTYPE_BF16), "fp16": (torch.float16, _lib.DTYPE_FP16),
       "fp32": (torch.float32, _lib.DTYPE_FP32)}
 CODE = {torch.bfloat16: _lib.DTYPE_BF16, torch.float16: _lib.DTYPE_FP16, torch.float32: _lib.DTYPE_FP32}
-
-# Documented accuracy of the fp16x2 activations (gemm.cu, include/vdk_b200.h).  The sweeps below run every finite 16-bit
-# pre-activation through them: on an H100 the worst GELU error was 4.3e-4 |x|, the worst GELU' error 7.6e-3 (near |x| = 3, where
-# the error of tanh.approx.f16 in 1 - tanh^2 is multiplied by x (c1 + 3 c3 x^2) ~ 5)
-GELU_REL_ERR = 6e-4     # |gelu~(x) - gelu(x)| <= GELU_REL_ERR |x|
-GELU_GRAD_ERR = 8e-3    # |gelu~'(x) - gelu'(x)| <= GELU_GRAD_ERR
-GELU_GRAD_MAX = 1.13    # max |gelu'(x)| = 1.1289...
-
 
 def sm_count():
     return torch.cuda.get_device_properties(0).multi_processor_count
@@ -40,18 +32,6 @@ def tile_n(N, epilogue):
     if epilogue == _lib.EPI_LAYERNORM:
         wide = N > 128
     return 256 if wide else 128
-
-
-def gelu64(x):
-    return 0.5 * x * (1.0 + torch.special.erf(x / math.sqrt(2.0)))
-
-
-def gelu_grad64(x):
-    return 0.5 * (1.0 + torch.special.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
-
-
-def out_rounding(ref, dtype):
-    return torch.zeros_like(ref) if dtype == torch.float32 else ulp(ref, dtype)
 
 
 def describe_tiles(M, N, BN):
@@ -101,73 +81,18 @@ def run(a, b, out_dtype, epilogue=_lib.EPI_NONE, bias=None, gamma=None, beta=Non
     return d, ax
 
 
-def acc_reference(a, b):
-    """fp64 A . B^T of the 16-bit operands and the fp32 accumulation bound (ceil(K/16) + 17) 2^-23 (|A| |B|^T)."""
-    A, Bm = a.double(), b.double()
-    K = A.shape[1]
-    return A @ Bm.t(), (-(-K // 16) + 17) * U32 * (A.abs() @ Bm.abs().t())
-
-
 def check_epilogue(a, b, out_dtype, epilogue, d, ax, bias=None, gamma=None, beta=None, residual=None, ln_eps=1e-6, name=""):
-    """Compares D (and the saved pre-activation) with the fp64 epilogue of the exact accumulator.
-
-      x = acc + bias in fp32:         |x~ - x| <= ex = e_acc + 2^-24 |x|  (no rounding without a bias)
-      NONE                            ref = x, bound ex
-      GELU                            ref = gelu(x), bound max|gelu'| ex + GELU_REL_ERR |x| + 2^-24 |ref|
-      GELU + aux_out                  aux: ref x, bound ex + ulp(x); out: ref gelu(aux), bound GELU_REL_ERR |aux| + 2^-24 |ref|
-      SCALE_RESIDUAL                  ref = res + gamma x, bound |gamma| ex + 2^-24 (|gamma x| + |ref|)
-      MUL_GELU_GRAD                   ref = acc gelu'(pre), bound (|gelu'(pre)| + GELU_GRAD_ERR) e_acc + GELU_GRAD_ERR |acc|
-                                      + 2^-24 |ref|
-      LAYERNORM (row of n = N values, E = max_j ex_j, r = 1/sqrt(var + eps), d_i = x_i - mean):
-        mean: ~n/4 sequential fp32 adds per thread, 2 shuffles, a divide: |dmean| <= E + (n/4 + 3) 2^-24 mean|x| = dm
-        d~_i off by D_i = ex_i + dm + 2^-24 |d_i|; the two-pass variance off by the relative
-        rho = (2 max D sqrt(var) + max D^2) / (var + eps) + (n/4 + 4) 2^-24, rsqrtf adds 2^-22:
-        bound |g_i| r D_i + |g_i d_i| r (rho / 2 + 2^-22) + 2^-24 (3 |g_i d_i| r + |ref|)
-    plus one ulp of a 16-bit output type at |ref| everywhere.
-    """
+    """Compares D (and the saved pre-activation) with the fp64 epilogue of the exact accumulator, within
+    kernel_ref.epilogue_reference's bounds."""
     M, N = d.view.shape
-    acc, e = acc_reference(a, b)
-    bias64 = bias.double() if bias is not None else torch.zeros(N, dtype=torch.float64, device=acc.device)
-    x = acc + bias64
-    ex = e + (2.0 ** -24 * x.abs() if bias is not None else 0.0)
     describe = describe_tiles(M, N, tile_n(N, epilogue))
+    r = epilogue_reference(a, b, epilogue, out_dtype, bias=bias, gamma=gamma, beta=beta, residual=residual,
+                           aux=ax.view if ax is not None else None, ln_eps=ln_eps)
+    if ax is not None:
+        check_within(ax.view, r["aux_ref"], r["aux_bound"], f"{name} aux", describe)
     got = d.view.double()
-    if epilogue == _lib.EPI_NONE:
-        ref, bound = x, ex
-    elif epilogue == _lib.EPI_GELU and ax is not None:
-        check_within(ax.view, x, ex + ulp(x, out_dtype), f"{name} aux", describe)
-        pre = ax.view.double()
-        ref = gelu64(pre)
-        bound = GELU_REL_ERR * pre.abs() + 2.0 ** -24 * ref.abs()
-    elif epilogue == _lib.EPI_GELU:
-        ref = gelu64(x)
-        bound = GELU_GRAD_MAX * ex + GELU_REL_ERR * x.abs() + 2.0 ** -24 * ref.abs()
-    elif epilogue == _lib.EPI_SCALE_RESIDUAL:
-        g = gamma.double()
-        ref = residual.double() + g * x
-        bound = g.abs() * ex + 2.0 ** -24 * ((g * x).abs() + ref.abs())
-    elif epilogue == _lib.EPI_MUL_GELU_GRAD:
-        gp = gelu_grad64(residual.double())
-        ref = acc * gp
-        bound = (gp.abs() + GELU_GRAD_ERR) * e + GELU_GRAD_ERR * acc.abs() + 2.0 ** -24 * ref.abs()
-    elif epilogue == _lib.EPI_LAYERNORM:
-        mean = x.mean(1, keepdim=True)
-        dv = x - mean
-        var = (dv * dv).mean(1, keepdim=True)
-        r = 1.0 / torch.sqrt(var + ln_eps)
-        g, bt = gamma.double(), beta.double()
-        ref = dv * r * g + bt
-        E = ex.amax(1, keepdim=True) if torch.is_tensor(ex) else torch.zeros_like(mean)
-        dm = E + (N / 4 + 3) * 2.0 ** -24 * x.abs().mean(1, keepdim=True)
-        Di = ex + dm + 2.0 ** -24 * dv.abs()
-        Dmax = Di.amax(1, keepdim=True)
-        rho = (2 * Dmax * var.sqrt() + Dmax * Dmax) / (var + ln_eps) + (N / 4 + 4) * 2.0 ** -24
-        gd = (g * dv).abs()
-        bound = g.abs() * r * Di + gd * r * (rho / 2 + 2.0 ** -22) + 2.0 ** -24 * (3 * gd * r + ref.abs())
-    else:
-        raise ValueError(epilogue)
-    check_within(got, ref, bound + out_rounding(ref, out_dtype), f"{name} D", describe)
-    return got, ref
+    check_within(got, r["ref"], r["bound"], f"{name} D", describe)
+    return got, r["ref"]
 
 
 def operands(M, N, K, in_dtype, seed, a_scale=1.0, b_scale=1.0):
@@ -243,17 +168,6 @@ def test_gemm_transposed_storage(lib, ta, tb, M, N, K):
     a, b = operands(M, N, K, "bf16", M + N + K + ta * 2 + tb)
     d, _ = run(a, b, torch.float32, ta=ta, tb=tb)
     check_epilogue(a, b, torch.float32, _lib.EPI_NONE, d, None, name="transposed")
-
-
-def split_k_bound(a, b, n_split):
-    """Each split's partial is one wgmma chain over its K range; adding n_split partials (atomics or the slab sum) adds at most
-    n_split more roundings, each 2^-23 of the running |sum|: (ceil(K/16) + 17 + n_split) 2^-23 (|A| |B|^T).  At K = 12544 and
-    50176 the measured error is a few 1e-4 of this bound: the bound takes every one of the ~800 / ~3200 roundings at its maximum
-    and of one sign, and |A| |B|^T of random-sign operands exceeds |A B^T| by ~sqrt(K), while the rounding errors of the real
-    sums cancel like a random walk.  It stays the worst-case model; a lost or doubled split (one partial, ~sqrt(K / n_split)
-    times the operand scales) is still several times larger than it."""
-    A, Bm = a.double(), b.double()
-    return A @ Bm.t(), (-(-A.shape[1] // 16) + 17 + n_split) * U32 * (A.abs() @ Bm.abs().t())
 
 
 def test_gemm_wgrad_form_split_k(lib):

@@ -8,8 +8,8 @@ import ctypes as C
 import pytest
 import torch
 
-from kernel_ref import (bf16_store_bound, check_within, layernorm_bwd_bound, layernorm_bwd_dgamma, layernorm_bwd_reference,
-                        ln_bwd_launch)
+from kernel_ref import (bf16_store_bound, check_within, fused_launch, layernorm_bwd_bound, layernorm_bwd_dgamma,
+                        layernorm_bwd_reference, ln_bwd_launch)
 from visiondk_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -23,21 +23,6 @@ def sm_count():
 def gemm_desc(A, Bw, D, M, N, K, epi, **kw):
     return _lib.GemmDesc(A=A.data_ptr(), B=Bw.data_ptr(), D=D.data_ptr(), M=M, N=N, K=K, lda=K, ldb=N, ldd=N,
                          in_dtype=_lib.DTYPE_BF16, out_dtype=_lib.DTYPE_BF16, epilogue=epi, split_k=1, trans_b=1, **kw)
-
-
-def fused_launch(M, N, G, sm):
-    """Summation depths of the fused epilogue in ln_bwd_launch's terms (layernorm_bwd_bound): a row group's sums chain
-    16 adds per 64-column box, G / 64 boxes and 2 shuffles (n1 = 8 IT + log2 LPP with IT = G / 64, LPP = 4 covers it); a
-    column sum chains 6 roundings per tile over a CTA's tiles, 8 warps and the slab reduction's partials (8 groups)."""
-    BN = 256 if N % 256 == 0 else 128
-    num_n = N // BN
-    tiles = -(-M // 128) * num_n
-    # clusters (G > BN): at least half the SMs hold a co-resident cluster; fewer CTAs only lengthen the chains
-    slots = sm if G <= BN else sm // 2
-    grid = min(tiles, slots - slots % num_n)
-    per_cta = -(-tiles // grid)
-    parts = (grid // num_n) * (N // G)
-    return dict(lpp=4, it=G // 64, u=1, max_trips=6 * per_cta + 8 + -(-parts // 8) + 8, blocks=0, per_cta=per_cta)
 
 
 def ln_problem(P, G, seed):

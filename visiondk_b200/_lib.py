@@ -191,6 +191,7 @@ SIGNATURES = {
     "vdk_convnext_train_backward": (_i, [_p, _p, _p, _p, _i, _p, _sz, _p]),
     "vdk_convnext_train_backward_units": (_i, [_p]),
     "vdk_convnext_train_backward_range": (_i, [_p, _p, _p, _p, _i, _p, _sz, _p, _i, _i]),
+    "vdk_convnext_train_buffer": (_i, [_p, _i, _i, _i, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "vdk_vit_workspace_bytes": (_sz, [_p, _i]),
     "vdk_vit_pack": (_i, [_p, _p, _p]),
     "vdk_vit_train_workspace_bytes": (_sz, [_p, _i]),
@@ -198,6 +199,7 @@ SIGNATURES = {
     "vdk_vit_train_backward": (_i, [_p, _p, _p, _p, _i, _p, _sz, _p]),
     "vdk_vit_train_backward_units": (_i, [_p]),
     "vdk_vit_train_backward_range": (_i, [_p, _p, _p, _p, _i, _p, _sz, _p, _i, _i]),
+    "vdk_vit_train_buffer": (_i, [_p, _i, _i, _i, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "vdk_attention_fwd_lse": (_i, [_p, _i, _i, _i, _i, _p, _p, _p]),
     "vdk_attention_bwd": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p, _p]),
     "vdk_vit_forward": (_i, [_p, _p, _i, _i, _p, _p, _sz, _p]),

@@ -31,19 +31,19 @@ struct TrainLayout {
   StageDims st[4];
   int depth[4];
   int n_blocks;
-  size_t p0, z0, rstd0;                                        // stem: patch rows [M0,48], pre-LN output, 1/sigma
-  size_t xs[4][VDK_CONVNEXT_MAX_BLOCKS + 1];                   // residual stream at every node of a stage
-  size_t y[VDK_CONVNEXT_MAX_BLOCKS], rstd[VDK_CONVNEXT_MAX_BLOCKS];
-  size_t hpre[VDK_CONVNEXT_MAX_BLOCKS], hpost[VDK_CONVNEXT_MAX_BLOCKS];
-  size_t patch[4], prstd[4];                                   // downsample: LayerNorm'ed 2x2 patch rows, 1/sigma
-  size_t f, frstd, fn, bn2_mean, bn2_rstd, z, zslab, bn1_mean, bn1_rstd;
-  size_t dxa, dxb, dy, dconv, G, sdo, dw49, gwc, gwneck, dz, dzb, dfn, wslab;
+  WsRange p0, z0, rstd0;                                       // stem: patch rows [M0,48], pre-LN output, 1/sigma
+  WsRange xs[4][VDK_CONVNEXT_MAX_BLOCKS + 1];                  // residual stream at every node of a stage
+  WsRange y[VDK_CONVNEXT_MAX_BLOCKS], rstd[VDK_CONVNEXT_MAX_BLOCKS];
+  WsRange hpre[VDK_CONVNEXT_MAX_BLOCKS], hpost[VDK_CONVNEXT_MAX_BLOCKS];
+  WsRange patch[4], prstd[4];                                  // downsample: LayerNorm'ed 2x2 patch rows, 1/sigma
+  WsRange f, frstd, fn, bn2_mean, bn2_rstd, z, zslab, bn1_mean, bn1_rstd;
+  WsRange dxa, dxb, dy, dconv, G, sdo, dw49, gwc, gwneck, dz, dzb, dfn, wslab;
   size_t total;
 };
 
 static void make_layout(const vdk_convnext_net* net, int batch, TrainLayout* L) {
   size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += al(bytes); return o; };
+  auto take = [&](size_t bytes) { WsRange r{off, bytes}; off += al(bytes); return r; };
   int H = net->image_size / 4, W = H;
   L->n_blocks = 0;
   for (int s = 0; s < 4; ++s) {
@@ -204,6 +204,33 @@ extern "C" size_t vdk_convnext_train_workspace_bytes(const vdk_convnext_net* net
   TrainLayout L;
   make_layout(net, batch, &L);
   return L.total;
+}
+
+extern "C" int vdk_convnext_train_buffer(const vdk_convnext_net* net, int batch, int id, int index, size_t* offset, size_t* bytes) {
+  VDK_REQUIRE(net && batch > 1 && offset && bytes, "vdk_convnext_train_buffer: bad arguments");
+  TrainLayout L;
+  make_layout(net, batch, &L);
+  const WsRange* one[] = {&L.p0, &L.z0, &L.rstd0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &L.f, &L.frstd,
+                          &L.fn, &L.bn2_mean, &L.bn2_rstd, &L.z, &L.zslab, &L.bn1_mean, &L.bn1_rstd, &L.dxa, &L.dxb, &L.dy, &L.dconv,
+                          &L.G, &L.sdo, &L.dw49, &L.gwc, &L.gwneck, &L.dz, &L.dzb, &L.dfn, &L.wslab};
+  static_assert(sizeof(one) / sizeof(one[0]) == VDK_CONVNEXT_TRAIN_NUM_BUFFERS, "one entry per buffer id");
+  VDK_REQUIRE(id >= 0 && id < VDK_CONVNEXT_TRAIN_NUM_BUFFERS, "vdk_convnext_train_buffer: unknown buffer id %d", id);
+  const WsRange* r = one[id];
+  if (id == VDK_CONVNEXT_TRAIN_XS) {
+    const int st = index / (VDK_CONVNEXT_MAX_BLOCKS + 1), j = index % (VDK_CONVNEXT_MAX_BLOCKS + 1);
+    VDK_REQUIRE(index >= 0 && st < 4 && j <= L.depth[st], "vdk_convnext_train_buffer: no residual-stream node %d", index);
+    r = &L.xs[st][j];
+  } else if (id == VDK_CONVNEXT_TRAIN_PATCH || id == VDK_CONVNEXT_TRAIN_PRSTD) {
+    VDK_REQUIRE(index >= 1 && index < 4, "vdk_convnext_train_buffer: no downsample in stage %d", index);
+    r = id == VDK_CONVNEXT_TRAIN_PATCH ? &L.patch[index] : &L.prstd[index];
+  } else if (r == nullptr) {
+    VDK_REQUIRE(index >= 0 && index < L.n_blocks, "vdk_convnext_train_buffer: no block %d", index);
+    const WsRange* per_block[] = {L.y, L.rstd, L.hpre, L.hpost};
+    r = &per_block[id - VDK_CONVNEXT_TRAIN_Y][index];
+  }
+  *offset = r->off;
+  *bytes = r->bytes;
+  return VDK_OK;
 }
 
 // ---- weight packing, batched: the blocks of a stage have identical shapes, so ONE launch per (stage, kind) walks a table

@@ -27,6 +27,12 @@ inline size_t wgrad_slab_bytes(int M, int N, size_t K) {
   return static_cast<size_t>(std::max(2, wgrad_splits(M, N, K))) * M * (static_cast<size_t>(N) + 1) * 4;
 }
 
+// one buffer of a train workspace: its byte offset, which the kernels index with, and its size (vdk_*_train_buffer)
+struct WsRange {
+  size_t off = 0, bytes = 0;
+  operator size_t() const { return off; }
+};
+
 struct Gemm {
   cudaStream_t s;
   int run(const void* A, const void* B, void* D, int M, int N, int K, int lda, int ldb, int ldd, int epi, const float* bias,

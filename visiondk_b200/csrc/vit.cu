@@ -503,12 +503,12 @@ namespace vdk {
 struct VitTrainLayout {
   int N, T, C, Kp, depth;
   size_t M;
-  size_t rows, x0;                                   // patch rows [B*N, Kp], x after patch embed + cls + pos
-  size_t y1[VDK_VIT_MAX_BLOCKS], r1[VDK_VIT_MAX_BLOCKS], qkv[VDK_VIT_MAX_BLOCKS], att[VDK_VIT_MAX_BLOCKS], lse[VDK_VIT_MAX_BLOCKS];
-  size_t xm[VDK_VIT_MAX_BLOCKS], y2[VDK_VIT_MAX_BLOCKS], r2[VDK_VIT_MAX_BLOCKS], hpre[VDK_VIT_MAX_BLOCKS], hpost[VDK_VIT_MAX_BLOCKS];
-  size_t xo[VDK_VIT_MAX_BLOCKS];                     // block outputs (residual stream)
-  size_t f1, rf1, f2, rf2, z, zslab, bn_mean, bn_rstd;
-  size_t dxa, dxb, dy, dbig, dz, dzb, gw, wslab, tok, dtok;
+  WsRange rows, x0;                                  // patch rows [B*N, Kp], x after patch embed + cls + pos
+  WsRange y1[VDK_VIT_MAX_BLOCKS], r1[VDK_VIT_MAX_BLOCKS], qkv[VDK_VIT_MAX_BLOCKS], att[VDK_VIT_MAX_BLOCKS], lse[VDK_VIT_MAX_BLOCKS];
+  WsRange xm[VDK_VIT_MAX_BLOCKS], y2[VDK_VIT_MAX_BLOCKS], r2[VDK_VIT_MAX_BLOCKS], hpre[VDK_VIT_MAX_BLOCKS], hpost[VDK_VIT_MAX_BLOCKS];
+  WsRange xo[VDK_VIT_MAX_BLOCKS];                    // block outputs (residual stream)
+  WsRange f1, rf1, f2, rf2, z, zslab, bn_mean, bn_rstd;
+  WsRange dxa, dxb, dy, dbig, dz, dzb, gw, wslab, tok, dtok;
   size_t total;
 };
 
@@ -522,7 +522,7 @@ static int vit_train_layout(const vdk_vit_net* n, int batch, VitTrainLayout* L) 
   L->N = base.N; L->T = base.T; L->C = base.C; L->Kp = base.Kp; L->M = base.M; L->depth = n->depth;
   const size_t M = L->M, C = L->C, F = n->feat_dim;
   size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += up256v(bytes); return o; };
+  auto take = [&](size_t bytes) { WsRange r{off, bytes}; off += up256v(bytes); return r; };
   L->rows = take(static_cast<size_t>(batch) * L->N * L->Kp * 2);
   L->tok = take(static_cast<size_t>(batch) * L->N * C * 2);
   L->x0 = take(M * C * 2);
@@ -619,6 +619,27 @@ extern "C" size_t vdk_vit_train_workspace_bytes(const vdk_vit_net* net, int batc
   VitTrainLayout L;
   if (!net || batch <= 1 || refuse_inference_only_features(net) != VDK_OK || vit_train_layout(net, batch, &L) != VDK_OK) return 0;
   return L.total;
+}
+
+extern "C" int vdk_vit_train_buffer(const vdk_vit_net* net, int batch, int id, int index, size_t* offset, size_t* bytes) {
+  VDK_REQUIRE(net && offset && bytes, "vdk_vit_train_buffer: null argument");
+  RC(refuse_inference_only_features(net));
+  VitTrainLayout L;
+  RC(vit_train_layout(net, batch, &L));
+  const WsRange* one[] = {&L.rows, &L.tok, &L.x0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                          nullptr, nullptr, &L.f1, &L.rf1, &L.f2, &L.rf2, &L.z, &L.zslab, &L.bn_mean, &L.bn_rstd, &L.dxa, &L.dxb,
+                          &L.dy, &L.dbig, &L.dz, &L.dzb, &L.gw, &L.wslab, &L.dtok};
+  static_assert(sizeof(one) / sizeof(one[0]) == VDK_VIT_TRAIN_NUM_BUFFERS, "one entry per buffer id");
+  VDK_REQUIRE(id >= 0 && id < VDK_VIT_TRAIN_NUM_BUFFERS, "vdk_vit_train_buffer: unknown buffer id %d", id);
+  const WsRange* r = one[id];
+  if (r == nullptr) {
+    VDK_REQUIRE(index >= 0 && index < net->depth, "vdk_vit_train_buffer: no block %d", index);
+    const WsRange* per_block[] = {L.y1, L.r1, L.qkv, L.att, L.lse, L.xm, L.y2, L.r2, L.hpre, L.hpost, L.xo};
+    r = &per_block[id - VDK_VIT_TRAIN_Y1][index];
+  }
+  *offset = r->off;
+  *bytes = r->bytes;
+  return VDK_OK;
 }
 
 static int refuse_pre_norm(const vdk_vit_net* net) {
