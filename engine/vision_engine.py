@@ -94,6 +94,7 @@ def check(task: str, cfgs: dict) -> None:
 class CenterProcessor:
     def __init__(self, cfgs: dict, rank: int, project: Optional[str] = None, train: bool = True, opt=None):
         self.cfgs, self.rank, self.project, self.opt = cfgs, rank, project, opt
+        self._gathered_head_state: Optional[dict] = None  # a class-sharded trainer's full head state for the next save
         self.model_cfg, self.data_cfg, self.hyp_cfg = cfgs["model"], cfgs["data"], cfgs["hyp"]
         self.task = self.model_cfg["task"]
         if self.task not in ("face", "cbir"):
@@ -137,9 +138,20 @@ class CenterProcessor:
     def _resume(self, trainer: FaceTrainer, path: str) -> int:
         """Restores everything the reference's checkpoint carries (:494-507: model, EMA + `updates`, optimizer, scheduler) and
         what it forgets (the head's class weights are not in its `state_dict` entry): backbone + head weights, EMA copies,
-        momentum buffers, step counters, the position in the LR schedule and the post-warm-up momentum."""
+        momentum buffers, step counters, the position in the LR schedule and the post-warm-up momentum.  Checkpoints hold the
+        full head in either mode: a class-sharded trainer loads this rank's columns of it."""
         ckpt = torch.load(path, map_location="cpu", weights_only=False)
-        wrap = self.model.trainingwrapper
+        self.restore_checkpoint(trainer, ckpt)
+        start_epoch = ckpt["epoch"] + 1
+        if start_epoch > self.hyp_cfg["warm_ep"]:  # the `epoch == warm_ep` switch below has already happened
+            trainer.set_momentum(self.hyp_cfg["momentum"])
+        self.log(f"resume: {path}")
+        return start_epoch
+
+    @staticmethod
+    def restore_checkpoint(trainer: FaceTrainer, ckpt: dict) -> None:
+        """Model, head, EMA copies and trainer state of an Epoch_N.pt dict, in place."""
+        wrap = trainer.model.trainingwrapper
         wrap["backbone"].load_state_dict(ckpt["state_dict"], strict=True)  # in place: the parameters live in the flat buffers
         if "head" in ckpt:
             wrap["head"].load_state_dict(ckpt["head"], strict=True)
@@ -148,11 +160,6 @@ class CenterProcessor:
             if "ema_head" in ckpt:
                 trainer.ema.trainingwrapper["head"].load_state_dict(ckpt["ema_head"], strict=True)
         trainer.load_state_dict({"optimizer": ckpt["optimizer"], "scheduler": ckpt["scheduler"], "updates": ckpt["updates"]})
-        start_epoch = ckpt["epoch"] + 1
-        if start_epoch > self.hyp_cfg["warm_ep"]:  # the `epoch == warm_ep` switch below has already happened
-            trainer.set_momentum(self.hyp_cfg["momentum"])
-        self.log(f"resume: {path}")
-        return start_epoch
 
     def run_embedding(self, resume: Optional[str] = None):
         hyp = self.hyp_cfg
@@ -162,10 +169,11 @@ class CenterProcessor:
             raise NotImplementedError("the H100 step implements sgd + cosine_with_warm (the faceX / cbir configs)")
         if self.model_cfg.get("load_from"):
             self._load_from(self.model_cfg["load_from"])
+        shard_head = bool(getattr(self.opt, "shard_head", False))
         trainer = FaceTrainer(self.model, lr0=hyp["lr0"], momentum=hyp["warmup_momentum"], weight_decay=hyp["weight_decay"],
                               label_smooth=hyp.get("label_smooth", 0.0), layer_wise=layer_wise,
                               warm_steps=hyp["warm_ep"] * steps_per_epoch, total_steps=hyp["epochs"] * steps_per_epoch,
-                              lrf_ratio=hyp.get("lrf_ratio"), use_ema=self.rank in (-1, 0))
+                              lrf_ratio=hyp.get("lrf_ratio"), use_ema=self.rank in (-1, 0) or shard_head, shard_head=shard_head)
         start_epoch = self._resume(trainer, resume) if resume else 0
         t0 = time.time()
         save_freq = getattr(self.opt, "save_freq", 1) if self.opt else 1
@@ -182,15 +190,46 @@ class CenterProcessor:
                              f"loss {running.item() / n:.4f}")
                     running.zero_()
                     n = 0
+            if shard_head and (epoch + 1) % save_freq == 0:  # gathering the head's shards is a collective: every rank joins
+                self._gathered_head_state = self.gathered_head_state(trainer)
             if self.rank in (-1, 0) and (epoch + 1) % save_freq == 0:
                 self.save_and_eval(trainer, epoch, steps_per_epoch)
+            self._gathered_head_state = None
         self.log(f"Training complete ({(time.time() - t0) / 3600:.3f} hours)")
         return trainer
+
+    @staticmethod
+    def gathered_head_state(trainer: FaceTrainer) -> dict:
+        """The full head, EMA head and trainer state of a class-sharded trainer (a collective: every rank must call it), in
+        the unsharded layout save_and_eval writes."""
+        host = lambda sd: {k: v.detach().cpu().clone() for k, v in sd.items()}
+        src = trainer.ema if trainer.ema is not None else trainer.model
+        return {"head": host(trainer.model.trainingwrapper["head"].state_dict()),
+                "ema_head": host(src.trainingwrapper["head"].state_dict()), "trainer": trainer.state_dict()}
+
+    @staticmethod
+    def checkpoint(trainer: FaceTrainer, epoch: int, steps_per_epoch: int, fitness: dict, full: Optional[dict] = None) -> dict:
+        """The Epoch_N.pt dict: the reference's key set plus 'head', 'ema_head' and the momentum buffers, always in the
+        unsharded layout (`full`: gathered_head_state of a class-sharded trainer)."""
+        wrap = trainer.model.trainingwrapper
+        src = trainer.ema if trainer.ema is not None else trainer.model
+        state = trainer.state_dict() if full is None else full["trainer"]
+
+        def host(sd):  # parameters are views into the optimizer's flat buffers: save compact per-tensor copies
+            return {k: v.detach().cpu().clone() for k, v in sd.items()}
+
+        return {"epoch": epoch, "batch_id": steps_per_epoch - 1, "fitness": fitness,
+                "state_dict": host(wrap["backbone"].state_dict()), "ema": host(src.trainingwrapper["backbone"].state_dict()),
+                "head": host(wrap["head"].state_dict()) if full is None else full["head"],
+                "ema_head": host(src.trainingwrapper["head"].state_dict()) if full is None else full["ema_head"],
+                "updates": state["updates"], "optimizer": state["optimizer"], "scheduler": state["scheduler"]}
 
     def save_and_eval(self, trainer: FaceTrainer, epoch: int, steps_per_epoch: int):
         """engine/procedure/train.py:244-278: evaluate the EMA backbone (face: pair verification -> Val_mean / Val_std; cbir:
         valuate_cbir -> {metric: float}), write Epoch_N.pt with
-        the reference's key set, plus the entries a faithful resume needs ('head', 'ema_head', momentum buffers)."""
+        the reference's key set, plus the entries a faithful resume needs ('head', 'ema_head', momentum buffers).
+        A class-sharded trainer's full head state is gathered on every rank before this rank-0-only call
+        (`_gathered_head_state`, set by run_embedding)."""
         src = trainer.ema if trainer.ema is not None else self.model
         ema_backbone = src.trainingwrapper["backbone"]
         if self.task == "face":  # train.py:246-253: 10-fold pair verification of the EMA backbone
@@ -204,16 +243,7 @@ class CenterProcessor:
         fitness = {"fitness": metrics, "checkpoint": f"Epoch_{epoch + 1}.pt"}
         out_dir = Path(self.project or "run/exp")
         out_dir.mkdir(parents=True, exist_ok=True)
-        wrap = self.model.trainingwrapper
-        state = trainer.state_dict()
-
-        def host(sd):  # parameters are views into the optimizer's flat buffers: save compact per-tensor copies
-            return {k: v.detach().cpu().clone() for k, v in sd.items()}
-
-        ckpt = {"epoch": epoch, "batch_id": steps_per_epoch - 1, "fitness": fitness,
-                "state_dict": host(wrap["backbone"].state_dict()), "ema": host(ema_backbone.state_dict()),
-                "head": host(wrap["head"].state_dict()), "ema_head": host(src.trainingwrapper["head"].state_dict()),
-                "updates": state["updates"], "optimizer": state["optimizer"], "scheduler": state["scheduler"]}
+        ckpt = self.checkpoint(trainer, epoch, steps_per_epoch, fitness, self._gathered_head_state)
         torch.save(ckpt, out_dir / f"Epoch_{epoch + 1}.pt")
         self.log(str(fitness))
         return fitness

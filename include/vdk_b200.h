@@ -783,6 +783,42 @@ int vdk_head_backward(const vdk_head_desc* d, const float* feats, const float* w
                       const float* row_lse, const float* grad_loss, const float* dlogits, float* dfeats,
                       float* dweight, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Class-sharded head: rank `rank` of `world` holds the columns [class_offset, class_offset + d->num_class) of a head with
+ * num_class_total classes, and every rank sees the same N = d->batch gathered rows (world equal batches of N / world, in rank
+ * order) with GLOBAL labels.  The per-element arithmetic is the unsharded head's; with world = 1 and the whole head the five
+ * calls below give vdk_head_forward / vdk_head_backward's results bit for bit.  Workspace: vdk_head_workspace_bytes(d), the
+ * same buffer through one step (shard_forward reads the cosines shard_cos left in it, shard_finalize the normalised
+ * features shard_backward left in it).  Label smoothing divides by num_class_total. */
+typedef struct vdk_head_shard {
+  int class_offset;     /* first class of this shard */
+  int num_class_total;  /* C of the whole head (> 1); d->num_class is the shard's width (>= 1) */
+  int world, rank;      /* d->batch is a multiple of world; this rank's own rows are [rank, rank + 1) * d->batch / world */
+} vdk_head_shard;
+/* sizeof(vdk_head_shard) (vdk_struct_sizes' contract for it). */
+int vdk_head_shard_struct_sizes(size_t* out, int n);
+/* 1. cos of the shard's columns into the workspace; label_cos fp32 [N]: the label column's cos where this shard owns the
+ *    label, else 0 (summed over the ranks it is every row's label cos, which MV-Softmax needs before any logit). */
+int vdk_head_shard_cos(const vdk_head_desc* d, const vdk_head_shard* s, const float* feats, const float* weight,
+                       const int64_t* labels, float* label_cos, void* workspace, size_t workspace_bytes, void* stream);
+/* 2. logits of the shard and per-row partials fp32 [N, 4]: (max z, sum exp(z - max), sum z, label z or 0).  label_cos: the
+ *    rank-summed label cosines (MV-Softmax only; may be NULL otherwise).  logits / cos_saved: fp32 [N, d->num_class] or NULL. */
+int vdk_head_shard_forward(const vdk_head_desc* d, const vdk_head_shard* s, const int64_t* labels, const float* label_cos,
+                           float* logits, float* cos_saved, float* partials, void* workspace, size_t workspace_bytes,
+                           void* stream);
+/* 3. partials of every rank fp32 [world, N, 4] -> row_lse [N], row_loss [N] (CE with smoothing over num_class_total) and
+ *    loss (device scalar): the mean of row_loss over this rank's own rows. */
+int vdk_head_shard_combine(const vdk_head_desc* d, const vdk_head_shard* s, const float* partials, float* row_lse,
+                           float* row_loss, float* loss, void* stream);
+/* 4. dweight fp32 [D, d->num_class]: the gradient of the mean CE over all N rows (the rank-average of the per-rank losses'
+ *    gradients); dfn fp32 [N, D]: this shard's part of d(loss_r)/d(normalised features) for every row, with each rank's
+ *    loss the mean over its own rows (to be summed over the ranks).  grad_loss: device scalar or NULL for 1. */
+int vdk_head_shard_backward(const vdk_head_desc* d, const vdk_head_shard* s, const float* feats, const float* weight,
+                            const int64_t* labels, const float* label_cos, const float* row_lse, const float* grad_loss,
+                            float* dfn, float* dweight, void* workspace, size_t workspace_bytes, void* stream);
+/* 5. dfn summed over the ranks fp32 [N, D] -> dfeats fp32 [N / world, D] of this rank's own rows (normalisation backward). */
+int vdk_head_shard_finalize(const vdk_head_desc* d, const vdk_head_shard* s, const float* dfn, float* dfeats,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- optimizer step -------------------------------------------------------------------------- */
 /* Replaces Trainer.update's clip_grad_norm_(max_norm=10) -> SGD step -> zero_grad -> ModelEMA.update
  * (engine/procedure/train.py:203-215, engine/optimizer.py:119-121, models/ema.py:28-37) on FLAT fp32 buffers

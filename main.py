@@ -30,6 +30,9 @@ def parse_opt():
     ap.add_argument("--local_rank", type=int, default=-1)
     ap.add_argument("--print_freq", type=int, default=50)
     ap.add_argument("--save_freq", type=int, default=1)
+    ap.add_argument("--shard_head", action="store_true",
+                    help="split the margin head's classes over the ranks (each holds and updates C/W columns; checkpoints keep "
+                         "the full head)")
     return ap.parse_args()
 
 

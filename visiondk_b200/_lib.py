@@ -28,6 +28,10 @@ class HeadDesc(C.Structure):
                 ("mv_weight", C.c_float), ("is_am", C.c_int)]
 
 
+class HeadShard(C.Structure):
+    _fields_ = [("class_offset", C.c_int), ("num_class_total", C.c_int), ("world", C.c_int), ("rank", C.c_int)]
+
+
 class TopkPlan(C.Structure):
     _fields_ = [
         ("n_query", C.c_int64),
@@ -209,6 +213,12 @@ SIGNATURES = {
     "vdk_head_workspace_bytes": (_sz, [_p]),
     "vdk_head_forward": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "vdk_head_backward": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "vdk_head_shard_struct_sizes": (_i, [_p, _i]),
+    "vdk_head_shard_cos": (_i, [_p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "vdk_head_shard_forward": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "vdk_head_shard_combine": (_i, [_p, _p, _p, _p, _p, _p, _p]),
+    "vdk_head_shard_backward": (_i, [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "vdk_head_shard_finalize": (_i, [_p, _p, _p, _p, _p, _sz, _p]),
     "vdk_grad_sumsq_workspace_bytes": (_sz, []),
     "vdk_grad_sumsq": (_i, [_p, _i64, _p, _i, _p, _sz, _p]),
     "vdk_sgd_clip_ema_step": (_i, [_p, _p, _p, _p, _i64, _p, C.c_float, C.c_float, C.c_float, C.c_float, _i, C.c_float,

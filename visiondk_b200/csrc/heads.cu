@@ -205,16 +205,24 @@ __device__ __forceinline__ void head_logit(const HeadCfg& h, const MvRow& mv, fl
   dz_dcos = clamp_pass ? d : 0.f;
 }
 
-// forward: one CTA per row; online softmax over the classes; optional logits output
+// CE with label smoothing over Ctot classes: (1-e) * (lse - z_y) + e * (lse - mean_c z)
+__device__ __forceinline__ float ce_row_loss(const HeadCfg& h, float lse, float ZY, float Z, int Ctot) {
+  return (1.f - h.label_smooth) * (lse - ZY) + h.label_smooth * (lse - Z / static_cast<float>(Ctot));
+}
+
+// forward: one CTA per row; online softmax over the classes; optional logits output.  A class shard passes its first class
+// c_off, the whole head's Ctot, the label cosines gt (MV-Softmax, whose label column may live on another shard) and
+// `partials`, which then receives the row's (max, sumexp, sum z, label z) instead of row_lse / row_loss.
 __global__ void __launch_bounds__(256)
-margin_ce_fwd_kernel(const float* __restrict__ cosm, int ldc, int B, int Cn, const int64_t* __restrict__ labels, HeadCfg h,
-                     float* __restrict__ logits /*[B,Cn] or null*/, float* __restrict__ row_lse, float* __restrict__ row_loss) {
+margin_ce_fwd_kernel(const float* __restrict__ cosm, int ldc, int B, int Cn, const int64_t* __restrict__ labels, int64_t c_off,
+                     int Ctot, const float* __restrict__ gt, HeadCfg h, float* __restrict__ logits /*[B,Cn] or null*/,
+                     float* __restrict__ row_lse, float* __restrict__ row_loss, float4* __restrict__ partials) {
   __shared__ float red[3][8];
   const int row = blockIdx.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t y = labels[row];
+  const int64_t y = labels[row] - c_off;
   MvRow mv{0.f, 0.f, 0.f};
-  if (h.kind == VDK_HEAD_MV_SOFTMAX) mv = mv_row(h, cosm[static_cast<int64_t>(row) * ldc + y]);
+  if (h.kind == VDK_HEAD_MV_SOFTMAX) mv = mv_row(h, gt ? gt[row] : cosm[static_cast<int64_t>(row) * ldc + y]);
   float mx = -FLT_MAX, se = 0.f, sz = 0.f, zy = 0.f;
   for (int c = tid; c < Cn; c += 256) {
     float z, dz;
@@ -252,11 +260,45 @@ margin_ce_fwd_kernel(const float* __restrict__ cosm, int ldc, int B, int Cn, con
       Z += red[2][w];
       ZY += s_zy[w];
     }
+    if (partials) {
+      partials[row] = make_float4(M, S, Z, ZY);
+      return;
+    }
     const float lse = M + logf(S);
     row_lse[row] = lse;
-    // CE with label smoothing: (1-e) * (lse - z_y) + e * (lse - mean_c z)
-    row_loss[row] = (1.f - h.label_smooth) * (lse - ZY) + h.label_smooth * (lse - Z / static_cast<float>(Cn));
+    row_loss[row] = ce_row_loss(h, lse, ZY, Z, Ctot);
   }
+}
+
+// the shards' partials [world, B] -> row_lse, row_loss; one thread per row, ranks in order (the block combine above, one
+// level up: with world = 1 it returns that combine's values unchanged)
+__global__ void __launch_bounds__(256)
+margin_ce_combine_kernel(const float4* __restrict__ partials, int world, int B, int Ctot, HeadCfg h, float* __restrict__ row_lse,
+                         float* __restrict__ row_loss) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= B) return;
+  float M = -FLT_MAX;
+  for (int w = 0; w < world; ++w) M = fmaxf(M, partials[static_cast<int64_t>(w) * B + row].x);
+  float S = 0.f, Z = 0.f, ZY = 0.f;
+  for (int w = 0; w < world; ++w) {
+    const float4 p = partials[static_cast<int64_t>(w) * B + row];
+    S += p.y * __expf(p.x - M);
+    Z += p.z;
+    ZY += p.w;
+  }
+  const float lse = M + logf(S);
+  row_lse[row] = lse;
+  row_loss[row] = ce_row_loss(h, lse, ZY, Z, Ctot);
+}
+
+// gt[r] = cos of row r's label column if this shard [c_off, c_off + Cn) holds it, else 0
+__global__ void __launch_bounds__(256)
+label_cos_kernel(const float* __restrict__ cosm, int ldc, int B, int Cn, const int64_t* __restrict__ labels, int64_t c_off,
+                 float* __restrict__ gt) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= B) return;
+  const int64_t y = labels[row] - c_off;
+  gt[row] = (y >= 0 && y < Cn) ? cosm[static_cast<int64_t>(row) * ldc + y] : 0.f;
 }
 
 __global__ void mean_kernel(const float* __restrict__ x, int n, float* out) {
@@ -267,35 +309,39 @@ __global__ void mean_kernel(const float* __restrict__ x, int n, float* out) {
   if (threadIdx.x == 0) *out = s / static_cast<float>(n);
 }
 
-// backward: dcos[b,c] = gout/B * (softmax - target) * dz/dcos * inv_wnorm[c]   (column norm folded in for dF~ = dcos' . W^T)
-// and dcos_plain (without the column norm) for dW~ = f~^T . dcos
+// backward: dcos[b,c] = gout/B_f * (softmax - target) * dz/dcos * inv_wnorm[c]   (column norm folded in for dF~ = dcos' . W^T)
+// and dcos_plain = gout/B * ... (without the column norm) for dW~ = f~^T . dcos.  Unsharded B_f = B; a class shard over
+// `world` ranks passes B_f = B / world, so that dF~ is the gradient of each rank's own mean loss and dW~ the gradient of the
+// mean over all B rows (the rank-average DDP would form), plus c_off, Ctot and gt as in the forward.
 __global__ void __launch_bounds__(256)
-margin_ce_bwd_kernel(const float* __restrict__ cosm, int ldc, int B, int Cn, const int64_t* __restrict__ labels, HeadCfg h,
-                     const float* __restrict__ row_lse, const float* __restrict__ grad_out, const float* __restrict__ dlogits,
-                     const float* __restrict__ inv_wnorm, float* __restrict__ dcos_plain, float* __restrict__ dcos_scaled,
-                     int ldd) {
+margin_ce_bwd_kernel(const float* __restrict__ cosm, int ldc, int B, int Bf, int Cn, const int64_t* __restrict__ labels,
+                     int64_t c_off, int Ctot, const float* __restrict__ gt, HeadCfg h, const float* __restrict__ row_lse,
+                     const float* __restrict__ grad_out, const float* __restrict__ dlogits, const float* __restrict__ inv_wnorm,
+                     float* __restrict__ dcos_plain, float* __restrict__ dcos_scaled, int ldd) {
   const int row = blockIdx.x;
-  const int64_t y = labels[row];
-  const float g = (grad_out ? *grad_out : 1.f) / static_cast<float>(B);
+  const int64_t y = labels[row] - c_off;
+  const float gw = (grad_out ? *grad_out : 1.f) / static_cast<float>(B);
+  const float gf = (grad_out ? *grad_out : 1.f) / static_cast<float>(Bf);
   const float lse = row_lse ? row_lse[row] : 0.f;
-  const float t_off = h.label_smooth / static_cast<float>(Cn);
+  const float t_off = h.label_smooth / static_cast<float>(Ctot);
   MvRow mv{0.f, 0.f, 0.f};
-  if (h.kind == VDK_HEAD_MV_SOFTMAX) mv = mv_row(h, cosm[static_cast<int64_t>(row) * ldc + y]);
+  if (h.kind == VDK_HEAD_MV_SOFTMAX) mv = mv_row(h, gt ? gt[row] : cosm[static_cast<int64_t>(row) * ldc + y]);
   for (int c = threadIdx.x; c < ldd; c += 256) {
-    float v = 0.f;
+    float vw = 0.f, vf = 0.f;
     if (c < Cn) {
       float z, dz;
       head_logit(h, mv, cosm[static_cast<int64_t>(row) * ldc + c], c == y, z, dz);
       if (dlogits) {  // un-fused path: the caller's criterion produced d(loss)/d(logits)
-        v = dlogits[static_cast<int64_t>(row) * Cn + c] * dz;
+        vw = vf = dlogits[static_cast<int64_t>(row) * Cn + c] * dz;
       } else {
         const float p = __expf(z - lse);
         const float target = (c == y ? (1.f - h.label_smooth) : 0.f) + t_off;
-        v = g * (p - target) * dz;
+        vw = gw * (p - target) * dz;
+        vf = gf * (p - target) * dz;
       }
     }
-    dcos_plain[static_cast<int64_t>(row) * ldd + c] = v;
-    dcos_scaled[static_cast<int64_t>(row) * ldd + c] = c < Cn ? v * inv_wnorm[c] : 0.f;
+    dcos_plain[static_cast<int64_t>(row) * ldd + c] = vw;
+    dcos_scaled[static_cast<int64_t>(row) * ldd + c] = c < Cn ? vf * inv_wnorm[c] : 0.f;
   }
 }
 
@@ -338,11 +384,12 @@ wgrad_finalize_kernel(const float* __restrict__ dwn, int ldw, const float* __res
 static size_t a256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 static int pad8(int v) { return (v + 7) & ~7; }
 
-static int make_cfg(const vdk_head_desc* d, HeadCfg* h) {
+// min_class: 2 for a whole head; a class shard may hold a single class (its total is checked by make_shard)
+static int make_cfg(const vdk_head_desc* d, HeadCfg* h, int min_class = 2) {
   VDK_REQUIRE(d, "null head descriptor");
   VDK_REQUIRE(d->kind == VDK_HEAD_ARCFACE || d->kind == VDK_HEAD_CIRCLELOSS || d->kind == VDK_HEAD_MV_SOFTMAX,
               "head kind must be arcface, circleloss or mv-softmax");
-  VDK_REQUIRE(d->batch > 0 && d->feat_dim > 0 && d->num_class > 1, "bad head shape");
+  VDK_REQUIRE(d->batch > 0 && d->feat_dim > 0 && d->num_class >= min_class, "bad head shape");
   VDK_REQUIRE(d->label_smooth >= 0.f && d->label_smooth < 1.f, "label_smooth must be in [0,1)");
   h->kind = d->kind;
   h->cos_m = cosf(d->margin_arc);
@@ -452,7 +499,7 @@ extern "C" int vdk_head_forward(const vdk_head_desc* d, const float* feats, cons
   rc = head_cos(d, feats, weight, w, s);
   if (rc != VDK_OK) return rc;
   const int B = d->batch, Cn = d->num_class;
-  margin_ce_fwd_kernel<<<B, 256, 0, s>>>(w.cosm, w.Cp, B, Cn, labels, h, logits, row_lse, w.row_loss);
+  margin_ce_fwd_kernel<<<B, 256, 0, s>>>(w.cosm, w.Cp, B, Cn, labels, 0, Cn, nullptr, h, logits, row_lse, w.row_loss, nullptr);
   mean_kernel<<<1, 32, 0, s>>>(w.row_loss, B, loss);
   if (cos_saved)
     VDK_CUDA_OK(cudaMemcpy2DAsync(cos_saved, static_cast<size_t>(Cn) * 4, w.cosm, static_cast<size_t>(w.Cp) * 4,
@@ -460,6 +507,75 @@ extern "C" int vdk_head_forward(const vdk_head_desc* d, const float* feats, cons
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }
+
+namespace vdk {
+
+// Everything of the backward after the cos recompute: dcos, dF~ [B, D] into dfn (fixed-order split-K slabs), dW [D, Cn].
+// The unsharded backward passes c_off = 0, Ctot = Cn, gt = null, Bf = B.
+static int head_backward_core(const vdk_head_desc* d, const HeadCfg& h, const float* weight, const int64_t* labels,
+                              int64_t c_off, int Ctot, const float* gt, int Bf, const float* row_lse, const float* grad_loss,
+                              const float* dlogits, float* dfn, float* dweight, const HeadWs& w, cudaStream_t s) {
+  const int B = d->batch, D = d->feat_dim, Cn = d->num_class;
+  int rc;
+  margin_ce_bwd_kernel<<<B, 256, 0, s>>>(w.cosm, w.Cp, B, Bf, Cn, labels, c_off, Ctot, gt, h, row_lse, grad_loss, dlogits, w.inv_w,
+                                         w.dcos_plain, w.dcos_scaled, w.Cp);
+  VDK_CUDA_OK(cudaGetLastError());
+  // dF~ [B,D] = dcos' [B,C] . W^T   (A = dcos' rows over K=C, B = W rows [D, C])
+  split3_rows_kernel<<<blocks_for(static_cast<int64_t>(B) * w.Cp, 256), 256, 0, s>>>(w.dcos_scaled, B, w.Cp, w.Cp, w.Cp, nullptr,
+                                                                                    nullptr, 0, w.a_split, nullptr);
+  split3_rows_kernel<<<blocks_for(static_cast<int64_t>(D) * w.Cp, 256), 256, 0, s>>>(weight, D, Cn, Cn, w.Cp, nullptr, nullptr, 1,
+                                                                                    w.b_split, nullptr);
+  VDK_CUDA_OK(cudaGetLastError());
+  if (w.dfn_splits > 1) {
+    vdk_gemm_desc g{};
+    g.A = w.a_split; g.B = w.b_split; g.D = w.dfn_slabs;
+    g.M = B; g.N = D; g.K = 6 * w.Cp; g.lda = 6 * w.Cp; g.ldb = 6 * w.Cp; g.ldd = D;
+    g.in_dtype = VDK_DTYPE_BF16; g.out_dtype = VDK_DTYPE_FP32; g.epilogue = VDK_EPI_NONE;
+    g.split_k = w.dfn_splits; g.split_stride = static_cast<long long>(B) * D;
+    rc = gemm_run(g, s);
+    if (rc != VDK_OK) return rc;
+    rc = launch_slab_reduce(w.dfn_slabs, w.dfn_splits, static_cast<size_t>(B) * D, static_cast<int64_t>(B) * D / 4, dfn, 0, s);
+  } else {
+    rc = split_gemm(w.a_split, w.b_split, dfn, B, D, 6 * w.Cp, D, s);
+  }
+  if (rc != VDK_OK) return rc;
+  // dW~ [D,C] = f~^T [D,B] . dcos [B,C]   (A = f~^T over K=B, B = dcos^T [C, B])
+  {
+    dim3 ga((D + 31) / 32, (w.Bp + 31) / 32);
+    split3_cols_kernel<<<ga, 256, 0, s>>>(w.fn, D, B, D, D, w.Bp, nullptr, 0, w.a_split);
+    dim3 gb((w.Cp + 31) / 32, (w.Bp + 31) / 32);
+    split3_cols_kernel<<<gb, 256, 0, s>>>(w.dcos_plain, w.Cp, B, w.Cp, w.Cp, w.Bp, nullptr, 1, w.b_split);
+    VDK_CUDA_OK(cudaGetLastError());
+  }
+  rc = split_gemm(w.a_split, w.b_split, w.dwn, D, w.Cp, 6 * w.Bp, w.Cp, s);
+  if (rc != VDK_OK) return rc;
+  wgrad_finalize_kernel<<<(Cn + 31) / 32, 256, 0, s>>>(w.dwn, w.Cp, weight, w.inv_w, D, Cn, dweight);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
+// the shard descriptor against the head descriptor; fills the head constants (the whole head's C must exceed 1, a shard may
+// hold one class)
+static int make_shard(const vdk_head_desc* d, const vdk_head_shard* sh, HeadCfg* h) {
+  VDK_REQUIRE(sh, "null head shard descriptor");
+  int rc = make_cfg(d, h, 1);
+  if (rc != VDK_OK) return rc;
+  VDK_REQUIRE(sh->num_class_total > 1, "head shard: num_class_total must exceed 1");
+  VDK_REQUIRE(sh->class_offset >= 0 && d->num_class <= sh->num_class_total - sh->class_offset,
+              "head shard: classes [class_offset, class_offset + num_class) must lie inside [0, num_class_total)");
+  VDK_REQUIRE(sh->world >= 1 && sh->rank >= 0 && sh->rank < sh->world, "head shard: need 0 <= rank < world");
+  VDK_REQUIRE(d->batch % sh->world == 0, "head shard: the gathered batch must be world equal rank batches");
+  return VDK_OK;
+}
+
+static int ws_ok(const vdk_head_desc* d, void* workspace, size_t workspace_bytes) {
+  VDK_REQUIRE(workspace && workspace_bytes >= vdk_head_workspace_bytes(d) && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
+              "head: workspace too small or misaligned");
+  return VDK_OK;
+}
+
+}  // namespace vdk
+
 
 extern "C" int vdk_head_backward(const vdk_head_desc* d, const float* feats, const float* weight, const int64_t* labels,
                                  const float* row_lse, const float* grad_loss, const float* dlogits, float* dfeats,
@@ -479,40 +595,113 @@ extern "C" int vdk_head_backward(const vdk_head_desc* d, const float* feats, con
   // recompute cos (cheaper than keeping [B,C] alive between forward and backward at face-scale C)
   rc = head_cos(d, feats, weight, w, s);
   if (rc != VDK_OK) return rc;
-  margin_ce_bwd_kernel<<<B, 256, 0, s>>>(w.cosm, w.Cp, B, Cn, labels, h, row_lse, grad_loss, dlogits, w.inv_w, w.dcos_plain,
-                                         w.dcos_scaled, w.Cp);
-  VDK_CUDA_OK(cudaGetLastError());
-  // dF~ [B,D] = dcos' [B,C] . W^T   (A = dcos' rows over K=C, B = W rows [D, C])
-  split3_rows_kernel<<<blocks_for(static_cast<int64_t>(B) * w.Cp, 256), 256, 0, s>>>(w.dcos_scaled, B, w.Cp, w.Cp, w.Cp, nullptr,
-                                                                                    nullptr, 0, w.a_split, nullptr);
-  split3_rows_kernel<<<blocks_for(static_cast<int64_t>(D) * w.Cp, 256), 256, 0, s>>>(weight, D, Cn, Cn, w.Cp, nullptr, nullptr, 1,
-                                                                                    w.b_split, nullptr);
-  VDK_CUDA_OK(cudaGetLastError());
-  if (w.dfn_splits > 1) {
-    vdk_gemm_desc g{};
-    g.A = w.a_split; g.B = w.b_split; g.D = w.dfn_slabs;
-    g.M = B; g.N = D; g.K = 6 * w.Cp; g.lda = 6 * w.Cp; g.ldb = 6 * w.Cp; g.ldd = D;
-    g.in_dtype = VDK_DTYPE_BF16; g.out_dtype = VDK_DTYPE_FP32; g.epilogue = VDK_EPI_NONE;
-    g.split_k = w.dfn_splits; g.split_stride = static_cast<long long>(B) * D;
-    rc = gemm_run(g, s);
-    if (rc != VDK_OK) return rc;
-    rc = launch_slab_reduce(w.dfn_slabs, w.dfn_splits, static_cast<size_t>(B) * D, static_cast<int64_t>(B) * D / 4, w.dfn, 0, s);
-  } else {
-    rc = split_gemm(w.a_split, w.b_split, w.dfn, B, D, 6 * w.Cp, D, s);
-  }
+  rc = head_backward_core(d, h, weight, labels, 0, Cn, nullptr, B, row_lse, grad_loss, dlogits, w.dfn, dweight, w, s);
   if (rc != VDK_OK) return rc;
   fgrad_finalize_kernel<<<(B * 32 + 255) / 256, 256, 0, s>>>(w.dfn, w.fn, w.inv_f, B, D, dfeats);
-  // dW~ [D,C] = f~^T [D,B] . dcos [B,C]   (A = f~^T over K=B, B = dcos^T [C, B])
-  {
-    dim3 ga((D + 31) / 32, (w.Bp + 31) / 32);
-    split3_cols_kernel<<<ga, 256, 0, s>>>(w.fn, D, B, D, D, w.Bp, nullptr, 0, w.a_split);
-    dim3 gb((w.Cp + 31) / 32, (w.Bp + 31) / 32);
-    split3_cols_kernel<<<gb, 256, 0, s>>>(w.dcos_plain, w.Cp, B, w.Cp, w.Cp, w.Bp, nullptr, 1, w.b_split);
-    VDK_CUDA_OK(cudaGetLastError());
-  }
-  rc = split_gemm(w.a_split, w.b_split, w.dwn, D, w.Cp, 6 * w.Bp, w.Cp, s);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
+extern "C" int vdk_head_shard_struct_sizes(size_t* out, int n) {
+  if (out && n >= 1) out[0] = sizeof(vdk_head_shard);
+  return 1;
+}
+
+extern "C" int vdk_head_shard_cos(const vdk_head_desc* d, const vdk_head_shard* sh, const float* feats, const float* weight,
+                                  const int64_t* labels, float* label_cos, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  HeadCfg h;
+  int rc = make_shard(d, sh, &h);
   if (rc != VDK_OK) return rc;
-  wgrad_finalize_kernel<<<(Cn + 31) / 32, 256, 0, s>>>(w.dwn, w.Cp, weight, w.inv_w, D, Cn, dweight);
+  VDK_REQUIRE(feats && weight && labels && label_cos, "vdk_head_shard_cos: null operand");
+  rc = ws_ok(d, workspace, workspace_bytes);
+  if (rc != VDK_OK) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  HeadWs w;
+  head_ws_layout(d, workspace, &w);
+  rc = head_cos(d, feats, weight, w, s);
+  if (rc != VDK_OK) return rc;
+  label_cos_kernel<<<(d->batch + 255) / 256, 256, 0, s>>>(w.cosm, w.Cp, d->batch, d->num_class, labels, sh->class_offset, label_cos);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
+extern "C" int vdk_head_shard_forward(const vdk_head_desc* d, const vdk_head_shard* sh, const int64_t* labels,
+                                      const float* label_cos, float* logits, float* cos_saved, float* partials,
+                                      void* workspace, size_t workspace_bytes, void* stream) {
+  HeadCfg h;
+  int rc = make_shard(d, sh, &h);
+  if (rc != VDK_OK) return rc;
+  VDK_REQUIRE(labels && partials && (label_cos || d->kind != VDK_HEAD_MV_SOFTMAX), "vdk_head_shard_forward: null operand");
+  VDK_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 15) == 0, "vdk_head_shard_forward: partials must be 16-byte aligned");
+  rc = ws_ok(d, workspace, workspace_bytes);
+  if (rc != VDK_OK) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  HeadWs w;
+  head_ws_layout(d, workspace, &w);
+  const int B = d->batch, Cn = d->num_class;
+  margin_ce_fwd_kernel<<<B, 256, 0, s>>>(w.cosm, w.Cp, B, Cn, labels, sh->class_offset, sh->num_class_total,
+                                         d->kind == VDK_HEAD_MV_SOFTMAX ? label_cos : nullptr, h, logits, nullptr, nullptr,
+                                         reinterpret_cast<float4*>(partials));
+  if (cos_saved)
+    VDK_CUDA_OK(cudaMemcpy2DAsync(cos_saved, static_cast<size_t>(Cn) * 4, w.cosm, static_cast<size_t>(w.Cp) * 4,
+                                  static_cast<size_t>(Cn) * 4, B, cudaMemcpyDeviceToDevice, s));
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
+extern "C" int vdk_head_shard_combine(const vdk_head_desc* d, const vdk_head_shard* sh, const float* partials, float* row_lse,
+                                      float* row_loss, float* loss, void* stream) {
+  HeadCfg h;
+  int rc = make_shard(d, sh, &h);
+  if (rc != VDK_OK) return rc;
+  VDK_REQUIRE(partials && row_lse && row_loss && loss, "vdk_head_shard_combine: null operand");
+  VDK_REQUIRE((reinterpret_cast<uintptr_t>(partials) & 15) == 0, "vdk_head_shard_combine: partials must be 16-byte aligned");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int B = d->batch, Bl = B / sh->world;
+  margin_ce_combine_kernel<<<(B + 255) / 256, 256, 0, s>>>(reinterpret_cast<const float4*>(partials), sh->world, B,
+                                                           sh->num_class_total, h, row_lse, row_loss);
+  mean_kernel<<<1, 32, 0, s>>>(row_loss + static_cast<int64_t>(sh->rank) * Bl, Bl, loss);
+  VDK_CUDA_OK(cudaGetLastError());
+  return VDK_OK;
+}
+
+extern "C" int vdk_head_shard_backward(const vdk_head_desc* d, const vdk_head_shard* sh, const float* feats, const float* weight,
+                                       const int64_t* labels, const float* label_cos, const float* row_lse,
+                                       const float* grad_loss, float* dfn, float* dweight, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  HeadCfg h;
+  int rc = make_shard(d, sh, &h);
+  if (rc != VDK_OK) return rc;
+  VDK_REQUIRE(feats && weight && labels && row_lse && dfn && dweight && (label_cos || d->kind != VDK_HEAD_MV_SOFTMAX),
+              "vdk_head_shard_backward: null operand");
+  VDK_REQUIRE(d->feat_dim % 8 == 0, "vdk_head_shard_backward: feat_dim must be a multiple of 8 (it is the N of the dF~ GEMM)");
+  rc = ws_ok(d, workspace, workspace_bytes);
+  if (rc != VDK_OK) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  HeadWs w;
+  head_ws_layout(d, workspace, &w);
+  rc = head_cos(d, feats, weight, w, s);
+  if (rc != VDK_OK) return rc;
+  return head_backward_core(d, h, weight, labels, sh->class_offset, sh->num_class_total,
+                            d->kind == VDK_HEAD_MV_SOFTMAX ? label_cos : nullptr, d->batch / sh->world, row_lse, grad_loss,
+                            nullptr, dfn, dweight, w, s);
+}
+
+extern "C" int vdk_head_shard_finalize(const vdk_head_desc* d, const vdk_head_shard* sh, const float* dfn, float* dfeats,
+                                       void* workspace, size_t workspace_bytes, void* stream) {
+  HeadCfg h;
+  int rc = make_shard(d, sh, &h);
+  if (rc != VDK_OK) return rc;
+  VDK_REQUIRE(dfn && dfeats, "vdk_head_shard_finalize: null operand");
+  rc = ws_ok(d, workspace, workspace_bytes);
+  if (rc != VDK_OK) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  HeadWs w;
+  head_ws_layout(d, workspace, &w);
+  const int D = d->feat_dim, Bl = d->batch / sh->world;
+  const int64_t r0 = static_cast<int64_t>(sh->rank) * Bl;
+  fgrad_finalize_kernel<<<(Bl * 32 + 255) / 256, 256, 0, s>>>(dfn + r0 * D, w.fn + r0 * D, w.inv_f + r0, Bl, D, dfeats);
   VDK_CUDA_OK(cudaGetLastError());
   return VDK_OK;
 }

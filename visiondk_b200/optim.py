@@ -9,7 +9,7 @@ ramp of models/ema.py:24.  FusedSGDClipEMA does everything after backward in two
 from __future__ import annotations
 
 import math
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import torch
 import torch.nn as nn
@@ -43,11 +43,14 @@ class FusedSGDClipEMA:
     param_groups: list of {'params': iterable, 'lr': float} like SeperateLayerParams.create_ParamSequence.
     ema_model: a deepcopy of the model (ModelEMA.ema) whose floating state is updated in place; its parameters
     are re-pointed into flat buffers parallel to the model's.
+    sharded_groups: indices of groups that hold a different shard of one tensor on every rank (the class-sharded head).
+    clip_grad_norm_ then uses the global norm: their sum of squares is summed over the ranks (one fp64 scalar) before the
+    replicated groups' is added.
     """
 
     def __init__(self, param_groups, lr: float, momentum: float, weight_decay: float, max_norm: float = 10.0,
                  model: Optional[nn.Module] = None, ema_model: Optional[nn.Module] = None, ema_decay: float = 0.9999,
-                 ema_tau: float = 2000.0):
+                 ema_tau: float = 2000.0, sharded_groups: Sequence[int] = ()):
         lib = _lib.load()
         if isinstance(param_groups, (list, tuple)) and param_groups and isinstance(param_groups[0], dict):
             groups = [(list(g["params"]), float(g.get("lr", lr))) for g in param_groups]
@@ -60,6 +63,7 @@ class FusedSGDClipEMA:
         self.param_groups = [{"lr": g.lr, "initial_lr": g.lr, "momentum": momentum, "weight_decay": weight_decay}
                              for g in self.groups]  # scheduler-facing view (torch LR schedulers mutate 'lr')
         self.max_norm = float(max_norm)
+        self.sharded_groups = tuple(sharded_groups)
         self.steps = 0
         dev = self.groups[0].p.device
         self._sumsq = torch.zeros((), dtype=torch.float64, device=dev)
@@ -93,9 +97,12 @@ class FusedSGDClipEMA:
         """Everything Trainer.update does after backward (train.py:206-215)."""
         lib = _lib.load()
         s = _lib.stream_ptr()
-        for i, g in enumerate(self.groups):
-            _lib.check(lib.vdk_grad_sumsq(g.g.data_ptr(), g.n, self._sumsq.data_ptr(), int(i > 0), self._ws.data_ptr(),
-                                          self._ws.numel(), s), "vdk_grad_sumsq")
+        if self.sharded_groups:
+            self._global_sumsq(lib, s)
+        else:
+            for i, g in enumerate(self.groups):
+                _lib.check(lib.vdk_grad_sumsq(g.g.data_ptr(), g.n, self._sumsq.data_ptr(), int(i > 0), self._ws.data_ptr(),
+                                              self._ws.numel(), s), "vdk_grad_sumsq")
         d, omd = -1.0, 0.0
         if self.ema_model is not None:
             self.updates += 1
@@ -111,6 +118,18 @@ class FusedSGDClipEMA:
             _lib.check(lib.vdk_ema_update(e.data_ptr(), b.data_ptr(), b.numel(), d, omd, s), "vdk_ema_update")
         self.steps += 1
         self._invalidate_packed()
+
+    def _global_sumsq(self, lib, s) -> None:
+        """Sum of squares of the whole model's gradient when some groups are sharded over the ranks: the shards' sums first,
+        summed over the ranks, then the replicated groups' added on every rank."""
+        from .sharding import all_reduce_sum_
+        order = list(self.sharded_groups) + [i for i in range(len(self.groups)) if i not in self.sharded_groups]
+        for j, i in enumerate(order):
+            g = self.groups[i]
+            _lib.check(lib.vdk_grad_sumsq(g.g.data_ptr(), g.n, self._sumsq.data_ptr(), int(j > 0), self._ws.data_ptr(),
+                                          self._ws.numel(), s), "vdk_grad_sumsq")
+            if j == len(self.sharded_groups) - 1:
+                all_reduce_sum_(self._sumsq)
 
     def _invalidate_packed(self) -> None:
         """The kernels above write parameters, EMA parameters and EMA buffers through raw pointers, which does not bump

@@ -62,6 +62,19 @@ def all_reduce_max_(t: torch.Tensor) -> None:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
 
 
+def all_reduce_sum_(t: torch.Tensor) -> None:
+    """In-place element-wise sum over the ranks (the class-sharded head's label cosines and feature-gradient partials).  NCCL
+    reduces device memory; gloo (the test harness) reduces host memory, so device tensors are staged through the host."""
+    if not _active():
+        return
+    if t.is_cuda and dist.get_backend() != "nccl":
+        host = t.cpu()
+        dist.all_reduce(host, op=dist.ReduceOp.SUM)
+        t.copy_(host)
+    else:
+        dist.all_reduce(t, op=dist.ReduceOp.SUM)
+
+
 class DistComm:
     """The shards' collectives over torch.distributed (NCCL between GPUs): the product path."""
 
@@ -81,20 +94,28 @@ class DistComm:
         _all_gather_into(out, src.contiguous())
         return out
 
+    def __deepcopy__(self, memo):  # a handle on the process group: copies of a module holding it share it
+        return self
+
     def all_reduce_max_(self, t: torch.Tensor) -> None:
         all_reduce_max_(t)
+
+    def all_reduce_sum_(self, t: torch.Tensor) -> None:
+        all_reduce_sum_(t)
 
 
 class LocalShardGroup:
     """W shards living on ONE device, one host thread each: the same protocol with the collectives replaced by a barrier and a
     `torch.stack` (all threads launch on the device's default stream, so stream order = launch order).  Test / measurement
-    harness only: it checks the W-shard protocol (and times a shard's share of the work) where a single GPU is available."""
+    harness only: it checks the W-shard protocol (and times a shard's share of the work) where a single GPU is available.
+    A shard that waits more than `timeout` seconds for the others fails with threading.BrokenBarrierError, so that a protocol
+    bug (one shard skipping a collective) fails its test instead of hanging it."""
 
-    def __init__(self, world: int):
+    def __init__(self, world: int, timeout: float = 120.0):
         import threading
-        self.world = world
+        self.world, self.timeout = world, timeout
         self._slots = [None] * world
-        self._barrier = threading.Barrier(world)
+        self._barrier = threading.Barrier(world, timeout=timeout)
 
     def comm(self, rank: int) -> "LocalShardGroup._Comm":
         return LocalShardGroup._Comm(self, rank)
@@ -103,7 +124,7 @@ class LocalShardGroup:
         """fn(comm) on one thread per shard; returns the per-shard results in rank order (re-raises the first failure)."""
         import threading
         results, errors = [None] * self.world, []
-        self._barrier = threading.Barrier(self.world)  # a failed run leaves the old one broken
+        self._barrier = threading.Barrier(self.world, timeout=self.timeout)  # a failed run leaves the old one broken
 
         def work(rank: int) -> None:
             try:
@@ -128,6 +149,9 @@ class LocalShardGroup:
         def __init__(self, group: "LocalShardGroup", rank: int):
             self.g, self.rank, self.world = group, rank, group.world
 
+        def __deepcopy__(self, memo):  # a handle on the group: copies of a module holding it share it
+            return self
+
         def all_gather(self, src: torch.Tensor) -> torch.Tensor:
             self.g._slots[self.rank] = src
             self.g._barrier.wait()
@@ -137,6 +161,14 @@ class LocalShardGroup:
 
         def all_reduce_max_(self, t: torch.Tensor) -> None:
             t.copy_(self.all_gather(t).amax(dim=0))
+
+        def all_reduce_sum_(self, t: torch.Tensor) -> None:
+            """Sum in rank order (every shard gets the same bits)."""
+            parts = self.all_gather(t)
+            acc = parts[0].clone()
+            for p in parts[1:]:
+                acc += p
+            t.copy_(acc)
 
 
 def all_gather_rows(local: torch.Tensor, sizes: List[int]) -> torch.Tensor:

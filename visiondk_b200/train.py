@@ -20,7 +20,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from .backbone import BackboneFactory
-from .heads import HeadFactory, margin_ce_loss
+from .heads import HeadFactory, ShardedHead, margin_ce_loss, sharded_margin_ce_loss
 from .optim import FusedSGDClipEMA
 
 
@@ -41,7 +41,18 @@ class FaceTrainingModel(nn.Module):
         """criterion(self(data, label), label) with criterion = CrossEntropyLoss(label_smoothing), fused
         (train.py:196: the two are only ever called together)."""
         feat = self.trainingwrapper["backbone"](data)
-        return margin_ce_loss(self.trainingwrapper["head"], feat, label, label_smooth)
+        head = self.trainingwrapper["head"]
+        if isinstance(head, ShardedHead):
+            return sharded_margin_ce_loss(head, feat, label, label_smooth)
+        return margin_ce_loss(head, feat, label, label_smooth)
+
+    def shard_head_(self, comm=None) -> None:
+        """Replaces the head by this rank's class shard (heads.ShardedHead) of rank 0's full weight: the columns the unsharded
+        trainer would hold after broadcasting rank 0's initial state."""
+        head = self.trainingwrapper["head"]
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            dist.broadcast(head.weight.data, src=0)
+        self.trainingwrapper["head"] = ShardedHead(head, comm)
 
 
 def cosine_with_warm_lr(step: int, base_lr: float, lr0: float, warm: int, total: int, lrf_ratio: Optional[float]) -> float:
@@ -65,21 +76,35 @@ def layer_wise_groups(model: FaceTrainingModel, layer_wise: bool, lr: float):
 
 
 class FaceTrainer:
-    """The per-batch body of Trainer.train_one_epoch_face (engine/procedure/train.py:217-233) on H100."""
+    """The per-batch body of Trainer.train_one_epoch_face (engine/procedure/train.py:217-233) on H100.
+
+    shard_head: split the head's classes over the ranks (heads.ShardedHead).  The head then is its own flat parameter group
+    (also with layer_wise=False), which the DDP all-reduce and the initial broadcast leave out; clipping uses the global
+    gradient norm.  Every rank must pass the same use_ema: each keeps the EMA of its own head columns.  `state_dict` and
+    `load_state_dict` read and write the unsharded layout, so checkpoints move between the two modes; `state_dict` is then
+    a collective."""
 
     def __init__(self, model: FaceTrainingModel, lr0: float, momentum: float, weight_decay: float, label_smooth: float = 0.0,
                  layer_wise: bool = True, warm_steps: int = 0, total_steps: int = 1, lrf_ratio: Optional[float] = None,
-                 use_ema: bool = True, max_norm: float = 10.0):
+                 use_ema: bool = True, max_norm: float = 10.0, shard_head: bool = False):
         self.model = model
         self.label_smooth = label_smooth
+        self.shard_head, self.layer_wise = shard_head, layer_wise
+        if shard_head:
+            model.shard_head_()
         self.ema = copy.deepcopy(model).eval() if use_ema else None  # models/ema.py:20-26
         if self.ema is not None:
             for p in self.ema.parameters():
                 p.requires_grad_(False)
         groups = layer_wise_groups(model, layer_wise, lr0)
+        if shard_head and not layer_wise:
+            groups = [{"params": list(model.trainingwrapper["backbone"].parameters()), "lr": lr0},
+                      {"params": list(model.trainingwrapper["head"].parameters()), "lr": lr0}]
         self.base_lrs = [g["lr"] for g in groups]
         self.opt = FusedSGDClipEMA(groups, lr=lr0, momentum=momentum, weight_decay=weight_decay, max_norm=max_norm, model=model,
-                                   ema_model=self.ema)
+                                   ema_model=self.ema, sharded_groups=(len(groups) - 1,) if shard_head else ())
+        # the groups DDP averages and the initial broadcast covers: every group but the head's shard
+        self._ddp_groups = self.opt.groups[:-1] if shard_head else self.opt.groups
         self.lr0, self.warm, self.total, self.lrf = lr0, warm_steps, total_steps, lrf_ratio
         self.sched_step = 0
         self._apply_lr()
@@ -91,23 +116,65 @@ class FaceTrainer:
         gradients would be shared.  Same here, on the flat parameter buffers (+ momentum) and every module buffer."""
         if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
             return
-        for g in self.opt.groups:
+        for g in self._ddp_groups:
             dist.broadcast(g.p, src=0)
             dist.broadcast(g.mom, src=0)
+            if self.shard_head and g.ema is not None:  # every rank keeps an EMA: start it from rank 0's
+                dist.broadcast(g.ema, src=0)
         for b in self.model.buffers():
             dist.broadcast(b, src=0)
+        if self.shard_head and self.ema is not None:
+            for b in self.ema.buffers():
+                dist.broadcast(b, src=0)
         self.opt._invalidate_packed()
 
     def state_dict(self) -> dict:
         """The trainer-side entries of the reference's checkpoint (engine/procedure/train.py:266-276): 'optimizer',
         'scheduler' (position in cosine_with_warm) and the EMA's 'updates'."""
-        return {"optimizer": self.opt.state_dict(), "scheduler": {"step": self.sched_step}, "updates": self.opt.updates}
+        opt = self.opt.state_dict()
+        if self.shard_head:
+            opt = self._unsharded_optimizer_state(opt)
+        return {"optimizer": opt, "scheduler": {"step": self.sched_step}, "updates": self.opt.updates}
 
     def load_state_dict(self, state: dict) -> None:
-        self.opt.load_state_dict(state["optimizer"])
+        opt = state["optimizer"]
+        if self.shard_head:
+            opt = self._sharded_optimizer_state(opt)
+        self.opt.load_state_dict(opt)
         self.opt.updates = int(state.get("updates", self.opt.updates))
         self.sched_step = int(state["scheduler"]["step"])
         self._apply_lr()  # param_groups' lr follow the restored schedule position, not the saved (pre-step) value
+
+    def _head_dims(self):
+        head = self.model.trainingwrapper["head"]
+        return head, head.weight.shape[0], head.num_class_total
+
+    def _unsharded_optimizer_state(self, opt: dict) -> dict:
+        """The sharded optimizer state in the unsharded trainer's layout: the head's momentum gathered to [D, C] (a collective)
+        and, with layer_wise=False, the backbone and head groups joined into the single group the unsharded trainer has."""
+        from .heads import gather_columns
+        head, D, Cn = self._head_dims()
+        mom = self.opt.groups[-1].mom.view(D, -1)
+        bufs = opt["momentum_buffers"][:-1] + [gather_columns(head.comm, mom, Cn).reshape(-1).cpu()]
+        pgs = opt["param_groups"]
+        if not self.layer_wise:
+            bufs, pgs = [torch.cat(bufs)], pgs[:1]
+        return dict(opt, momentum_buffers=bufs, param_groups=pgs)
+
+    def _sharded_optimizer_state(self, opt: dict) -> dict:
+        """The inverse of _unsharded_optimizer_state: this rank's columns of the head's momentum."""
+        from .heads import shard_columns
+        head, D, Cn = self._head_dims()
+        bufs, pgs = list(opt["momentum_buffers"]), [dict(pg) for pg in opt["param_groups"]]
+        if not self.layer_wise:
+            if len(bufs) != 1:
+                raise ValueError("optimizer state has a different number of parameter groups")
+            nb = self.opt.groups[0].n
+            bufs, pgs = [bufs[0][:nb], bufs[0][nb:]], pgs * 2
+        if bufs[-1].numel() != D * Cn:
+            raise ValueError("optimizer state does not match the full head (different model?)")
+        bufs[-1] = shard_columns(bufs[-1].reshape(D, Cn), head.comm.world, head.comm.rank).reshape(-1)
+        return dict(opt, momentum_buffers=bufs, param_groups=pgs)
 
     def _apply_lr(self):
         for pg, base in zip(self.opt.param_groups, self.base_lrs):
@@ -172,7 +239,7 @@ class FaceTrainer:
             backbone.grad_section_hook = None
             for w in self._pending:
                 w.wait()  # the compute stream waits for the collectives (no host block)
-            for g in self.opt.groups:  # whatever the sections did not cover (the head group; gaps; a failed overlap)
+            for g in self._ddp_groups:  # whatever the sections did not cover (the head group; gaps; a failed overlap)
                 done = sorted((lo, hi) for gid, lo, hi in self._reduced if gid == id(g)) if not self._overlap_failed else []
                 if self._overlap_failed and self._reduced:
                     raise RuntimeError("DDP overlap: gradient sections were not contiguous after some were already reduced")
