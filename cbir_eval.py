@@ -2,11 +2,11 @@
 """cbir_eval.py — stand-alone CBIR evaluation on H100 (entry point kept from the reference; new code).
 
     python cbir_eval.py [--cfgs configs/faceX/cbir_convnext_b200.yaml] [--weight Epoch_N.pt] [--ema]
-                        [--gallery 100000] [--queries 1000] [--k 10]
+                        [--gallery 100000] [--queries 1000] [--k 10] [--index_factory IVF1024,PQ64 --nprobe 32]
 
 The reference script (cbir_eval.py) hard-codes its paths, builds a random-init model, extracts gallery and query
 embeddings, builds a faiss Flat/IP index and searches k=10.  This one does the same through visiondk_b200:
-ConvNeXt embeddings on the sm_90a kernels, FlatIPIndex for index/search, everything resident in HBM.  Without a
+ConvNeXt embeddings on the sm_90a kernels, FlatIPIndex (or an IVF index, --index_factory / --nprobe) for index/search, everything resident in HBM.  Without a
 dataset on disk it evaluates on synthetic images (random tensors: timing / plumbing) — real datasets plug in through
 any iterable of [B,3,S,S] float tensors (the reference's CBIRDatasets + DataLoader yield exactly that).
 """
@@ -47,6 +47,8 @@ def main(argv=None):
     ap.add_argument("--queries", type=int, default=1000)
     ap.add_argument("--k", type=int, default=10)
     ap.add_argument("--device", default="cuda:0")
+    ap.add_argument("--index_factory", default="Flat", help="'Flat', 'IVF<nlist>,Flat' or 'IVF<nlist>,PQ<M>[x8]'")
+    ap.add_argument("--nprobe", type=int, default=1, help="lists probed per query by an IVF index")
     opt = ap.parse_args(argv)
 
     with open(opt.cfgs, errors="ignore") as f:
@@ -74,7 +76,9 @@ def main(argv=None):
         gallery, queries = SyntheticImages(opt.gallery, bs, size, device, 1), SyntheticImages(opt.queries, bs, size, device, 2)
         g_label = q_label = None
     t0 = time.perf_counter()
-    faiss_index = index(extractor, gallery, device)
+    faiss_index = index(extractor, gallery, device, index_factory=opt.index_factory)
+    if opt.index_factory != "Flat":
+        faiss_index.nprobe = opt.nprobe
     torch.cuda.synchronize()
     t1 = time.perf_counter()
     scores, indices = search(extractor, queries, faiss_index, device, k=opt.k)
@@ -83,7 +87,10 @@ def main(argv=None):
     print(f"indexed {faiss_index.ntotal} gallery images in {t1 - t0:.2f} s "
           f"({faiss_index.ntotal / (t1 - t0):.0f} embeddings/s incl. synthetic image generation)")
     print(f"searched {n_q} queries (k={opt.k}) in {t2 - t1:.3f} s; top-1 scores mean {scores[:, 0].mean():.4f}")
-    print("status", faiss_index.check_status())
+    if opt.index_factory == "Flat":
+        print("status", faiss_index.check_status())
+    else:
+        print(f"{opt.index_factory} nprobe {faiss_index.nprobe}: {faiss_index.nbytes / max(faiss_index.ntotal, 1):.1f} bytes per row")
     if g_label is not None:  # cbir_eval.py:124-199 `evaluate`: metrics at the config's cutoffs (capped at k)
         cutoffs = [c for c in data_cfg["val"]["metrics"]["cutoffs"] if c <= opt.k] or [opt.k]
         m = compute_metrics(torch.from_numpy(indices).to(device), torch.from_numpy(scores).to(device), q_label, g_label,

@@ -960,6 +960,38 @@ int vdk_topk_merge_packed(const void* packed, int n_lists, int64_t n_query, int 
 int vdk_ip_exact_pairs(const float* q32, const float* g32, int dim, const int64_t* qi, const int64_t* gi, int64_t n,
                        float* out, void* stream);
 
+/* ---- inverted-file indexes: IVF-Flat and IVF-PQ (visiondk_b200/ivf.py, oracle/ivf.py, DESIGN §3b) --------------------------- */
+/* One Lloyd update of n_sub independent k-means problems of k centroids each, plus the empty-cluster split.  Problem s reads
+ * columns [s*dim, (s+1)*dim) of the rows of x (row pitch ld floats).  order: row ids grouped by centroid g = s*k + c, ascending
+ * within a group; offsets [n_sub*k + 1] delimit the groups in order.  centroids [n_sub*k][dim]: a non-empty centroid becomes
+ * fp32(fp64 sequential sum of its members / count).  counts [n_sub*k] (in: the group sizes) is updated by the split: each empty
+ * centroid, in ascending order, copies the then-largest one of its problem (lowest index on ties), the two copies are scaled
+ * by 1 + 1/1024 and 1 - 1/1024 on even dimensions and the other way on odd ones, and the count is halved between them. */
+int vdk_kmeans_update(const float* x, int64_t ld, int dim, int n_sub, int k, const int64_t* order, const int64_t* offsets,
+                      int64_t* counts, float* centroids, void* stream);
+/* PQ encoding by residual, 8-bit codes: residual[n][d] = fl32(x - coarse[list_of_row]); codes[n][M] = per sub-space (d/M wide)
+ * argmin_j of the sequential fp64 sum of (r_t - cw_jt)^2, ties -> lowest j.  codebooks [M][256][d/M].  M <= 128. */
+int vdk_pq_encode(const float* x, int64_t n, int d, const float* coarse, const int64_t* list_of_row, int M, const float* codebooks,
+                  float* residual, uint8_t* codes, void* stream);
+/* PQ lookup tables: lut[q][m][j] = fp32(sequential fp64 sum over t of q[m*dsub + t] * cw[m][j][t]). */
+int vdk_pq_lut(const float* q, int64_t n_query, int d, int M, const float* codebooks, float* lut, void* stream);
+/* IVF-Flat list scan.  The (query, list) probe pairs are sorted by list; items [n_items][3] = {list, first pair, count <= 8}.
+ * Pair i scores query pair_query[i] (row of q32) against every row of its list (list_rows, list-major fp32, rows
+ * [list_offsets[l], list_offsets[l+1])) with the canonical score and writes the key (ordered score << 32 | ~id) of row r of the
+ * list to keys[pair_out[i] + r]. */
+int vdk_ivf_flat_scan(const float* q32, int dim, const int32_t* items, int64_t n_items, const int32_t* pair_query,
+                      const int64_t* pair_out, const int64_t* list_offsets, const float* list_rows, const int64_t* list_ids,
+                      void* keys, void* stream);
+/* IVF-PQ list scan, one CTA per query: for probe p of query q (list probe_lists[q][p], coarse score probe_scores[q][p]) the key
+ * of row r of the list, score s = coarse; s = fl32(s + lut[q][m][code_m]) for m = 0..M-1, goes to keys[pair_out[q][p] + r]. */
+int vdk_ivf_pq_scan(int64_t n_query, int nprobe, const int64_t* probe_lists, const float* probe_scores, const int64_t* pair_out,
+                    const int64_t* list_offsets, const uint8_t* codes, int M, const int64_t* list_ids, const float* lut, void* keys,
+                    void* stream);
+/* Exact top-k of each query's keys keys[offsets[q] .. offsets[q] + counts[q]) (unique 64-bit keys as written by the scans)
+ * -> (score desc, id asc), padded with (-FLT_MAX, -1); the selection of vdk_ip_topk_exhaustive. */
+int vdk_topk_select_keys(const void* keys, const int64_t* offsets, const int64_t* counts, int64_t n_query, int k, float* out_scores,
+                         int64_t* out_ids, void* stream);
+
 /* ---- eval-time image preprocessing (SURVEY.md §8f-3: the GPU input pipeline) ------------------------------------------ */
 /* Replaces, for a BATCH of decoded RGB images of different sizes, the `val.augment` list of configs/faceX/{face,cbir}.yaml:
  * ResizeAndPadding2Square(size, training=False) (dataset/transforms.py:325-365: PIL Image.resize(BILINEAR) of the longer side

@@ -243,6 +243,12 @@ SIGNATURES = {
     "vdk_ip_exact_pairs": (_i, [_p, _p, _i, _p, _p, _i64, _p, _p]),
     "vdk_ip_topk_exhaustive_workspace_bytes": (_sz, [_i64]),
     "vdk_ip_topk_exhaustive": (_i, [_p, _i64, _p, _i64, _i, _i, _i64, _p, _p, _p, _sz, _p]),
+    "vdk_kmeans_update": (_i, [_p, _i64, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "vdk_pq_encode": (_i, [_p, _i64, _i, _p, _p, _i, _p, _p, _p, _p]),
+    "vdk_pq_lut": (_i, [_p, _i64, _i, _i, _p, _p, _p]),
+    "vdk_ivf_flat_scan": (_i, [_p, _i, _p, _i64, _p, _p, _p, _p, _p, _p, _p]),
+    "vdk_ivf_pq_scan": (_i, [_i64, _i, _p, _p, _p, _p, _p, _i, _p, _p, _p, _p]),
+    "vdk_topk_select_keys": (_i, [_p, _p, _p, _i64, _i, _p, _p, _p]),
 }
 
 _lib = None

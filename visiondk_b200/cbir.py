@@ -6,7 +6,7 @@ Mirrors, by name and argument meaning:
   search(...)                     engine/cbir/evaluation.py:171-200   (cbir_eval.py:98-122)
 with the arithmetic on the sm_90a kernels: the backbone's `embed()` fuses F.normalize into the neck epilogue,
 embeddings stay in HBM between extraction and search (the reference copies every batch to the host,
-face_model.py:140), and the faiss objects are replaced by visiondk_b200.retrieval.FlatIPIndex.
+face_model.py:140), and the faiss objects are replaced by visiondk_b200.retrieval.FlatIPIndex and visiondk_b200.ivf.IVFIndex.
 """
 from __future__ import annotations
 
@@ -16,6 +16,7 @@ from typing import Optional
 import numpy as np
 import torch
 
+from .ivf import index_factory as make_index, parse_index_factory
 from .retrieval import FlatIPIndex
 
 
@@ -143,13 +144,16 @@ def memmap_shard(path: str, feat_dim: int, dtype=np.float16, rank: int = 0, worl
 
 def index(extractor: FeatureExtractor, gallery_dataloader, device, logger=None, index_factory: str = "Flat",
           memmap_feat_dim: Optional[int] = None, memmap_dtype=np.float16, memmap_save_path: Optional[str] = None,
-          memmap_load_embedding: bool = False, shard: Optional[tuple] = None) -> FlatIPIndex:
-    """engine/cbir/evaluation.py:106-169: encode the gallery, build the flat inner-product index (resident on
-    `device`), optionally save / load the embeddings as a raw np.memmap (:124-152).
+          memmap_load_embedding: bool = False, shard: Optional[tuple] = None):
+    """engine/cbir/evaluation.py:106-169: encode the gallery, build the inner-product index named by `index_factory`
+    ("Flat" -> FlatIPIndex, "IVF<nlist>,Flat" / "IVF<nlist>,PQ<M>[x8]" -> visiondk_b200.ivf.IVFIndex; resident on `device`),
+    optionally save / load the embeddings as a raw np.memmap (:124-152).  An IVF index trains on the sampled rows of a loaded
+    store and adds it chunk by chunk, so the store is never uploaded whole.
     shard=(rank, world) with memmap_load_embedding: this rank loads only ITS rows of the store and the index carries their
     global ids (`id_offset`) — the per-rank index visiondk_b200.retrieval.sharded_flat_search expects (BASELINE config 4)."""
-    if index_factory != "Flat":
-        raise ValueError("only the 'Flat' (exact inner product) index of the reference's CBIR path is built")
+    flat = parse_index_factory(index_factory) is None  # refuses unknown strings before anything runs
+    if shard is not None and not flat:
+        raise ValueError(f"shard=(rank, world) builds per-rank Flat indexes; index_factory {index_factory!r} is not sharded")
     device = torch.device(device)
     id_offset = 0
     if shard is not None and not memmap_load_embedding:
@@ -159,7 +163,8 @@ def index(extractor: FeatureExtractor, gallery_dataloader, device, logger=None, 
             emb, id_offset, _ = memmap_shard(memmap_save_path, memmap_feat_dim, memmap_dtype, shard[0], shard[1])
         else:
             emb = np.memmap(memmap_save_path, mode="r", dtype=memmap_dtype).reshape(-1, memmap_feat_dim)
-        emb = torch.from_numpy(np.ascontiguousarray(emb, dtype=np.float32)).to(device)
+        if flat:
+            emb = torch.from_numpy(np.ascontiguousarray(emb, dtype=np.float32)).to(device)
     else:
         emb = extractor.extract_cbir_device(gallery_dataloader, device)
         if memmap_save_path is not None:
@@ -169,7 +174,7 @@ def index(extractor: FeatureExtractor, gallery_dataloader, device, logger=None, 
             mm = np.memmap(memmap_save_path, shape=host.shape, mode="w+", dtype=host.dtype)
             mm[:] = host
             mm.flush()
-    faiss_index = FlatIPIndex(emb.shape[-1], device, id_offset=id_offset)
+    faiss_index = make_index(emb.shape[-1], index_factory, device, id_offset=id_offset)
     if logger is not None:
         logger.console("Adding embeddings...")
     faiss_index.train(emb)
@@ -177,7 +182,7 @@ def index(extractor: FeatureExtractor, gallery_dataloader, device, logger=None, 
     return faiss_index
 
 
-def search(extractor: FeatureExtractor, query_dataloader, faiss_index: FlatIPIndex, device, logger=None, k: int = 100,
+def search(extractor: FeatureExtractor, query_dataloader, faiss_index, device, logger=None, k: int = 100,
            batch_size: int = 256):
     """engine/cbir/evaluation.py:171-200.  The reference searches in `batch_size` slices because faiss wants host
     arrays per call; here the whole query block is scored in one pass (each gallery tile is read once for all

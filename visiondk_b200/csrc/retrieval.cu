@@ -17,31 +17,12 @@
 // The gallery is scanned in geometrically growing ranges so that tau is tight when most of it streams by.
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
+#include "topk_keys.cuh"  // canonical arithmetic (restated in oracle/retrieval.py; the two must agree bit for bit)
 
 #include <cfloat>
 #include <cmath>
 
 namespace vdk {
-
-// ------------------------------------------------------------------------------------------------
-// canonical arithmetic (restated in oracle/retrieval.py; the two must agree bit for bit)
-// ------------------------------------------------------------------------------------------------
-// Fixed-order fp64 dot: lane l accumulates elements l, l+32, ... in order, then a 16/8/4/2/1 xor butterfly.
-// Products of two fp32 values are exact in fp64, so fma(a,b,acc) and acc + a*b round identically.
-__device__ __forceinline__ double warp_sum_f64(double v) {
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-  return v;
-}
-
-__device__ __forceinline__ uint32_t ord_u32(float f) {  // order-preserving float -> uint32
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float unord_u32(uint32_t o) {
-  const uint32_t u = (o & 0x80000000u) ? (o & 0x7fffffffu) : ~o;
-  return __uint_as_float(u);
-}
 
 // ------------------------------------------------------------------------------------------------
 // rows_prepare: one warp per row
@@ -825,8 +806,6 @@ __global__ void exact_pairs_kernel(const float* __restrict__ q32, const float* _
 // this one.  No approximate pass, no capacity: key = (ordered canonical score, ~row), unique per row, so the k-th
 // largest key is found exactly by an 8 x 8-bit radix select and the k survivors are sorted.
 // ------------------------------------------------------------------------------------------------
-constexpr int kExQ = 8;  // queries scored per pass over the gallery
-
 __global__ void __launch_bounds__(256) exhaustive_scores_kernel(const float* __restrict__ q32, int nq, const float* __restrict__ g32,
                                                                 int64_t ng, int dim, unsigned long long* __restrict__ keys) {
   extern __shared__ float ex_q[];  // [nq][dim]
@@ -835,105 +814,19 @@ __global__ void __launch_bounds__(256) exhaustive_scores_kernel(const float* __r
   const int lane = threadIdx.x & 31;
   const int64_t warps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
   for (int64_t row = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; row < ng; row += warps) {
-    const float* g = g32 + row * dim;
-    double acc[kExQ];
+    float s[kExQ];
+    canonical_scores_x8(ex_q, nq, g32 + row * dim, dim, lane, s);
 #pragma unroll
-    for (int j = 0; j < kExQ; ++j) acc[j] = 0.0;
-    for (int i = lane; i < dim; i += 32) {  // the canonical order: lane l takes l, l+32, ... then the xor butterfly
-      const double gv = static_cast<double>(g[i]);
-#pragma unroll
-      for (int j = 0; j < kExQ; ++j)
-        if (j < nq) acc[j] = fma(static_cast<double>(ex_q[j * dim + i]), gv, acc[j]);
-    }
-#pragma unroll
-    for (int j = 0; j < kExQ; ++j) {
-      if (j < nq) {
-        const double s = warp_sum_f64(acc[j]);
-        if (lane == 0)
-          keys[static_cast<size_t>(j) * ng + row] = (static_cast<unsigned long long>(ord_u32(static_cast<float>(s))) << 32) |
-                                                    static_cast<unsigned long long>(~static_cast<uint32_t>(row));
-      }
-    }
+    for (int j = 0; j < kExQ; ++j)
+      if (j < nq && lane == 0) keys[static_cast<size_t>(j) * ng + row] = score_key(s[j], static_cast<uint32_t>(row));
   }
 }
-
-constexpr int kExThreads = 1024;
 
 __global__ void __launch_bounds__(kExThreads) exhaustive_select_kernel(const unsigned long long* __restrict__ keys, int64_t ng, int k,
                                                                        int64_t id_offset, float* __restrict__ out_scores,
                                                                        int64_t* __restrict__ out_ids) {
-  __shared__ unsigned hist[256];
-  __shared__ unsigned long long s_sort[1024];
-  __shared__ unsigned s_bin, s_krem, s_m;
-  const int tid = threadIdx.x;
-  const unsigned long long* e = keys + static_cast<size_t>(blockIdx.x) * ng;
-  const int kk = static_cast<int>(ng < k ? ng : k);
-  unsigned long long prefix = 0ull, mask = 0ull;
-  unsigned k_rem = static_cast<unsigned>(kk);
-  if (kk > 0 && ng > kk) {
-    for (int shift = 56; shift >= 0; shift -= 8) {
-      for (int i = tid; i < 256; i += kExThreads) hist[i] = 0;
-      __syncthreads();
-      for (int64_t i = tid; i < ng; i += kExThreads) {
-        const unsigned long long key = e[i];
-        if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255ull], 1u);
-      }
-      __syncthreads();
-      if (tid == 0) {
-        unsigned acc = 0;
-        int b = 255;
-        for (; b > 0; --b) {
-          if (acc + hist[b] >= k_rem) break;
-          acc += hist[b];
-        }
-        s_bin = static_cast<unsigned>(b);
-        s_krem = k_rem - acc;
-      }
-      __syncthreads();
-      prefix |= static_cast<unsigned long long>(s_bin) << shift;
-      mask |= 255ull << shift;
-      k_rem = s_krem;
-      __syncthreads();
-    }
-  }
-  // keys are unique: exactly kk keys are >= the k-th largest (prefix); with ng <= k every key survives (prefix = 0)
-  if (tid == 0) s_m = 0;
-  for (int i = tid; i < 1024; i += kExThreads) s_sort[i] = 0ull;
-  __syncthreads();
-  for (int64_t i = tid; i < ng; i += kExThreads) {
-    const unsigned long long key = e[i];
-    if (key >= prefix) {
-      const unsigned pos = atomicAdd(&s_m, 1u);
-      if (pos < 1024u) s_sort[pos] = key;
-    }
-  }
-  __syncthreads();
-  for (int size = 2; size <= 1024; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int i = tid; i < 512; i += kExThreads) {
-        const int lo = 2 * i - (i & (stride - 1));
-        const int hi = lo + stride;
-        const bool desc = ((lo & size) == 0);
-        const unsigned long long a = s_sort[lo], b = s_sort[hi];
-        if ((a < b) == desc) {
-          s_sort[lo] = b;
-          s_sort[hi] = a;
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (int j = tid; j < k; j += kExThreads) {
-    float sc = -FLT_MAX;
-    int64_t id = -1;
-    if (j < kk) {
-      const unsigned long long key = s_sort[j];
-      sc = unord_u32(static_cast<uint32_t>(key >> 32));
-      id = static_cast<int64_t>(~static_cast<uint32_t>(key & 0xffffffffull)) + id_offset;
-    }
-    out_scores[static_cast<size_t>(blockIdx.x) * k + j] = sc;
-    out_ids[static_cast<size_t>(blockIdx.x) * k + j] = id;
-  }
+  select_topk_keys(keys + static_cast<size_t>(blockIdx.x) * ng, ng, k, id_offset, out_scores + static_cast<size_t>(blockIdx.x) * k,
+                   out_ids + static_cast<size_t>(blockIdx.x) * k);
 }
 
 static int pow2_ceil(int v) {
