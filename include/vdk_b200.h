@@ -828,7 +828,10 @@ size_t vdk_grad_sumsq_workspace_bytes(void);
 int vdk_grad_sumsq(const float* grads, int64_t n, double* total_sumsq, int accumulate, void* workspace,
                    size_t workspace_bytes, void* stream);
 /* One param group: g *= min(1, max_norm / (sqrt(total_sumsq) + 1e-6)); g += wd * p; buf = first_step ? g : mom*buf + g;
- * p -= lr * buf; ema = ema*d + (1-d)*p (ema may be NULL); g = 0 if zero_grad. */
+ * p -= lr * buf; ema = ema*d + (1-d)*p (ema may be NULL); g = 0 if zero_grad.  At momentum 0, buf = g and the momentum
+ * buffer is neither read nor written.  If total_sumsq is not finite the step is skipped (GradScaler.step): p and the momentum
+ * buffer are left as they are, while the EMA update and the zeroing of g still run.  A zero-initialised buffer with
+ * first_step = 0 gives first_step = 1's result up to the sign of a zero. */
 int vdk_sgd_clip_ema_step(float* params, float* grads, float* momentum_buf, float* ema, int64_t n,
                           const double* total_sumsq, float max_norm, float lr, float momentum, float weight_decay,
                           int first_step, float ema_decay, float ema_one_minus_decay, int zero_grad, void* stream);

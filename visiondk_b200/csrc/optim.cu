@@ -1,10 +1,13 @@
 // optim.cu — the optimizer half of the faceX train step as two HBM-bound sweeps over flat fp32 buffers.
 //
-// Replaces Trainer.update (engine/procedure/train.py:203-215): clip_grad_norm_(max_norm=10) -> SGD(momentum,
-// weight_decay) step (engine/optimizer.py:119-121 = torch.optim.SGD) -> optimizer.zero_grad() -> ModelEMA.update
-// (models/ema.py:28-37), which the reference runs as ~1400 small ATen launches per step (GradScaler is a no-op in
-// fp32).  Here: one reduction (sum of squared gradients, deterministic two-level order) and one fused update pass
-// that reads p, g, momentum, ema and writes p, momentum, ema, g(=0): 32 bytes per parameter.
+// Replaces Trainer.update (engine/procedure/train.py:203-215): GradScaler.unscale_ -> clip_grad_norm_(max_norm=10) ->
+// GradScaler.step(SGD(momentum, weight_decay)) (engine/optimizer.py:119-121 = torch.optim.SGD) -> optimizer.zero_grad() ->
+// ModelEMA.update (models/ema.py:28-37), which the reference runs as ~1400 small ATen launches per step.  The reference's
+// scaler is enabled on CUDA (engine/vision_engine.py:232,440): it scales the fp16-autocast loss and skips the SGD step when a
+// gradient is inf or NaN, while zero_grad and the EMA update still run.  This port trains in bf16 and does not scale the loss;
+// it keeps the skip: a step whose sum of squared gradients is not finite leaves parameters and momentum as they are.
+// Here: one reduction (sum of squared gradients, deterministic two-level order) and one fused update pass that reads p, g,
+// momentum, ema and writes p, momentum, ema, g(=0): 32 bytes per parameter.
 #include "vdk_host.h"
 
 #include <cuda_runtime.h>
@@ -65,19 +68,25 @@ struct StepArgs {
 };
 
 __global__ void __launch_bounds__(256) sgd_clip_ema_kernel(const StepArgs a) {
+  // GradScaler.step: a non-finite gradient anywhere skips the SGD step (p and momentum kept); EMA and zero_grad still run.
+  // The condition is uniform over the grid: every thread reads the same scalar.
+  const double sumsq = *a.total_sumsq;
+  const bool apply = isfinite(sumsq);
   // torch.nn.utils.clip_grad_norm_: coef = max_norm / (total_norm + 1e-6), clamped to 1
-  const float total_norm = static_cast<float>(sqrt(*a.total_sumsq));
+  const float total_norm = static_cast<float>(sqrt(sumsq));
   const float coef = fminf(a.max_norm / (total_norm + 1e-6f), 1.0f);
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < a.n;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     float p = a.p[i];
-    float g = a.g[i] * coef;
-    if (a.weight_decay != 0.f) g = fmaf(a.weight_decay, p, g);  // torch SGD: grad = grad + wd * param
-    float buf = a.first_step ? g : fmaf(a.momentum, a.mom[i], g);
-    if (a.momentum == 0.f) buf = g;
-    p = fmaf(-a.lr, buf, p);
-    a.p[i] = p;
-    a.mom[i] = buf;
+    if (apply) {
+      float g = a.g[i] * coef;
+      if (a.weight_decay != 0.f) g = fmaf(a.weight_decay, p, g);  // torch SGD: grad = grad + wd * param
+      float buf = a.first_step ? g : fmaf(a.momentum, a.mom[i], g);
+      if (a.momentum == 0.f) buf = g;
+      p = fmaf(-a.lr, buf, p);
+      a.p[i] = p;
+      if (a.momentum != 0.f) a.mom[i] = buf;  // torch SGD keeps no buffer at momentum 0: leave it as it is
+    }
     // ema.py:35-36: v *= d; v += (1-d) * msd[k]  (three separately rounded fp32 operations, as in the reference)
     if (a.ema) a.ema[i] = __fadd_rn(__fmul_rn(a.ema[i], a.ema_decay), __fmul_rn(a.ema_one_minus_decay, p));
     if (a.zero_grad) a.g[i] = 0.f;

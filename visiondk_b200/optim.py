@@ -94,7 +94,12 @@ class FusedSGDClipEMA:
 
     @torch.no_grad()
     def step(self) -> None:
-        """Everything Trainer.update does after backward (train.py:206-215)."""
+        """Everything Trainer.update does after backward (train.py:206-215).
+
+        A gradient that is not finite skips the SGD step on the device, as the reference's GradScaler.step does: parameters
+        and momentum stay as they are, the gradients are still zeroed and the EMA still moves (`updates` counts the step).
+        No host read decides it.  The momentum buffers start at zero and a skipped step leaves them there, so the first step
+        that applies computes momentum * 0 + d = d: torch's clone of the first update, up to the sign of a zero."""
         lib = _lib.load()
         s = _lib.stream_ptr()
         if self.sharded_groups:
@@ -113,7 +118,7 @@ class FusedSGDClipEMA:
                                                  g.ema.data_ptr() if g.ema is not None else 0, g.n,
                                                  self._sumsq.data_ptr(), self.max_norm, float(pg["lr"]),
                                                  float(pg["momentum"]), float(pg["weight_decay"]),
-                                                 int(self.steps == 0), d, omd, 1, s), "vdk_sgd_clip_ema_step")
+                                                 0, d, omd, 1, s), "vdk_sgd_clip_ema_step")
         for e, b in self._buffers:
             _lib.check(lib.vdk_ema_update(e.data_ptr(), b.data_ptr(), b.numel(), d, omd, s), "vdk_ema_update")
         self.steps += 1
