@@ -995,6 +995,33 @@ int vdk_ivf_pq_scan(int64_t n_query, int nprobe, const int64_t* probe_lists, con
 int vdk_topk_select_keys(const void* keys, const int64_t* offsets, const int64_t* counts, int64_t n_query, int k, float* out_scores,
                          int64_t* out_ids, void* stream);
 
+/* ---- DBSCAN, metric="cosine" (visiondk_b200/cluster.py, oracle/cluster.py, DESIGN §3c) ------------------------------------ */
+/* Replaces DBSCAN(eps, min_samples, metric="cosine").fit(X) of the reference's tools/clustering.py, label for label.
+ * Rows are the unit rows of vdk_rows_prepare (normalize = 1): x32 fp32 [n, dim], xh their fp16 copy, row_norm / row_err the
+ * per-row bounds, norm_max / err_max device scalars, their maxima (vdk_reduce_max).  j is a neighbour of i iff i == j or the
+ * canonical score s_ij >= threshold (the host derives the threshold from eps: the least fp32 score whose float32 cosine
+ * distance passes scikit-learn's test).  Outputs, device int32 [n]: counts = neighbours including the row itself (core iff
+ * >= min_samples), labels = cluster of every row (clusters numbered by ascending smallest core row; a border row takes the
+ * smallest label among its core neighbours; noise -1).  Three Gram passes (count, union, border) on fp16 tensor cores; pairs
+ * within the tensor-core error bound of the threshold are decided by the canonical fp64 score.  boundary_capacity (>= 32768,
+ * one tile) pairs are buffered per pass; a 128-row band whose boundary pairs do not fit is redone, so the result is always
+ * complete.  The call synchronises the stream.  dim a multiple of 64, <= 512; 1 <= n <= 2^25 - 4096 = 33 550 336 (the count pass launches
+ * ceil(n/128) * ceil(n/4096) CTAs, below 2^31). */
+typedef struct vdk_dbscan_stats {
+  int64_t n_core;
+  int64_t n_clusters;
+  int64_t rechecked_pairs;  /* pairs decided by the canonical fp64 score */
+  int64_t redone_bands;     /* 128-row bands redone after their boundary pairs overflowed the buffer (all three passes) */
+  float phase_ms[4];        /* count, union, border, finalise; CUDA events, filled when timing != 0 */
+  float gram_ms[3];         /* the Gram kernels alone of count, union, border */
+  float reserved;
+} vdk_dbscan_stats;
+size_t vdk_dbscan_workspace_bytes(int64_t n, int dim, int64_t boundary_capacity);
+int vdk_dbscan(const float* x32, const void* xh, const float* row_norm, const float* row_err, const float* norm_max,
+               const float* err_max, int64_t n, int dim, float threshold, int min_samples, int64_t boundary_capacity,
+               int32_t* labels, int32_t* counts, vdk_dbscan_stats* stats, int timing, void* workspace, size_t workspace_bytes,
+               void* stream);
+
 /* ---- eval-time image preprocessing (SURVEY.md §8f-3: the GPU input pipeline) ------------------------------------------ */
 /* Replaces, for a BATCH of decoded RGB images of different sizes, the `val.augment` list of configs/faceX/{face,cbir}.yaml:
  * ResizeAndPadding2Square(size, training=False) (dataset/transforms.py:325-365: PIL Image.resize(BILINEAR) of the longer side

@@ -46,6 +46,11 @@ class TopkPlan(C.Structure):
     ]
 
 
+class DbscanStats(C.Structure):
+    _fields_ = [("n_core", C.c_int64), ("n_clusters", C.c_int64), ("rechecked_pairs", C.c_int64), ("redone_bands", C.c_int64),
+                ("phase_ms", C.c_float * 4), ("gram_ms", C.c_float * 3), ("reserved", C.c_float)]
+
+
 _p, _i, _i64, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_size_t
 
 
@@ -249,6 +254,9 @@ SIGNATURES = {
     "vdk_ivf_flat_scan": (_i, [_p, _i, _p, _i64, _p, _p, _p, _p, _p, _p, _p]),
     "vdk_ivf_pq_scan": (_i, [_i64, _i, _p, _p, _p, _p, _p, _i, _p, _p, _p, _p]),
     "vdk_topk_select_keys": (_i, [_p, _p, _p, _i64, _i, _p, _p, _p]),
+    "vdk_dbscan_workspace_bytes": (_sz, [_i64, _i, _i64]),
+    "vdk_dbscan": (_i, [_p, _p, _p, _p, _p, _p, _i64, _i, C.c_float, _i, _i64, _p, _p, C.POINTER(DbscanStats), _i, _p, _sz,
+                        _p]),
 }
 
 _lib = None

@@ -17,6 +17,7 @@
 // The gallery is scanned in geometrically growing ranges so that tau is tight when most of it streams by.
 #include "vdk_host.h"
 #include "vdk_ptx.cuh"
+#include "score_tile.cuh"
 #include "topk_keys.cuh"  // canonical arithmetic (restated in oracle/retrieval.py; the two must agree bit for bit)
 
 #include <cfloat>
@@ -89,6 +90,9 @@ constexpr int kScoreThreads = 384;  // producer warpgroup, two consumer warpgrou
 constexpr int kStageLd = 64 + 1;  // fp32 pitch of the staged 128 x 64 score chunk (odd: conflict-free row reads)
 constexpr int kMaxKB = 8;         // dim <= 512
 constexpr int kMaxSeg = 32;       // candidate segments per query = 2 x gallery splits per range (two epilogue threads per row)
+static_assert(kQM == kTileM && kGN == kTileN && kSBK == kTileKB && kQBlockBytes == kTileABlockBytes &&
+                  kGStageBytes == kTileBStageBytes && kGStages == kTileStages && kStageLd == kTileStageLd,
+              "score_filter_kernel runs the mainloop of score_tile.cuh");
 
 struct ScoreParams {
   int n_query;
@@ -154,18 +158,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         for (int kb = 0; kb < p.num_kb; ++kb)
           tma_load_2d(smem_q + kb * kQBlockBytes, &map_q, q_full, kb * kSBK, qt * kQM, kEvictLast);
         uphase ^= 1;
-        for (int t = t0; t < t1; ++t) {
-          const int grow = static_cast<int>(p.g_lo) + t * kGN;
-          for (int kb = 0; kb < p.num_kb; ++kb) {
-            mbar_wait<true>(&empty_bar[stage], phase ^ 1);
-            mbar_arrive_expect_tx(&full_bar[stage], kGStageBytes);
-            tma_load_2d(smem_g + stage * kGStageBytes, &map_g, &full_bar[stage], kb * kSBK, grow, kEvictNormal);
-            if (++stage == kGStages) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-        }
+        tile_produce_b(smem_g, &map_g, full_bar, empty_bar, p.num_kb, static_cast<int>(p.g_lo), t0, t1, stage, phase);
       }
     }
   } else {
@@ -196,41 +189,12 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
       uint2* seg = p.seg + static_cast<size_t>(row_ok ? row : 0) * p.seg_stride + (kDense ? 0 : (sp * 2 + half) * p.seg_cap);
       unsigned cnt = 0;
       for (int t = t0; t < t1; ++t) {
-        int prev = -1;
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait<true>(&full_bar[stage], phase);
-          const uint64_t da = wgmma_desc_k_sw128(smem_u32(smem_q + kb * kQBlockBytes) + cg * 8192);
-          const uint64_t db = wgmma_desc_k_sw128(smem_u32(smem_g + stage * kGStageBytes));
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < kSBK / 16; ++k)
-            wgmma_m64n256k16_ss<false, 0, 0>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-          prev = stage;
-          if (++stage == kGStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        wgmma_wait<0>();
-        wgmma_fence_regs(acc);
-        if (lane == 0) {
-          mbar_arrive(&empty_bar[prev]);
-          if (t + 1 == t1) mbar_arrive(q_empty);  // every MMA of this unit has retired: the query tile may be overwritten
-        }
+        tile_mma(acc, smem_q, smem_g, full_bar, empty_bar, p.num_kb, cg, lane, stage, phase);
+        if (lane == 0 && t + 1 == t1) mbar_arrive(q_empty);  // every MMA of this unit has retired: the query tile may be overwritten
         const int64_t gbase = p.g_lo + static_cast<int64_t>(t) * kGN;
 #pragma unroll
         for (int cc = 0; cc < kGN / 64; ++cc) {
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int j = cc * 8 + jj;
-            stage_sm[frow * kStageLd + jj * 8 + fcol] = __float_as_uint(acc[4 * j]);
-            stage_sm[frow * kStageLd + jj * 8 + fcol + 1] = __float_as_uint(acc[4 * j + 1]);
-            stage_sm[(frow + 8) * kStageLd + jj * 8 + fcol] = __float_as_uint(acc[4 * j + 2]);
-            stage_sm[(frow + 8) * kStageLd + jj * 8 + fcol + 1] = __float_as_uint(acc[4 * j + 3]);
-          }
+          tile_stage_chunk(stage_sm, acc, cc, frow, fcol);
           named_bar_sync(1, 256);
           uint32_t r[32];
 #pragma unroll
